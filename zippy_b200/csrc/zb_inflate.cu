@@ -84,18 +84,27 @@ static_assert(sizeof(GroupSmem) % 16 == 0, "group tables must keep 16-byte align
 struct BitReader {
   const uint32_t *gbase;  // member start rounded down to 4 bytes
   uint32_t nwords;        // words that contain member bytes (beyond: zeros)
-  uint32_t cur, nxt;      // lane-held words of the line that holds word wi + 3, and of the next line
+  uint32_t last_mask;     // member bytes of word nwords - 1: the bytes after the member read as zero too
+  uint32_t cur, nxt;     // lane-held words of the line that holds word wi + 3, and of the next line
   uint32_t w0, w1, w2;    // words wi, wi + 1, wi + 2
   uint32_t wi;
   uint32_t bo;            // next unread bit inside w0 (0..31)
-  uint32_t over_word;     // a reader whose wi is beyond this is far past the end of the member
   uint64_t end_bit;       // absolute bit (from gbase) one past the member's last byte
   bool overrun;           // the reader is far past the end: whatever is being decoded is garbage
 };
 
+// Bits past the member's last byte read as zero, as in the reference's bit reader
+// (bitstreams.nim:22-48): a verdict that reads them (extra bits of a truncated token or repeat code) must
+// not depend on the bytes that follow the member in the batch buffer.
 __device__ __forceinline__ uint32_t br_word(const BitReader &b, uint32_t idx) {
-  return idx < b.nwords ? __ldcg(b.gbase + idx) : 0u;  // L2 only: every word is read once, and with a gated queue the
-                                                       // line may hold bytes of a member whose copy-in has not landed yet
+  if (idx >= b.nwords) return 0u;
+  const uint32_t v = __ldcg(b.gbase + idx);  // L2 only: every word is read once, and with a gated queue the
+                                             // line may hold bytes of a member whose copy-in has not landed yet
+  return idx + 1u == b.nwords ? v & b.last_mask : v;
+}
+__device__ __forceinline__ uint32_t br_tail_mask(uint64_t end_byte) {  // end_byte: one past the last byte, from gbase
+  const uint32_t r = (uint32_t)end_byte & 3u;
+  return r ? (1u << (8u * r)) - 1u : 0xffffffffu;
 }
 __device__ __forceinline__ uint32_t br_load_line(const BitReader &b, uint32_t line) {
   return br_word(b, line * (uint32_t)INF_G + (uint32_t)g_lane());
@@ -120,7 +129,7 @@ __device__ __forceinline__ void br_advance_line(BitReader &b) {
   b.nxt = br_load_line(b, (b.wi + 3u) / (uint32_t)INF_G + 1u);
   // bits past the end read as zero; a reader that is well past the end can only be decoding
   // garbage: flag it here so that no decode loop runs away (checked by the callers)
-  if (b.wi > b.over_word) b.overrun = true;
+  if (b.wi > (uint32_t)((b.end_bit + 64ull) >> 5)) b.overrun = true;
 }
 // Consume n bits.  LOCKSTEP: every lane of the warp executes the call together (the symbol
 // loop), so the shuffle can name the full warp; groups with n == 0 keep their state; n <= 32
@@ -294,7 +303,8 @@ __device__ __forceinline__ uint32_t decode_clc(BitReader &b, const GroupSmem *gs
 // (loads first, then stores: the sources cannot alias anything written here); matches that read
 // bytes produced inside the batch, and long ones, follow in stream order, each copied by the
 // whole group (reads only touch finished output: i % dist).
-// Returns 0, or 2 (invalid token) / 3 (out of room) for the first offending token in stream order,
+// Returns 0, or 2 (invalid token) / 3 (out of room) for the first offending token in stream order
+// (bad_back: how many bits before the token's end its end-of-input verdict is taken),
 // whose index is stored to bad_k; only the tokens before it are written and counted in op.
 #define INF_ROUNDS (32 / INF_G)
 #define INF_LONG_MATCH 24u
@@ -305,7 +315,8 @@ __device__ __forceinline__ uint32_t decode_clc(BitReader &b, const GroupSmem *gs
 template <bool COUNT_ONLY, typename OutT>
 __device__ __forceinline__ int flush_tokens(OutT *out, uint32_t &op, uint32_t cap, uint32_t win,
                                             const uint32_t (&ta)[INF_ROUNDS], const uint32_t (&tb)[INF_ROUNDS],
-                                            uint32_t ntok, uint32_t len_addr, uint32_t dist_addr, uint32_t &bad_k) {
+                                            uint32_t ntok, uint32_t len_addr, uint32_t dist_addr, uint32_t &bad_k,
+                                            uint32_t &bad_back) {
   const int lane = g_lane();
   const uint32_t gsel = INF_G == 32 ? 0xffffffffu : ((1u << INF_G) - 1u);
   const uint32_t batch_op = op;
@@ -348,6 +359,11 @@ __device__ __forceinline__ int flush_tokens(OutT *out, uint32_t &op, uint32_t ca
         n_ok = (uint32_t)(r * INF_G + j);
         ev = ((badm[r] >> j) & 1u) ? 2 : 3;
         total = g_shfl(rel[r], j);
+        // a distance symbol >= 30 is judged before the end of the input is (inflate.nim:212-213): the
+        // caller checks the end where the literal/length code ends, this many bits before the token's end
+        const uint32_t li = (ta[r] & 511u) - 257u;
+        const uint32_t back = (li < 29u && ((ta[r] >> 14) & 31u) >= 30u) ? (ta[r] >> 25) + (lds_u32(len_addr + li * 4u) >> 16) : 0u;
+        bad_back = g_shfl(back, j);
       }
     }
     bad_k = n_ok;
@@ -527,7 +543,10 @@ __device__ __forceinline__ int begin_block(Grp<OutT> &g, GroupSmem *gs) {
     uint32_t prev = 0;
     while (i != total) {
       uint32_t sym = decode_clc(b, gs);
-      if (b.overrun) return ZB_ERR_END_OF_BUFFER;
+      // inflate.nim:135-168 order: a symbol that ends past the input is the end of the buffer before
+      // anything else; the repeat count read after it is not checked until the next symbol (or the
+      // symbol loop), so a repeat that overshoots hlit + hdist first is an invalid header
+      if (br_past_end(b)) return ZB_ERR_END_OF_BUFFER;
       if (sym <= 15) {
         if (lane == 0) gs->lens[i] = (uint8_t)sym;
         prev = sym;
@@ -549,17 +568,18 @@ __device__ __forceinline__ int begin_block(Grp<OutT> &g, GroupSmem *gs) {
         i += rep;
         prev = 0;
       } else {
-        if (br_past_end(b)) return ZB_ERR_END_OF_BUFFER;
         return ZB_ERR_INVALID_SYMBOL;  // also the undecodable-code case (0xffff)
       }
       if (i > total) return ZB_ERR_UNCOMPRESS;
     }
-    if (br_past_end(b)) return ZB_ERR_END_OF_BUFFER;
     g_sync();
   }
   if (!build_tree<1>(gs->lens, hlit, gs->syms_ll, gs->lut_ll, LL_BITS, gs, 0)) return ZB_ERR_UNCOMPRESS;
   if (!build_tree<2>(gs->lens + hlit, hdist, gs->syms_d, gs->lut_d, D_BITS, gs, 1)) return ZB_ERR_UNCOMPRESS;
   g_sync();
+  // the last repeat count of a dynamic header may have run past the input: the reference builds the
+  // codes first (an over-subscribed set is an invalid header) and stops at the first symbol after
+  if (br_past_end(b)) return ZB_ERR_END_OF_BUFFER;
   return BLK_SYMS;
 }
 
@@ -649,20 +669,25 @@ __device__ __forceinline__ int symbol_loop(Grp<OutT> &g, const GroupSmem *gs, ui
         act = emit && !b.overrun;
       }
     }
-    uint32_t bad_k = 0;
+    uint32_t bad_k = 0, bad_back = 0;
     // only the counting and the marker kernels ever see a segment with a window in front of it
     const uint32_t win = (COUNT_ONLY || sizeof(OutT) == 2) ? g.win : 0u;
-    const int fev = flush_tokens<COUNT_ONLY, OutT>(g.out, op, g.cap, win, ta, tb, ntok, len_addr, dist_addr, bad_k);
+    const int fev = flush_tokens<COUNT_ONLY, OutT>(g.out, op, g.cap, win, ta, tb, ntok, len_addr, dist_addr, bad_k,
+                                                    bad_back);
     // a group that stopped: end of block (symbol 256), or a reader far past the end of its input
     ev = (act0 && !act) ? (b.overrun ? 100 + ZB_ERR_END_OF_BUFFER : 1) : 0;
     if (fev) {
-      // inflate.nim:190-191 order: a token that ran off the input reports the end of the buffer
+      // inflate.nim:190-225 order: a token that ran off the input reports the end of the buffer, but a
+      // length symbol >= 29 or a distance symbol >= 30 is invalid wherever the input ends, as long as the
+      // literal/length code itself was read in full: for those, the end is checked where that code ends
+      // (a length symbol >= 29 has no distance after it in the token; bad_back covers the distance case)
       uint32_t pk = 0;
 #pragma unroll
       for (int r = 0; r < INF_ROUNDS; r++) {
         const uint32_t v = g_shfl(tb[r], (int)(bad_k & (uint32_t)(INF_G - 1)));
         if ((bad_k / (uint32_t)INF_G) == (uint32_t)r) pk = v >> 13;
       }
+      pk -= bad_back;
       const uint64_t now_abs = br_consumed_abs(b);  // the token lies < 2^11 bits before this
       const bool past = now_abs - (uint64_t)(((uint32_t)now_abs - pk) & 0x7ffffu) > b.end_bit;
       ev = 100 + (past ? ZB_ERR_END_OF_BUFFER : (fev == 2 ? ZB_ERR_UNCOMPRESS : ZB_ERR_DST_TOO_SMALL));
@@ -701,7 +726,8 @@ __global__ void __launch_bounds__(INF_THREADS, INF_MIN_CTAS)
   g.ready_seen = 0;
   g.b.gbase = nullptr;
   g.b.nwords = 0;
-  g.b.cur = g.b.nxt = g.b.over_word = 0;
+  g.b.last_mask = 0;
+  g.b.cur = g.b.nxt = 0;
   g.b.w0 = g.b.w1 = g.b.w2 = g.b.wi = g.b.bo = 0;
   g.b.end_bit = 0;
   g.b.overrun = false;
@@ -758,8 +784,8 @@ __global__ void __launch_bounds__(INF_THREADS, INF_MIN_CTAS)
         g.shift0 = (uint32_t)((uintptr_t)g.src & 3u);
         g.b.gbase = reinterpret_cast<const uint32_t *>(g.src - g.shift0);
         g.b.nwords = (uint32_t)min((uint64_t)0xffffffffu, (g.shift0 + g.len + 3u) >> 2);
+        g.b.last_mask = ((g.shift0 + g.len + 3u) >> 2) > 0xffffffffull ? 0xffffffffu : br_tail_mask(g.shift0 + g.len);
         g.b.end_bit = g.shift0 * 8ull + (eb - byte0 * 8ull);
-        g.b.over_word = (uint32_t)((g.b.end_bit + 64ull) >> 5);
         g.b.overrun = false;
         br_seek(g.b, g.shift0, 0);
         br_skip<false>(g.b, (uint32_t)(sb & 7ull));
@@ -793,8 +819,8 @@ __global__ void __launch_bounds__(INF_THREADS, INF_MIN_CTAS)
           g.shift0 = (uint32_t)((uintptr_t)g.src & 3u);
           g.b.gbase = reinterpret_cast<const uint32_t *>(g.src - g.shift0);
           g.b.nwords = (uint32_t)((g.shift0 + g.len + 3u) >> 2);
+          g.b.last_mask = br_tail_mask(g.shift0 + g.len);
           g.b.end_bit = (g.shift0 + g.len) * 8ull;
-          g.b.over_word = (uint32_t)((g.b.end_bit + 64ull) >> 5);
           g.b.overrun = false;
           br_seek(g.b, g.shift0, pos);
           g.st = ST_BLOCK;
