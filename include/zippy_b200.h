@@ -134,6 +134,13 @@ int zb200_uncompress_sizes(zb200_ctx *ctx, const uint8_t *src_base, const uint64
 int zb200_uncompress_batch(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n,
                            int data_format, uint8_t *dst_base, const uint64_t *dst_offsets,
                            uint64_t *dst_lens, int *statuses);
+/* zb200_uncompress_batch(..., ZB200_DF_DEFLATE, ...) -- the same slots, statuses and outputs -- that also
+ * returns crcs[i], the CRC-32 of output i, wherever statuses[i] == 0 (0 elsewhere).  The CRC is computed on the
+ * device from the decoded bytes, in the pass that verifies gzip / zlib trailers; raw deflate has no trailer, so
+ * nothing is compared.  For containers that keep each entry's CRC-32 in their headers (ZIP). */
+int zb200_inflate_batch_crc32(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n,
+                              uint8_t *dst_base, const uint64_t *dst_offsets, uint64_t *dst_lens, uint32_t *crcs,
+                              int *statuses);
 /* crc32 (kind 0) or adler32 (kind 1) of every input */
 int zb200_checksum_batch(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n,
                          int kind, uint32_t *out);

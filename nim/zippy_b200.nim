@@ -213,3 +213,30 @@ proc compressBatch*(items: openArray[string], level = DefaultCompression,
                              outOffs[0].addr, nil)
   for i in 0 ..< items.len:
     result.add dst[outOffs[i].int ..< outOffs[i + 1].int]
+
+proc zb200_inflate_batch_crc32(ctx: Zb200Ctx, srcBase: pointer, srcOffsets: ptr uint64, n: csize_t,
+                               dstBase: pointer, dstOffsets: ptr uint64, dstLens: ptr uint64,
+                               crcs: ptr uint32, statuses: ptr cint): cint {.importc, cdecl, dynlib: lib.}
+
+proc inflateBatchCrc32*(items: openArray[string], sizes: openArray[int]): seq[(string, uint32)] {.raises: [ZippyError].} =
+  ## raw deflate members (a ZIP archive's entries) into slots of `sizes` bytes (its directory's uncompressed sizes)
+  ## -> every output with its CRC-32, computed on the device in the decode call (what ziparchives_v1.nim:202-212
+  ## does per entry with uncompress + crc32).  A member whose output does not fit its slot raises.
+  var
+    base: string
+    offs = newSeq[uint64](items.len + 1)
+    dofs = newSeq[uint64](items.len + 1)
+    lens = newSeq[uint64](max(items.len, 1))
+    crcs = newSeq[uint32](max(items.len, 1))
+    st = newSeq[cint](max(items.len, 1))
+  for i, item in items:
+    base.add item
+    offs[i + 1] = base.len.uint64
+    dofs[i + 1] = dofs[i] + sizes[i].uint64
+  var dst = newString(dofs[items.len].int + 64)
+  if base.len == 0: base.add '\0'
+  check zb200_inflate_batch_crc32(getCtx(), base[0].addr, offs[0].addr, items.len.csize_t, dst[0].addr,
+                                  dofs[0].addr, lens[0].addr, crcs[0].addr, st[0].addr)
+  for i in 0 ..< items.len:
+    check st[i]
+    result.add (dst[dofs[i].int ..< (dofs[i] + lens[i]).int], crcs[i])

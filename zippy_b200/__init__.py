@@ -151,28 +151,58 @@ class Context:
                                                   out.ctypes.data, dst_offs.ctypes.data, lens.ctypes.data,
                                                   st.ctypes.data))
         st = np.where(st0 != 0, st0, st[:n]).astype(np.int32)
-        out = out[:int(dst_offs[n])]
-        lens = lens[:n]
+        out, dst_offs = self._redo_too_small(base, offsets, dataFormat, out[:int(dst_offs[n])], dst_offs, lens[:n], st)
+        return out, dst_offs, lens[:n], st
+
+    def _redo_too_small(self, base, offsets, dataFormat, out, dst_offs, lens, st, crcs=None):
+        """A size claim (gzip ISIZE, a container's directory) understated the content (status 19): the reference
+        inflates anyway and lets its checksum / size checks decide (gzip.nim:80-88) -- redo those members one by
+        one.  lens / st / crcs are updated in place; -> (out, dst_offs) with the redone outputs appended."""
         small = np.nonzero(st == 19)[0]
-        if len(small):
-            # a size claim (gzip ISIZE, a container's directory) understated the content: the reference inflates
-            # anyway and lets its checksum / size checks decide (gzip.nim:80-88) -- redo those members one by one
-            extra = []
-            end = int(dst_offs[n])
-            dst_offs = dst_offs.copy()
-            for i in small:
-                try:
-                    b = self.decode_one(base[int(offsets[i]):int(offsets[i + 1])], dataFormat)
-                    st[i] = 0
-                    dst_offs[i] = end          # appended behind the slots; callers use out[off : off + len]
-                    lens[i] = len(b)
-                    end += len(b)
-                    extra.append(np.frombuffer(b, dtype=np.uint8))
-                except ZippyError as e:
-                    st[i] = e.code
-            if extra:
-                out = np.concatenate([out] + extra)
-        return out, dst_offs, lens, st
+        if not len(small):
+            return out, dst_offs
+        extra = []
+        end = int(dst_offs[-1])
+        dst_offs = dst_offs.copy()
+        for i in small:
+            try:
+                b = self.decode_one(base[int(offsets[i]):int(offsets[i + 1])], dataFormat)
+                st[i] = 0
+                dst_offs[i] = end          # appended behind the slots; callers use out[off : off + len]
+                lens[i] = len(b)
+                if crcs is not None:
+                    crcs[i] = self.crc32(b)
+                end += len(b)
+                extra.append(np.frombuffer(b, dtype=np.uint8))
+            except ZippyError as e:
+                st[i] = e.code
+        if extra:
+            out = np.concatenate([out] + extra)
+        return out, dst_offs
+
+    def inflate_batch_crc32(self, base, offsets, sizes):
+        """Raw deflate members into slots of `sizes` bytes (a ZIP directory's uncompressed sizes)
+        -> (out uint8 array, out_offsets uint64[n+1], out_lens uint64[n], crcs uint32[n], statuses int32[n]):
+        uncompress_batch(..., dfDeflate, sizes=sizes), plus the CRC-32 of every output that inflated, computed on
+        the device in the decode call (zb200_inflate_batch_crc32).  crcs[i] is 0 where statuses[i] != 0."""
+        L = _native.lib()
+        base = _as_u8(base)
+        offsets = np.ascontiguousarray(offsets, dtype=np.uint64)
+        n = len(offsets) - 1
+        comp_lens = offsets[1:] - offsets[:-1]
+        sizes = np.minimum(np.ascontiguousarray(sizes, dtype=np.uint64), comp_lens * np.uint64(1032) + np.uint64(1024))
+        dst_offs = np.zeros(n + 1, dtype=np.uint64)
+        np.cumsum(sizes, out=dst_offs[1:])
+        out = np.empty(int(dst_offs[n]) + 64, dtype=np.uint8)
+        lens = np.zeros(max(n, 1), dtype=np.uint64)
+        crcs = np.zeros(max(n, 1), dtype=np.uint32)
+        st = np.zeros(max(n, 1), dtype=np.int32)
+        _check(self._h, L.zb200_inflate_batch_crc32(self._h, base.ctypes.data, offsets.ctypes.data, n, out.ctypes.data,
+                                                     dst_offs.ctypes.data, lens.ctypes.data, crcs.ctypes.data,
+                                                     st.ctypes.data))
+        lens, crcs, st = lens[:n], crcs[:n], st[:n]
+        out, dst_offs = self._redo_too_small(base, offsets, dfDeflate, out[:int(dst_offs[n])], dst_offs, lens, st, crcs)
+        return out, dst_offs, lens, crcs, st
 
     def checksum_batch(self, base, offsets, kind="crc32"):
         L = _native.lib()

@@ -47,6 +47,8 @@ SYMBOLS = {
     "zb200_host_unregister": (c_int, [ctypes.c_void_p]),
     "zb200_uncompress_sizes": (c_int, [ctypes.c_void_p, c_u8p, c_u64p, c_size_t, c_int, c_u64p, c_intp]),
     "zb200_uncompress_batch": (c_int, [ctypes.c_void_p, c_u8p, c_u64p, c_size_t, c_int, c_u8p, c_u64p, c_u64p, c_intp]),
+    "zb200_inflate_batch_crc32": (c_int, [ctypes.c_void_p, c_u8p, c_u64p, c_size_t, c_u8p, c_u64p, c_u64p,
+                                          ctypes.c_void_p, c_intp]),
     "zb200_checksum_batch": (c_int, [ctypes.c_void_p, c_u8p, c_u64p, c_size_t, c_int, ctypes.c_void_p]),
     "zb200_compress_batch_device": (c_int, [ctypes.c_void_p, c_u8p, c_u64p, c_size_t, c_int, c_int, c_u8p, c_u8p,
                                             c_size_t, c_u64p, c_intp]),

@@ -1034,11 +1034,33 @@ bool longest_first_order(const uint64_t *src_offsets, size_t n, std::vector<uint
   return true;
 }
 
+// The checksum pass behind an inflate launch over w's outputs (the piece table is already in cw).  Without d_crcs it
+// verifies every gzip / zlib trailer, checksum then size (gzip.nim:80-88 / zippy.nim:154-162), and skips raw deflate.
+// With d_crcs it is the plain crc32 configuration instead (no kinds, no expected values): d_crcs[i] gets the CRC-32 of
+// every output that inflated, raw deflate included, and nothing is compared -- a ZIP entry's CRC lives in the
+// archive's headers, not behind the stream.
+void set_check_pass(ZbChecksumWork &cw, const ZbInflateWork &w, uint32_t *d_crcs) {
+  cw.src = w.dst;
+  cw.off = w.dst_off;
+  cw.lens = w.out_len;
+  cw.status = w.status;
+  if (d_crcs) {
+    cw.out = d_crcs;
+    cw.kind = 0;
+    return;
+  }
+  cw.expect = w.expect;
+  cw.kinds = w.kind;
+  cw.isize_src = w.src;
+  cw.isize_off = w.src_off;
+}
+
 // ---- uncompress, device-resident ----
+// crcs (host, may be null): the CRC-32 of every output that inflated, computed on the device (set_check_pass)
 int uncompress_device_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint64_t *src_offsets, size_t n,
                              int data_format, uint64_t raw_pos, uint8_t *d_dst, const uint64_t *dst_offsets,
                              uint64_t *dst_lens, int *statuses, bool count_only,
-                             const std::function<int()> *after_launch = nullptr) {
+                             const std::function<int()> *after_launch = nullptr, uint32_t *crcs = nullptr) {
   if (data_format < ZB200_DF_DETECT || data_format > ZB200_DF_DEFLATE) return ZB200_ERR_INVALID_FORMAT;
   if (n == 0) return ZB200_OK;
   ENSURE(ctx->src_off, (n + 1) * sizeof(uint64_t));
@@ -1048,6 +1070,7 @@ int uncompress_device_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint64_
   ENSURE(ctx->expect, n * sizeof(uint32_t));
   ENSURE(ctx->kind, n * sizeof(uint32_t));
   ENSURE(ctx->counter, 64);
+  if (crcs) ENSURE(ctx->ck_out, n * sizeof(uint32_t));
   cudaStream_t s = ctx->stream;
   CK(cudaMemcpyAsync(ctx->src_off.p, src_offsets, (n + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, s));
   if (!count_only)
@@ -1112,15 +1135,7 @@ int uncompress_device_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint64_
   CK(zb_launch_inflate(w, s));
   CK(cudaEventRecord(ctx->ev[1], s));
   if (!count_only) {
-    // gzip.nim:80-88 / zippy.nim:154-162: checksum, then size, of every member that inflated
-    cw.src = d_dst;
-    cw.off = (const uint64_t *)ctx->dst_off.p;
-    cw.lens = (const uint64_t *)ctx->out_len.p;
-    cw.status = (int *)ctx->status.p;
-    cw.expect = (const uint32_t *)ctx->expect.p;
-    cw.kinds = (const uint32_t *)ctx->kind.p;
-    cw.isize_src = d_src;
-    cw.isize_off = (const uint64_t *)ctx->src_off.p;
+    set_check_pass(cw, w, crcs ? (uint32_t *)ctx->ck_out.p : nullptr);
     CK(zb_launch_checksum(cw, s));
   }
   CK(cudaEventRecord(ctx->ev[2], s));
@@ -1136,12 +1151,16 @@ int uncompress_device_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint64_
     st = st_tmp.data();
   }
   CK(cudaMemcpyAsync(st, ctx->status.p, n * sizeof(int), cudaMemcpyDeviceToHost, s));
+  if (crcs && !count_only) CK(cudaMemcpyAsync(crcs, ctx->ck_out.p, n * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
   ctx->timing.inflate_ms += ev_ms(ctx->ev[0], ctx->ev[1]);
   ctx->timing.verify_ms += ev_ms(ctx->ev[1], ctx->ev[2]);
   ctx->timing.kernel_launches += count_only ? 1 : 3;
   for (size_t i = 0; i < n; i++)
-    if (st[i] != ZB200_OK) dst_lens[i] = 0;
+    if (st[i] != ZB200_OK) {
+      dst_lens[i] = 0;
+      if (crcs) crcs[i] = 0;
+    }
   return ZB200_OK;
 }
 
@@ -1155,7 +1174,7 @@ int uncompress_device_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint64_
 // host before it built and launched the next group, and each launch carried its own tail of long members.)
 int uncompress_host_pipelined(zb200_ctx *ctx, const uint8_t *h_src, const std::vector<uint64_t> &reb, size_t n,
                               int data_format, uint8_t *h_dst, const std::vector<uint64_t> &dreb, uint64_t *dst_lens,
-                              int *statuses, const std::vector<size_t> &gb) {
+                              int *statuses, const std::vector<size_t> &gb, uint32_t *crcs) {
   const size_t ng = gb.size() - 1;
   // gated: ONE inflate launch walks the whole batch behind the copy-in (no per-group launch tails), the D2H
   // stream waits on the per-group done counts; otherwise one launch per group, chained with events
@@ -1212,10 +1231,12 @@ int uncompress_host_pipelined(zb200_ctx *ctx, const uint8_t *h_src, const std::v
   ENSURE(ctx->ck_first, first.size() * sizeof(uint32_t));
   ENSURE(ctx->ck_piece_out, pieces.size() * sizeof(ZbChunkCheck));
   ENSURE(ctx->ck_partials, pieces.size() * (size_t)ZB_CK_PARTIAL_BYTES);
+  if (crcs) ENSURE(ctx->ck_out, n * sizeof(uint32_t));
+  uint32_t *d_crcs = crcs ? (uint32_t *)ctx->ck_out.p : nullptr;
   {
     int rc = ensure_group_events(ctx, 2 * ng + 2);
     if (rc) return rc;
-    rc = ensure_pinned(ctx, n * (sizeof(uint64_t) + sizeof(int)) + 64);
+    rc = ensure_pinned(ctx, n * (sizeof(uint64_t) + sizeof(int) + sizeof(uint32_t)) + 64);
     if (rc) return rc;
   }
   CK(cudaMemcpyAsync(ctx->src_off.p, reb.data(), (n + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, s));
@@ -1280,22 +1301,14 @@ int uncompress_host_pipelined(zb200_ctx *ctx, const uint8_t *h_src, const std::v
         if (armed) ctx->memops.write32((CUstream)ctx->h2d_stream, (CUdeviceptr)(uintptr_t)word, 0xffffffffu, 0);
       }
     } gate_release{ctx, d_gate, true};
-    // gzip.nim:80-88 / zippy.nim:154-162: checksum, then size, of every member that inflated (after the whole
-    // launch, under the last groups' copy-out)
+    // the checksum pass of every member that inflated (after the whole launch, under the last groups' copy-out)
     ZbChecksumWork cw;
     memset(&cw, 0, sizeof(cw));
-    cw.src = d_dst;
-    cw.off = w.dst_off;
-    cw.lens = w.out_len;
+    set_check_pass(cw, w, d_crcs);
     cw.pieces = (const ZbPiece *)ctx->ck_pieces.p;
     cw.first = (const uint32_t *)ctx->ck_first.p;
     cw.piece_out = (ZbChunkCheck *)ctx->ck_piece_out.p;
     cw.partials = (uint32_t *)ctx->ck_partials.p;
-    cw.status = w.status;
-    cw.expect = w.expect;
-    cw.kinds = w.kind;
-    cw.isize_src = d_src;
-    cw.isize_off = w.src_off;
     cw.tabs = ctx->d_tabs;
     cw.n = (uint32_t)n;
     cw.n_pieces = (uint32_t)pieces.size();
@@ -1376,21 +1389,14 @@ int uncompress_host_pipelined(zb200_ctx *ctx, const uint8_t *h_src, const std::v
     w.data_format = data_format;
     w.order = has_order[gi] ? (const uint32_t *)ctx->order.p + m0 : nullptr;
     CK(zb_launch_inflate(w, s));
-    // gzip.nim:80-88 / zippy.nim:154-162: checksum, then size, of every member that inflated
+    // the checksum pass of every member that inflated
     ZbChecksumWork cw;
     memset(&cw, 0, sizeof(cw));
-    cw.src = d_dst;
-    cw.off = w.dst_off;
-    cw.lens = w.out_len;
+    set_check_pass(cw, w, d_crcs ? d_crcs + m0 : nullptr);
     cw.pieces = (const ZbPiece *)ctx->ck_pieces.p + piece0[gi];
     cw.first = (const uint32_t *)ctx->ck_first.p + first0[gi];
     cw.piece_out = (ZbChunkCheck *)ctx->ck_piece_out.p + piece0[gi];
     cw.partials = (uint32_t *)ctx->ck_partials.p + piece0[gi] * (size_t)(ZB_CK_PARTIAL_BYTES / 4);
-    cw.status = w.status;
-    cw.expect = w.expect;
-    cw.kinds = w.kind;
-    cw.isize_src = d_src;
-    cw.isize_off = w.src_off;
     cw.tabs = ctx->d_tabs;
     cw.n = (uint32_t)nm;
     cw.n_pieces = (uint32_t)(piece0[gi + 1] - piece0[gi]);
@@ -1412,8 +1418,10 @@ int uncompress_host_pipelined(zb200_ctx *ctx, const uint8_t *h_src, const std::v
   }
   uint64_t *pl = (uint64_t *)ctx->pin;
   int *ps = (int *)(pl + n);
+  uint32_t *pc = (uint32_t *)(ps + n);
   CK(cudaMemcpyAsync(pl, ctx->out_len.p, n * sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
   CK(cudaMemcpyAsync(ps, ctx->status.p, n * sizeof(int), cudaMemcpyDeviceToHost, s));
+  if (crcs) CK(cudaMemcpyAsync(pc, d_crcs, n * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
   // the caller's stream ends after the last copy out
   CK(cudaEventRecord(ctx->gev[2 * ng + 1], sd));
   CK(cudaStreamWaitEvent(s, ctx->gev[2 * ng + 1], 0));
@@ -1422,6 +1430,7 @@ int uncompress_host_pipelined(zb200_ctx *ctx, const uint8_t *h_src, const std::v
   for (size_t i = 0; i < n; i++) {
     dst_lens[i] = ps[i] == ZB200_OK ? pl[i] : 0;
     if (statuses) statuses[i] = ps[i];
+    if (crcs) crcs[i] = ps[i] == ZB200_OK ? pc[i] : 0;
   }
   ctx->timing.inflate_ms = ev_ms(ctx->ev[0], ctx->ev[1]);  // inflate + verify of all groups (includes waits for copy-in)
   ctx->timing.verify_ms = 0.f;
@@ -1827,9 +1836,10 @@ int zb200_uncompress_sizes(zb200_ctx *ctx, const uint8_t *src_base, const uint64
   });
 }
 
-int zb200_uncompress_batch(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n,
-                           int data_format, uint8_t *dst_base, const uint64_t *dst_offsets, uint64_t *dst_lens,
-                           int *statuses) {
+// zb200_uncompress_batch, and with crcs (host, may be null) zb200_inflate_batch_crc32
+static int uncompress_batch_host(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n,
+                                 int data_format, uint8_t *dst_base, const uint64_t *dst_offsets, uint64_t *dst_lens,
+                                 int *statuses, uint32_t *crcs) {
   return guarded(ctx, [&]() -> int {
   if (!ctx || !src_offsets || !dst_offsets || !dst_lens || (n && !src_base)) return ZB200_ERR_ARG;
   std::lock_guard<std::mutex> lk(ctx->mu);
@@ -1887,7 +1897,7 @@ int zb200_uncompress_batch(zb200_ctx *ctx, const uint8_t *src_base, const uint64
     for (size_t i = 0; i < n && !any_big; i++) any_big = reb[i + 1] - reb[i] >= big_thr;
     if (!any_big) {
       int rc = uncompress_host_pipelined(ctx, src_base + slo, reb, n, data_format, dst_base ? dst_base + lo : nullptr, dreb,
-                                         dst_lens, statuses, gb);
+                                         dst_lens, statuses, gb, crcs);
       if (rc) return rc;
       ctx->timing.h2d_ms = ev_ms(ctx->ev[6], ctx->ev[7]);
       ctx->timing.d2h_ms = ev_ms(ctx->ev[8], ctx->ev[9]);
@@ -1932,7 +1942,7 @@ int zb200_uncompress_batch(zb200_ctx *ctx, const uint8_t *src_base, const uint64
     };
     rc = uncompress_device_locked(ctx, (const uint8_t *)ctx->in_stage.p, reb.data() + m0, m1 - m0, data_format, 0,
                                   (uint8_t *)ctx->out_stage.p, dreb.data() + m0, dst_lens + m0,
-                                  statuses ? statuses + m0 : nullptr, false, &copy_out);
+                                  statuses ? statuses + m0 : nullptr, false, &copy_out, crcs ? crcs + m0 : nullptr);
     if (rc) return rc;
   }
   CK(cudaEventRecord(ctx->ev[7], sh));
@@ -1948,6 +1958,21 @@ int zb200_uncompress_batch(zb200_ctx *ctx, const uint8_t *src_base, const uint64
   ctx->timing.d2h_bytes = hi - lo;
   return ZB200_OK;
   });
+}
+
+int zb200_uncompress_batch(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n,
+                           int data_format, uint8_t *dst_base, const uint64_t *dst_offsets, uint64_t *dst_lens,
+                           int *statuses) {
+  return uncompress_batch_host(ctx, src_base, src_offsets, n, data_format, dst_base, dst_offsets, dst_lens, statuses,
+                               nullptr);
+}
+
+int zb200_inflate_batch_crc32(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n,
+                              uint8_t *dst_base, const uint64_t *dst_offsets, uint64_t *dst_lens, uint32_t *crcs,
+                              int *statuses) {
+  if (!crcs) return ZB200_ERR_ARG;
+  return uncompress_batch_host(ctx, src_base, src_offsets, n, ZB200_DF_DEFLATE, dst_base, dst_offsets, dst_lens,
+                               statuses, crcs);
 }
 
 int zb200_checksum_batch_device(zb200_ctx *ctx, const uint8_t *d_src, const uint64_t *src_offsets, size_t n, int kind,
