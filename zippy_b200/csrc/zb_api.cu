@@ -12,6 +12,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <cmath>
 #include <condition_variable>
 #include <deque>
 #include <functional>
@@ -160,6 +161,7 @@ struct zb200_ctx {
   DevBuf in_stage, out_stage, lz2_tables;
   DevBuf seg_src, seg_dst, seg_len, seg_status, seg_kind, seg_expect, seg_cand, skip_mask;  // large-member segments
   DevBuf mark_scratch, mark_segs, seg_bits;  // speculative segments of a large member (uint16 symbols, descriptors)
+  DevBuf mark_win;          // window resolve scratch of the joint segments: group window maps (uint16) + incoming windows
   DevBuf order;             // work-queue order of an inflate launch (longest members first)
   DevBuf gate;              // gated inflate launch: [0] groups copied in, [1 .. ng] members done per group, then the group starts
   StreamMemOps memops;      // stream wait / write on device words (null: group-by-group launches instead)
@@ -172,6 +174,8 @@ struct zb200_ctx {
   uint64_t single_member_bytes = 512ull << 10; // threshold when the call holds ONE input.  (24 KiB was tried: alice29.txt.gz has three blocks,
                                                // two decode passes over three segments cost what one serial pass costs, so no gain)
   bool big_env = false;
+  bool joint_markers = true;       // env ZB200_JOINT_MARKERS=0 turns the marker segments at sync joints off (A/B timing)
+  uint32_t mark_window_segs = 8192;  // segments per window of the joint marker decode (env ZB200_MARK_WINDOW_SEGS)
   cudaEvent_t ev[10] = {};
   cudaStream_t h2d_stream = nullptr, d2h_stream = nullptr;
   std::vector<cudaEvent_t> gev;   // per-group events (H2D done, compute done, offsets ready)
@@ -839,7 +843,7 @@ int inflate_member_speculative(zb200_ctx *ctx, const uint8_t *d_src, uint64_t m0
   for (size_t i = 0; i < S; i++)
     if (sst[i] != ZB200_OK || sl[i] != want[i]) return ZB200_OK;
   // 4. markers -> bytes
-  CK(zb_launch_resolve((const uint16_t *)ctx->mark_scratch.p, ctx->mark_segs.p, (uint32_t)S, max_n, d_dst, d_bad, s));
+  CK(zb_launch_resolve((const uint16_t *)ctx->mark_scratch.p, ctx->mark_segs.p, (uint32_t)S, max_n, dst0, d_dst, d_bad, s));
   int bad = 0;
   CK(cudaMemcpyAsync(&bad, d_bad, 4, cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
@@ -847,6 +851,217 @@ int inflate_member_speculative(zb200_ctx *ctx, const uint8_t *d_src, uint64_t m0
   if (bad) return ZB200_OK;
   ok = true;
   out_len = total;
+  return ZB200_OK;
+}
+
+// ---- a large member cut at its sync joints, whose pieces refer back across them ----
+// This library's levels -1 and 2..9 stage every 64 KiB chunk with the member's previous 32 KiB, so its matches
+// reach back across the 00 00 ff ff joints and the pieces between them are not independent.  The joints are
+// still exact block boundaries: every segment is decoded from its joint (bit-exact seg_bits) straight into
+// uint16 symbols, with marker symbols for the unknown 32 KiB in front of it, and the markers are resolved.
+// Sizes: first the 64 KiB-per-segment guess (what this library's chunks produce) with no count pass; if a
+// segment disagrees, a count pass in marker mode.  A count pass whose segments on both sides of a joint fail
+// drops that joint (a 00 00 ff ff inside stored data or inside Huffman bits) and counts again, at most twice.
+// The member is processed in windows of segments (ctx->mark_window_segs, and about as much output as that many
+// full chunks): every window starts from the resolved output in front of it, so the scratch depends on the
+// window, not on the member.  Anything irregular leaves the member to the speculative and serial paths.
+// bounds: absolute byte offsets of the S + 1 segment boundaries in d_src.
+int inflate_member_joints(zb200_ctx *ctx, const uint8_t *d_src, uint64_t limit_byte, std::vector<uint64_t> bounds,
+                          uint8_t *d_dst, uint64_t dst0, uint64_t mcap, bool count_only, bool guess, bool &ok,
+                          uint64_t &out_len, bool &too_small) {
+  ok = false;
+  too_small = false;
+  cudaStream_t s = ctx->stream;
+  ZbInflateWork w;
+  memset(&w, 0, sizeof(w));
+  w.src = d_src;
+  w.seg_limit = limit_byte;
+  w.tabs = ctx->d_tabs;
+  w.data_format = ZB200_DF_DEFLATE;
+  w.seg_mode = 1;
+  std::vector<uint64_t> sl, sb;
+  std::vector<int> sst;
+  std::vector<uint32_t> sk;
+  // one decode launch over segments [a, b): counting, or marker symbols into mark_scratch at seg_dst
+  auto run = [&](size_t a, size_t b, bool count) -> int {
+    const size_t nw = b - a;
+    sb.resize(2 * nw);
+    for (size_t i = 0; i < nw; i++) {
+      sb[2 * i] = bounds[a + i] * 8ull;
+      sb[2 * i + 1] = bounds[a + i + 1] * 8ull;
+    }
+    ENSURE(ctx->seg_bits, 2 * nw * 8);
+    ENSURE(ctx->seg_len, nw * 8);
+    ENSURE(ctx->seg_status, nw * 4);
+    ENSURE(ctx->seg_kind, nw * 4);
+    ENSURE(ctx->seg_expect, nw * 4);
+    ENSURE(ctx->counter, 64);
+    CK(cudaMemcpyAsync(ctx->seg_bits.p, sb.data(), 2 * nw * 8, cudaMemcpyHostToDevice, s));
+    w.seg_bits = (const uint64_t *)ctx->seg_bits.p;
+    w.dst = count ? nullptr : (uint8_t *)ctx->mark_scratch.p;
+    w.dst_off = (const uint64_t *)ctx->seg_dst.p;
+    w.out_len = (uint64_t *)ctx->seg_len.p;
+    w.status = (int *)ctx->seg_status.p;
+    w.expect = (uint32_t *)ctx->seg_expect.p;
+    w.kind = (uint32_t *)ctx->seg_kind.p;
+    w.counter = (uint32_t *)ctx->counter.p + 4;
+    w.n = (uint32_t)nw;
+    w.seg_win0 = a > 0;
+    w.count_only = count ? 1 : 0;
+    w.mark = count ? 0 : 1;
+    CK(zb_launch_inflate(w, s));
+    sl.resize(nw);
+    sst.resize(nw);
+    sk.resize(nw);
+    CK(cudaMemcpyAsync(sl.data(), ctx->seg_len.p, nw * 8, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(sst.data(), ctx->seg_status.p, nw * 4, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(sk.data(), ctx->seg_kind.p, nw * 4, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    return ZB200_OK;
+  };
+  // exact sizes of every segment, with the repair rounds; counted = false: give up on this path
+  std::vector<uint64_t> size;
+  bool counted = false;
+  auto count_all = [&]() -> int {
+    for (int round = 0;; round++) {
+      const size_t S = bounds.size() - 1;
+      int rc = run(0, S, true);
+      if (rc) return rc;
+      ctx->timing.kernel_launches += 1;
+      std::vector<char> fail(S);
+      bool any = false;
+      for (size_t i = 0; i < S; i++) {
+        fail[i] = sst[i] != ZB200_OK || (sk[i] != 0) != (i + 1 == S) || sl[i] > 0xf0000000ull;
+        any = any || fail[i];
+      }
+      std::vector<uint64_t> nb(1, bounds[0]);
+      if (any) {   // a false joint: both segments around it fail
+        for (size_t k = 1; k < S; k++)
+          if (!(fail[k - 1] && fail[k])) nb.push_back(bounds[k]);
+      } else {     // a segment that starts before output byte 32768 could reach before the stream: join it to segment 0
+        uint64_t p = sl[0];
+        for (size_t k = 1; k < S; k++) {
+          if (p >= 32768ull) nb.push_back(bounds[k]);
+          p += sl[k];
+        }
+      }
+      nb.push_back(bounds[S]);
+      if (nb.size() == bounds.size()) {
+        counted = !any;
+        size = sl;
+        return ZB200_OK;
+      }
+      if (round == 2) return ZB200_OK;
+      bounds.swap(nb);
+    }
+  };
+  if (count_only || !guess) {
+    int rc = count_all();
+    if (rc || !counted) return rc;
+    uint64_t total = 0;
+    for (uint64_t v : size) total += v;
+    if (count_only) {
+      ok = true;
+      out_len = total;
+      return ZB200_OK;
+    }
+    if (total > mcap) {   // the whole stream decodes, so the serial decode could only run out of room: say so now
+      too_small = true;
+      return ZB200_OK;
+    }
+  } else if ((uint64_t)(bounds.size() - 2) * ZB_CHUNK_BYTES >= mcap) {
+    return ZB200_OK;
+  }
+  const uint64_t W = ctx->mark_window_segs, win_elems = W * (32768ull + ZB_CHUNK_BYTES);
+  ENSURE(ctx->counter, 64);
+  int *d_bad = (int *)((uint32_t *)ctx->counter.p + 12);
+  CK(cudaMemsetAsync(d_bad, 0, 4, s));
+  std::vector<ZbMarkSegHost> segs;
+  std::vector<uint64_t> dof;
+  uint64_t dpos = dst0;
+  for (size_t a = 0; a < bounds.size() - 1;) {
+    const size_t S = bounds.size() - 1;
+    size_t b = a;
+    uint64_t el = 0;
+    while (b < S && b - a < W) {
+      const uint64_t e = 32768ull + (counted ? size[b] : ZB_CHUNK_BYTES);
+      if (b > a && el + e > win_elems) break;
+      el += e;
+      b++;
+    }
+    const size_t nw = b - a;
+    segs.resize(nw);
+    dof.resize(nw + 1);
+    uint64_t se = 0, dp = dpos;
+    uint32_t max_n = 0;
+    for (size_t i = 0; i < nw; i++) {
+      const uint64_t n = counted ? size[a + i] : ZB_CHUNK_BYTES;
+      se += 32768ull;
+      segs[i].scr = se;
+      segs[i].dst = dp;
+      segs[i].n = (uint32_t)n;
+      segs[i].pad = 0;
+      dof[i] = se;
+      se += n;
+      dp += n;
+      max_n = std::max<uint32_t>(max_n, (uint32_t)n);
+    }
+    dof[nw] = se;
+    ENSURE(ctx->mark_scratch, (size_t)se * 2 + 64);
+    ENSURE(ctx->mark_segs, nw * sizeof(ZbMarkSegHost) + 16);
+    ENSURE(ctx->seg_dst, (nw + 1) * 8);
+    CK(cudaMemcpyAsync(ctx->seg_dst.p, dof.data(), (nw + 1) * 8, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(ctx->mark_segs.p, segs.data(), nw * sizeof(ZbMarkSegHost), cudaMemcpyHostToDevice, s));
+    CK(zb_launch_mark_prefill((uint16_t *)ctx->mark_scratch.p, ctx->mark_segs.p, (uint32_t)nw, s));
+    int rc = run(a, b, false);
+    if (rc) return rc;
+    ctx->timing.kernel_launches += 2;
+    bool wok = true;
+    for (size_t i = 0; i < nw && wok; i++) {
+      const bool last = a + i + 1 == S;
+      wok = sst[i] == ZB200_OK && (sk[i] != 0) == last &&
+            (counted ? sl[i] == size[a + i] : (last ? sl[i] <= (uint64_t)ZB_CHUNK_BYTES : sl[i] == (uint64_t)ZB_CHUNK_BYTES));
+    }
+    if (!wok) {
+      if (counted) return ZB200_OK;
+      // the 64 KiB guess does not hold: exact sizes, then this window again.  (The windows before decoded as
+      // guessed, so their segments pass the count too and no joint before `a` is dropped.)
+      rc = count_all();
+      if (rc || !counted) return rc;
+      uint64_t total = 0;
+      for (uint64_t v : size) total += v;
+      if (total > mcap) {
+        too_small = true;
+        return ZB200_OK;
+      }
+      continue;
+    }
+    if (!counted && b == S) {   // the member's last segment: its size is known now
+      dp = segs[nw - 1].dst + sl[nw - 1];
+      if (dp - dst0 > mcap) {
+        too_small = true;
+        return ZB200_OK;
+      }
+      segs[nw - 1].n = (uint32_t)sl[nw - 1];
+      CK(cudaMemcpyAsync((ZbMarkSegHost *)ctx->mark_segs.p + (nw - 1), &segs[nw - 1], sizeof(ZbMarkSegHost),
+                         cudaMemcpyHostToDevice, s));
+    }
+    const uint32_t gsz = std::max<uint32_t>(1u, (uint32_t)std::ceil(std::sqrt((double)nw)));
+    const size_t ngroups = (nw + gsz - 1) / gsz;
+    ENSURE(ctx->mark_win, ngroups * 32768ull * 3);
+    CK(zb_launch_resolve_groups((uint16_t *)ctx->mark_scratch.p, ctx->mark_segs.p, (uint32_t)nw, max_n, gsz, dst0,
+                                dpos - dst0, (uint16_t *)ctx->mark_win.p, (uint8_t *)ctx->mark_win.p + ngroups * 65536ull,
+                                d_dst, d_bad, s));
+    ctx->timing.kernel_launches += 4;
+    dpos = dp;
+    a = b;
+  }
+  int bad = 0;
+  CK(cudaMemcpyAsync(&bad, d_bad, 4, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  if (bad) return ZB200_OK;
+  ok = true;
+  out_len = dpos - dst0;
   return ZB200_OK;
 }
 
@@ -958,6 +1173,33 @@ int inflate_big_members(zb200_ctx *ctx, const uint8_t *d_src, const uint64_t *sr
     const uint64_t dst0 = count_only ? 0 : dst_offsets[m], mcap = count_only ? ~0ull : dst_offsets[m + 1] - dst_offsets[m];
     bool ok = false;
     int rc;
+    // segments that refer back across their joints: marker segments (inflate_member_joints); 1 = not handled there
+    auto joints = [&](bool guess) -> int {
+      if (!ctx->joint_markers) return 1;
+      bool jok = false, small = false;
+      uint64_t jlen = 0;
+      std::vector<uint64_t> jb(bounds.begin(), bounds.begin() + S + 1);
+      int rc_ = inflate_member_joints(ctx, d_src, m0 + hw.end, jb, d_dst, dst0, mcap, count_only, guess, jok, jlen, small);
+      if (rc_) return -rc_;
+      if (!jok && !small) return 1;
+      BigResult r;
+      r.member = m;
+      r.out_len = jok ? jlen : 0;
+      r.kind = (uint32_t)hw.fmt;
+      r.expect = hw.expect;
+      r.status = small ? ZB200_ERR_DST_TOO_SMALL : ZB200_OK;
+      done.push_back(r);
+      return 0;
+    };
+#define ZB_TRY_JOINTS(guess)         \
+  {                                  \
+    int _jr = joints(guess);         \
+    if (_jr < 0) return -_jr;        \
+    if (_jr == 0) continue;          \
+    ZB_TRY_SPECULATIVE();            \
+  }
+    // a segment after the first that refers back across its joint fails on its own: no count pass can help
+    bool back_refs = false, guess = false;
     // 2. the optimistic pass: this library's own members have 64 KiB of output per segment (the
     // last one takes what is left); if every segment agrees, one pass was enough
     if (!count_only && (S - 1) * (uint64_t)ZB_CHUNK_BYTES < mcap) {
@@ -973,7 +1215,15 @@ int inflate_big_members(zb200_ctx *ctx, const uint8_t *d_src, const uint64_t *sr
       for (size_t j = 0; j < S && ok; j++)
         ok = sst[j] == ZB200_OK && (sk[j] != 0) == (j + 1 == S) && (j + 1 == S || sl[j] == (uint64_t)ZB_CHUNK_BYTES);
       if (ok) dof[S] = dof[S - 1] + sl[S - 1];
+      // the 64 KiB guess stays plausible for the marker segments while no segment is known to be larger or smaller
+      guess = true;
+      for (size_t j = 0; j < S; j++) {
+        back_refs = back_refs || (j > 0 && sst[j] == ZB200_ERR_UNCOMPRESS);   // (distance beyond the segment start)
+        if (j + 1 < S && ((sst[j] == ZB200_OK && sl[j] != (uint64_t)ZB_CHUNK_BYTES) || sst[j] == ZB200_ERR_DST_TOO_SMALL))
+          guess = false;
+      }
     }
+    if (!ok && back_refs && ctx->joint_markers) ZB_TRY_JOINTS(guess);
     if (!ok) {
       // 3. sizes from a count pass, then the real pass with every segment at its place
       w.count_only = 1;
@@ -987,7 +1237,8 @@ int inflate_big_members(zb200_ctx *ctx, const uint8_t *d_src, const uint64_t *sr
         ok = sst[j] == ZB200_OK && (sk[j] != 0) == (j + 1 == S);
         dof[j + 1] = dof[j] + sl[j];
       }
-      if (!ok || dof[S] - dst0 > mcap) ZB_TRY_SPECULATIVE();
+      if (!ok) ZB_TRY_JOINTS(false);
+      if (dof[S] - dst0 > mcap) ZB_TRY_SPECULATIVE();
       if (!count_only) {
         std::vector<uint64_t> want = sl;
         CK(cudaMemcpyAsync(ctx->seg_dst.p, dof.data(), (S + 1) * 8, cudaMemcpyHostToDevice, s));
@@ -1560,6 +1811,11 @@ int zb200_init(int device, zb200_ctx **out) {
       ctx->big_env = true;
     }
   }
+  if (const char *e = getenv("ZB200_JOINT_MARKERS")) ctx->joint_markers = atoi(e) != 0;  // test hook: 0 = no marker segments at joints
+  if (const char *e = getenv("ZB200_MARK_WINDOW_SEGS")) {  // test hook: small windows in the joint marker decode
+    long v = atol(e);
+    if (v > 0) ctx->mark_window_segs = (uint32_t)std::min<long>(v, 60000);
+  }
   ctx->memops = load_stream_memops();
   if (const char *e = getenv("ZB200_UNC_GATED")) ctx->gated_unc = atoi(e) != 0;  // test hook: 0 = one launch per group
   if (const char *e = getenv("ZB200_UNC_GROUP_BYTES")) {  // test hook: small pipelined groups in the host uncompress
@@ -1601,7 +1857,7 @@ void zb200_shutdown(zb200_ctx *ctx) {
                     &ctx->cb, &ctx->chunk_off, &ctx->member_off, &ctx->member_check, &ctx->member_isize,
                     &ctx->src_off, &ctx->dst_off, &ctx->out_len, &ctx->status, &ctx->expect, &ctx->kind,
                     &ctx->counter, &ctx->ck_out, &ctx->ck_pieces, &ctx->ck_first, &ctx->ck_piece_out, &ctx->ck_partials, &ctx->in_stage, &ctx->out_stage, &ctx->lz2_tables,
-                    &ctx->seg_src, &ctx->seg_dst, &ctx->seg_len, &ctx->seg_status, &ctx->seg_kind, &ctx->seg_expect, &ctx->seg_cand, &ctx->skip_mask, &ctx->order, &ctx->mark_scratch, &ctx->mark_segs, &ctx->seg_bits, &ctx->gate};
+                    &ctx->seg_src, &ctx->seg_dst, &ctx->seg_len, &ctx->seg_status, &ctx->seg_kind, &ctx->seg_expect, &ctx->seg_cand, &ctx->skip_mask, &ctx->order, &ctx->mark_scratch, &ctx->mark_segs, &ctx->seg_bits, &ctx->mark_win, &ctx->gate};
   for (DevBuf *b : bufs)
     if (b->p) cudaFree(b->p);
   if (ctx->d_tabs) cudaFree(ctx->d_tabs);

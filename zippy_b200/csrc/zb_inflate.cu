@@ -23,6 +23,7 @@
 
 #include "zb_device.cuh"
 #include "zb_kernels.h"
+#include "zb_resolve.h"
 #include "zb_wrapper.h"
 
 #ifndef INF_G
@@ -777,7 +778,7 @@ __global__ void __launch_bounds__(INF_THREADS, INF_MIN_CTAS)
         g.final_block = false;
         g.kind = ZB_DF_DEFLATE;
         g.expect = 0;
-        g.win = i == 0 ? 0u : 32768u;   // segment 0 starts the stream: it has no window
+        g.win = (i == 0 && !w.seg_win0) ? 0u : 32768u;   // segment 0 starts the stream: it has no window
         g.out = COUNT_ONLY ? nullptr : reinterpret_cast<OutT *>(w.dst) + w.dst_off[i];
         const uint64_t cap64 = COUNT_ONLY ? ~0ull : w.dst_off[i + 1] - w.dst_off[i];
         g.cap = (uint32_t)min(cap64, (uint64_t)0xfffffdffu - 32768u);
@@ -1554,24 +1555,114 @@ __global__ void __launch_bounds__(RT_THREADS, 1) k_resolve_tails(const uint16_t 
   }
 }
 
-__global__ void __launch_bounds__(256) k_resolve_rest(const uint16_t *scr, const ZbMarkSeg *segs, uint8_t *dst, int *bad) {
-  const ZbMarkSeg sg = segs[blockIdx.y];
-  const uint64_t p0 = sg.dst - segs[0].dst;   // member position of the segment's first byte
-  const uint32_t T = min(sg.n, 32768u), rest = sg.n - T;
-  for (uint32_t j = blockIdx.x * 2048u + threadIdx.x; j < min(rest, blockIdx.x * 2048u + 2048u); j += 256u) {
-    const uint32_t sy = scr[sg.scr + j];
-    uint8_t v = (uint8_t)sy;
-    if (sy >= 256u) {
-      const uint32_t k = sy & 0x7fffu;
-      if (p0 + k < 32768ull) {   // before the start of the stream: the member goes to the serial decode
-        *bad = 1;
-        v = 0;
-      } else {
-        v = dst[sg.dst - 32768ull + k];
+// base: dst offset of the member's first output byte (markers before it are the "distance too far back" error)
+__global__ void __launch_bounds__(256) k_resolve_rest(const uint16_t *scr, const ZbMarkSeg *segs, uint32_t nseg, uint32_t slabs,
+                                                      uint64_t base, uint8_t *dst, int *bad) {
+  for (uint64_t b = blockIdx.x; b < (uint64_t)nseg * slabs; b += gridDim.x) {
+    const ZbMarkSeg sg = segs[b / slabs];
+    const uint32_t x = (uint32_t)(b % slabs);
+    const uint64_t p0 = sg.dst - base;   // member position of the segment's first byte
+    const uint32_t T = min(sg.n, 32768u), rest = sg.n - T;
+    for (uint32_t j = x * 2048u + threadIdx.x; j < min(rest, x * 2048u + 2048u); j += 256u) {
+      const uint32_t sy = scr[sg.scr + j];
+      uint8_t v = (uint8_t)sy;
+      if (sy >= 256u) {
+        const uint32_t k = sy & 0x7fffu;
+        if (p0 + k < 32768ull) {   // before the start of the stream: the member goes to the serial decode
+          *bad = 1;
+          v = 0;
+        } else {
+          v = dst[sg.dst - 32768ull + k];
+        }
+      }
+      dst[sg.dst + j] = v;
+    }
+  }
+}
+
+// ---- the parallel window resolve (segments at this library's sync joints, zb_api.cu: inflate_member_joints) ----
+// The per-element rules and the three steps are described in zb_resolve.h.  The segments of one launch are a
+// window of a member; its groups are gsz consecutive segments each.
+// (A) one CTA per group: tails in place as "byte or marker into the group's incoming window", the group's
+//     outgoing window map to gmap[group].
+__global__ void __launch_bounds__(RT_THREADS, 1) k_resolve_groups(uint16_t *scr, const ZbMarkSeg *segs, uint32_t nseg,
+                                                                  uint32_t gsz, uint64_t base, uint16_t *gmap, int *bad) {
+  extern __shared__ uint16_t rring[];   // rring[zb_rs_slot(p)] = symbol at member position p
+  const uint32_t tid = threadIdx.x, s0 = blockIdx.x * gsz, s1 = min(nseg, s0 + gsz);
+  const uint64_t q0 = segs[s0].dst - base;
+  for (uint32_t k = tid; k < ZB_RS_WIN; k += RT_THREADS) rring[zb_rs_slot(q0 + k)] = zb_rs_incoming(k);
+  __syncthreads();
+  bool any_bad = false;
+  for (uint32_t i = s0; i < s1; i++) {
+    const ZbMarkSeg sg = segs[i];
+    const uint32_t T = min(sg.n, ZB_RS_WIN), j0 = sg.n - T;
+    const uint64_t p0 = sg.dst - base;
+    uint16_t *tail = scr + sg.scr + j0;
+    uint32_t val[RT_PER / 2];   // two symbols per register (no spills at 1024 threads)
+#pragma unroll
+    for (int r = 0; r < RT_PER; r++) {
+      const uint32_t k = tid + (uint32_t)r * RT_THREADS;
+      const uint32_t v = k < T ? zb_rs_ring_lookup(tail[k], p0, rring, any_bad) : 0u;
+      val[r / 2] = (r & 1) ? (val[r / 2] | (v << 16)) : v;
+    }
+    __syncthreads();   // every read of the old window is done before it is overwritten
+#pragma unroll
+    for (int r = 0; r < RT_PER; r++) {
+      const uint32_t k = tid + (uint32_t)r * RT_THREADS;
+      if (k < T) {
+        const uint16_t v = (uint16_t)((r & 1) ? (val[r / 2] >> 16) : val[r / 2]);
+        rring[zb_rs_slot(p0 + j0 + k)] = v;
+        tail[k] = v;
       }
     }
-    dst[sg.dst + j] = v;
+    __syncthreads();
   }
+  const uint64_t q1 = segs[s1 - 1].dst + segs[s1 - 1].n - base;   // one past the group's last position
+  for (uint32_t k = tid; k < ZB_RS_WIN; k += RT_THREADS) gmap[(uint64_t)blockIdx.x * ZB_RS_WIN + k] = rring[zb_rs_slot(q1 + k)];
+  if (any_bad) *bad = 1;
+}
+
+// (B) one CTA: the incoming window of every group, in order.  The window's own incoming window is the resolved
+// output in front of member position w0 (positions before the member start read as 0: markers there set bad in (A)).
+__global__ void __launch_bounds__(RT_THREADS, 1) k_resolve_compose(const uint16_t *gmap, uint32_t ngroups, const uint8_t *dst,
+                                                                   uint64_t base, uint64_t w0, uint8_t *gin) {
+  __shared__ uint8_t win[ZB_RS_WIN];
+  const uint32_t tid = threadIdx.x;
+  for (uint32_t k = tid; k < ZB_RS_WIN; k += RT_THREADS) win[k] = w0 + k >= ZB_RS_WIN ? dst[base + w0 + k - ZB_RS_WIN] : (uint8_t)0;
+  __syncthreads();
+  for (uint32_t g = 0; g < ngroups; g++) {
+    const uint16_t *m = gmap + (uint64_t)g * ZB_RS_WIN;
+    uint8_t *in = gin + (uint64_t)g * ZB_RS_WIN;
+    uint8_t v[RT_PER];
+#pragma unroll
+    for (int r = 0; r < RT_PER; r++) {
+      const uint32_t k = tid + (uint32_t)r * RT_THREADS;
+      in[k] = win[k];
+      v[r] = zb_rs_compose(m[k], win);
+    }
+    __syncthreads();
+#pragma unroll
+    for (int r = 0; r < RT_PER; r++) win[tid + (uint32_t)r * RT_THREADS] = v[r];
+    __syncthreads();
+  }
+}
+
+// (C) every tail symbol against its group's incoming window -> dst
+__global__ void __launch_bounds__(256) k_resolve_tails_par(const uint16_t *scr, const ZbMarkSeg *segs, uint32_t nseg,
+                                                           uint32_t gsz, const uint8_t *gin, uint8_t *dst) {
+  const uint64_t total = (uint64_t)nseg * ZB_RS_WIN, stride = (uint64_t)gridDim.x * blockDim.x;
+  for (uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += stride) {
+    const uint32_t i = (uint32_t)(t / ZB_RS_WIN), jt = (uint32_t)(t % ZB_RS_WIN);
+    const ZbMarkSeg sg = segs[i];
+    const uint32_t T = min(sg.n, ZB_RS_WIN);
+    if (jt >= T) continue;
+    const uint32_t j = sg.n - T + jt;
+    dst[sg.dst + j] = zb_rs_compose(scr[sg.scr + j], gin + (uint64_t)(i / gsz) * ZB_RS_WIN);
+  }
+}
+
+static uint32_t resolve_rest_grid(uint32_t nseg, uint32_t slabs) {
+  return (uint32_t)std::min<uint64_t>((uint64_t)nseg * slabs, 64ull * (uint64_t)zb_sm_count());
 }
 
 cudaError_t zb_launch_mark_prefill(uint16_t *scr, const void *segs, uint32_t nseg, cudaStream_t s) {
@@ -1579,12 +1670,26 @@ cudaError_t zb_launch_mark_prefill(uint16_t *scr, const void *segs, uint32_t nse
   k_mark_prefill<<<dim3(128, nseg), 256, 0, s>>>(scr, (const ZbMarkSeg *)segs);
   return cudaGetLastError();
 }
-cudaError_t zb_launch_resolve(const uint16_t *scr, const void *segs, uint32_t nseg, uint32_t max_n, uint8_t *dst, int *bad,
-                              cudaStream_t s) {
+cudaError_t zb_launch_resolve(const uint16_t *scr, const void *segs, uint32_t nseg, uint32_t max_n, uint64_t base, uint8_t *dst,
+                              int *bad, cudaStream_t s) {
   if (!nseg) return cudaSuccess;
   k_resolve_tails<<<1, RT_THREADS, 32768, s>>>(scr, (const ZbMarkSeg *)segs, nseg, dst, bad);
   const uint32_t slabs = (max_n + 2047u) / 2048u;
-  if (slabs) k_resolve_rest<<<dim3(slabs, nseg), 256, 0, s>>>(scr, (const ZbMarkSeg *)segs, dst, bad);
+  if (slabs) k_resolve_rest<<<resolve_rest_grid(nseg, slabs), 256, 0, s>>>(scr, (const ZbMarkSeg *)segs, nseg, slabs, base, dst, bad);
+  return cudaGetLastError();
+}
+
+cudaError_t zb_launch_resolve_groups(uint16_t *scr, const void *segs, uint32_t nseg, uint32_t max_n, uint32_t gsz, uint64_t base,
+                                     uint64_t w0, uint16_t *gmap, uint8_t *gin, uint8_t *dst, int *bad, cudaStream_t s) {
+  if (!nseg) return cudaSuccess;
+  const ZbMarkSeg *sg = (const ZbMarkSeg *)segs;
+  const uint32_t ngroups = (nseg + gsz - 1) / gsz;
+  k_resolve_groups<<<ngroups, RT_THREADS, ZB_RS_WIN * 2, s>>>(scr, sg, nseg, gsz, base, gmap, bad);
+  k_resolve_compose<<<1, RT_THREADS, 0, s>>>(gmap, ngroups, dst, base, w0, gin);
+  const uint32_t tgrid = (uint32_t)std::min<uint64_t>(((uint64_t)nseg * ZB_RS_WIN + 255) / 256, 64ull * (uint64_t)zb_sm_count());
+  k_resolve_tails_par<<<tgrid, 256, 0, s>>>(scr, sg, nseg, gsz, gin, dst);
+  const uint32_t slabs = (max_n + 2047u) / 2048u;
+  if (slabs) k_resolve_rest<<<resolve_rest_grid(nseg, slabs), 256, 0, s>>>(scr, sg, nseg, slabs, base, dst, bad);
   return cudaGetLastError();
 }
 
@@ -1607,6 +1712,7 @@ cudaError_t zb_setup_inflate_attrs() {
   if (e == cudaSuccess) e = cudaFuncSetAttribute(k_inflate<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(k_inflate<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(k_resolve_tails, cudaFuncAttributeMaxDynamicSharedMemorySize, 32768);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(k_resolve_groups, cudaFuncAttributeMaxDynamicSharedMemorySize, ZB_RS_WIN * 2);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(k_piece_checksum<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, CK_SM_TOTAL);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(k_piece_checksum<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, CK_SM_TOTAL_ADLER);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(k_piece_checksum<true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
@@ -1621,6 +1727,8 @@ cudaError_t zb_setup_inflate_attrs() {
   if (e == cudaSuccess) e = cudaFuncGetAttributes(&fa, k_find_blocks);
   if (e == cudaSuccess) e = cudaFuncGetAttributes(&fa, k_mark_prefill);
   if (e == cudaSuccess) e = cudaFuncGetAttributes(&fa, k_resolve_rest);
+  if (e == cudaSuccess) e = cudaFuncGetAttributes(&fa, k_resolve_compose);
+  if (e == cudaSuccess) e = cudaFuncGetAttributes(&fa, k_resolve_tails_par);
   return e;
 }
 

@@ -87,6 +87,8 @@ struct ZbInflateWork {
                                //   speculative segments found by zb_launch_find_blocks; segment i > 0 may reference
                                //   32768 bytes before its own start (its unknown window)
   uint64_t seg_limit;          // with seg_bits: byte offset in src where the stream's payload ends
+  int seg_win0;                // with seg_bits: segment 0 does not start the stream (a later window of a member):
+                               //   it may reference 32768 bytes before its start too
   int mark;                    // with seg_bits: dst holds uint16 elements (dst_off in elements), 32768 marker
                                //   symbols sit in front of every segment's output
   int seg_mode;                // members are independently decodable SEGMENTS of one raw deflate stream:
@@ -120,8 +122,14 @@ struct ZbMarkSegHost {
   uint32_t pad;
 };
 cudaError_t zb_launch_mark_prefill(uint16_t *scr, const void *segs, uint32_t nseg, cudaStream_t s);
-cudaError_t zb_launch_resolve(const uint16_t *scr, const void *segs, uint32_t nseg, uint32_t max_n, uint8_t *dst, int *bad,
-                              cudaStream_t s);
+// base: dst offset of the member's first output byte
+cudaError_t zb_launch_resolve(const uint16_t *scr, const void *segs, uint32_t nseg, uint32_t max_n, uint64_t base, uint8_t *dst,
+                              int *bad, cudaStream_t s);
+// The parallel window resolve (zb_resolve.h): the segments are one window of a member, in groups of gsz; w0 is the
+// member position of the window's first byte (the resolved output in front of it is in dst already).  Scratch:
+// gmap [ceil(nseg / gsz) x 32768] uint16, gin the same count of bytes.  Rewrites the tails in scr.
+cudaError_t zb_launch_resolve_groups(uint16_t *scr, const void *segs, uint32_t nseg, uint32_t max_n, uint32_t gsz, uint64_t base,
+                                     uint64_t w0, uint16_t *gmap, uint8_t *gin, uint8_t *dst, int *bad, cudaStream_t s);
 
 // ---- checksums over a batch of buffers (standalone crc32/adler32, and the trailer
 // verification after inflate) ----
