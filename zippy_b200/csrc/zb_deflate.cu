@@ -180,7 +180,43 @@ __device__ __forceinline__ void lz_batch_pass(const uint8_t *wdata, bool active,
   }
 }
 
-template <int MODE>  // 1: single-probe hash matcher (level 1); 0: literals only (levels 0, -2)
+// -DZB_LZ1_STAGE_CLOCKS=1 (a diagnostic build, never the shipped one; tools/lz1_stages.py makes it): lane 0 of every
+// warp of k_lz<1> adds the clock64() cycles of each stage of the parse into zb_lz1_stage_clk, read back (and
+// zeroed) by zb200_lz1_stage_clocks.  The stage order is the one LZ1_STAGE_NAMES in that tool prints.
+#ifndef ZB_LZ1_STAGE_CLOCKS
+#define ZB_LZ1_STAGE_CLOCKS 0
+#endif
+enum { LZS_WAIT, LZS_CHECKSUM, LZS_SEED, LZS_PROBE, LZS_EXTEND, LZS_SELECT, LZS_BATCH, LZS_BARRIER, LZS_N };
+#if ZB_LZ1_STAGE_CLOCKS
+__device__ unsigned long long zb_lz1_stage_clk[LZS_N];
+#define LZ_CLK_DECL                          \
+  unsigned long long clk_acc[LZS_N] = {};    \
+  long long clk_t = clock64();
+#define LZ_CLK(s)                            \
+  if (MODE == 1) {                           \
+    const long long clk_n = clock64();       \
+    clk_acc[s] += (unsigned long long)(clk_n - clk_t); \
+    clk_t = clk_n;                           \
+  }
+#define LZ_CLK_PUBLISH()                                                                           \
+  if (MODE == 1 && lane == 0) {                                                                    \
+    _Pragma("unroll") for (int s_ = 0; s_ < LZS_N; s_++) atomicAdd(&zb_lz1_stage_clk[s_], clk_acc[s_]); \
+  }
+extern "C" int zb200_lz1_stage_clocks(unsigned long long *out) {
+  unsigned long long zero[LZS_N] = {};
+  if (cudaMemcpyFromSymbol(out, zb_lz1_stage_clk, sizeof(zero)) != cudaSuccess) return -1;
+  return cudaMemcpyToSymbol(zb_lz1_stage_clk, zero, sizeof(zero)) == cudaSuccess ? 0 : -1;
+}
+#else
+#define LZ_CLK_DECL
+#define LZ_CLK(s)
+#define LZ_CLK_PUBLISH()
+#endif
+
+// MODE 1: single-probe hash matcher (level 1); 0: literals only (levels 0, -2).
+// CK: the chunk checksums k_member_check reads for the batch's format (ZB_CK_CRC for gzip, ZB_CK_ADLER for
+// zlib, 0 for raw DEFLATE); the other fields of chk are left 0.
+template <int MODE, int CK>
 __global__ void __launch_bounds__(LZ_THREADS, 3)
     k_lz(const uint8_t *__restrict__ src, const ZbChunkDesc *__restrict__ desc, uint2 *__restrict__ masks,
          uint32_t *__restrict__ recs, uint16_t *__restrict__ hist, ZbChunkCheck *__restrict__ chk,
@@ -197,7 +233,10 @@ __global__ void __launch_bounds__(LZ_THREADS, 3)
   const uint32_t chunk = blockIdx.x;
   const ZbChunkDesc d = desc[chunk];
   const uint32_t len = d.len;
-  const int tid = (int)threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int tid = (int)threadIdx.x, lane = tid & 31;
+  // tid >> 5, taken through a warp reduction so that the compiler knows it is warp-uniform: then so are every piece
+  // bound and the window loop's control flow, and the loop's warp intrinsics need no divergence guards (BRA.DIV)
+  const int warp = (int)__reduce_max_sync(ZB_FULL, (uint32_t)tid >> 5);
 
   if (tid == 0) {
     zb_mbar_init(bar, 1);
@@ -212,18 +251,20 @@ __global__ void __launch_bounds__(LZ_THREADS, 3)
   // checksums of this warp's pieces, each already shifted to the end of the chunk (uniform across the warp)
   uint32_t acc_crc = 0;
   uint64_t acc_a = 0, acc_b = 0;
+  LZ_CLK_DECL
 
   for (uint32_t ph = 0; ph < LZ_PHASES; ph++) {
     const uint32_t pbase = ph * LZ_PHASE_BYTES;               // first byte parsed in this phase
     if (ph && pbase >= len) break;
     const uint32_t sbase = ph ? pbase - LZ_PHASE_HIST : 0u;   // first byte staged (a multiple of 16: same misalignment)
     if (ph) __syncthreads();                                  // every warp is done with the previous phase's bytes
+    LZ_CLK(LZS_BARRIER)
     if (tid == 0 && len) {
       zb_fence_proxy_async();
       zb_stage_chunk(data, src + d.src_off + sbase, min(len, pbase + LZ_PHASE_BYTES + 384u) - sbase, bar);
     }
     // while the bulk copy is in flight: clear histograms (once), load the CRC tables
-    {
+    if (CK & ZB_CK_CRC) {
       uint32_t *crc_tab = reinterpret_cast<uint32_t *>(table);
       for (int i = lane; i < 1024; i += 32) crc_tab[i] = (&tabs->mul1024[0][0])[i];
     }
@@ -237,6 +278,7 @@ __global__ void __launch_bounds__(LZ_THREADS, 3)
       __syncwarp();
     }
     if (len) zb_mbar_wait(bar, ph & 1u);
+    LZ_CLK(LZS_WAIT)
 
     const uint32_t b0 = pbase + (uint32_t)warp * LZ_PIECE_BYTES;
     if (b0 >= len) continue;
@@ -247,21 +289,24 @@ __global__ void __launch_bounds__(LZ_THREADS, 3)
     uint32_t *whist = hist_all + (b0 / ZB_SUB_BYTES) * ZB_HIST_WORDS;
 
     // ---- checksums of this piece, shifted to the end of the chunk ----
-    {
-      ZbCheck c = zb_warp_checksums<LZ_PIECE_BYTES, LZ_LMUL_PQ>(data, doff + b0, b1 - b0,
-                                                                reinterpret_cast<const uint32_t *>(table), lane_mul);
+    if (CK) {
+      ZbCheck c = zb_warp_checksums<LZ_PIECE_BYTES, LZ_LMUL_PQ, CK>(data, doff + b0, b1 - b0,
+                                                                    reinterpret_cast<const uint32_t *>(table), lane_mul);
       const uint32_t after = len - b1;
       if (after) {
-        const uint32_t shift =
-            ((after & (LZ_PIECE_BYTES - 1)) == 0) ? lane_mul[LZ_LMUL_PIECE + after / LZ_PIECE_BYTES] : zb_xpow8_t(tabs->pow2, after);
-        c.crc_raw = zb_gf2_mul(c.crc_raw, shift);
-        c.b_sum += (uint64_t)after * c.a_sum;
+        if (CK & ZB_CK_CRC) {
+          const uint32_t shift = ((after & (LZ_PIECE_BYTES - 1)) == 0) ? lane_mul[LZ_LMUL_PIECE + after / LZ_PIECE_BYTES]
+                                                                       : zb_xpow8_t(tabs->pow2, after);
+          c.crc_raw = zb_gf2_mul(c.crc_raw, shift);
+        }
+        if (CK & ZB_CK_ADLER) c.b_sum += (uint64_t)after * c.a_sum;
       }
       acc_crc ^= c.crc_raw;
       acc_a += c.a_sum;
       acc_b += c.b_sum;
       __syncwarp();
     }
+    LZ_CLK(LZS_CHECKSUM)
 
     if (MODE == 1) {
       // the table region held the CRC step table until now: empty it
@@ -287,6 +332,7 @@ __global__ void __launch_bounds__(LZ_THREADS, 3)
       }
       __syncwarp();
     }
+    LZ_CLK(LZS_SEED)
     uint32_t entry = b0;
     uint32_t ksel = 0, kism = 0;  // lanes i and i + 16 keep the masks of window i of the current batch of 16
     uint32_t *grecs = recs + (size_t)chunk * ZB_RECS_PER_CHUNK + (b0 >> 2);  // this piece's record stream
@@ -301,7 +347,11 @@ __global__ void __launch_bounds__(LZ_THREADS, 3)
         const uint32_t cur = entry - wb;
         uint32_t m = 0, c = 0;
         if (MODE == 1) {
-          const uint32_t v = zb_ld32_unaligned(data, doff + p);
+          // this lane's 4 bytes; the word pair stays in registers for the compare below
+          const uint32_t *wp = reinterpret_cast<const uint32_t *>(data) + ((doff + p) >> 2);
+          const uint32_t sp = ((doff + p) & 3u) * 8u;
+          const uint32_t p0 = wp[0], p1 = wp[1];
+          const uint32_t v = __funnelshift_r(p0, p1, sp);
           const bool can = (p + 4 <= len);
           const uint32_t h = lz_hash(v);
           c = table[h];
@@ -323,14 +373,14 @@ __global__ void __launch_bounds__(LZ_THREADS, 3)
             __syncwarp();
           }
 #endif
+          LZ_CLK(LZS_PROBE)
           // a match may not cross the piece end (another warp starts its own parse there)
           const uint32_t limit = p < b1 ? min((uint32_t)ZB_MAX_MATCH, b1 - p) : 0u;
           if (can && c < p && p - c <= ZB_MAX_DIST && p >= entry && limit >= ZB_MIN_MATCH) {
             // unaligned compare, 4 bytes per step, carrying the upper word of each side
-            const uint32_t *wp = reinterpret_cast<const uint32_t *>(data) + ((doff + p) >> 2);
             const uint32_t *wc = reinterpret_cast<const uint32_t *>(data) + ((doff + c) >> 2);
-            const uint32_t sp = ((doff + p) & 3u) * 8u, sc = ((doff + c) & 3u) * 8u;
-            uint32_t hp = wp[1], hc = wc[1];
+            const uint32_t sc = ((doff + c) & 3u) * 8u;
+            uint32_t hp = p1, hc = wc[1];
             if (__funnelshift_r(wc[0], hc, sc) == v) {
               m = 4;
 #pragma unroll 1
@@ -348,10 +398,12 @@ __global__ void __launch_bounds__(LZ_THREADS, 3)
               if (m < LZ_LANE_CAP) m = min(m, limit);
             }
           }
+          LZ_CLK(LZS_EXTEND)
         }
         uint32_t endw;
         lz_select(data, doff, wb, b1, cur, nvalid, m, p - c, ring + slot * ZB_MATCH_SLOTS, sel, ism, endw);
         entry = wb + max(endw, nvalid);
+        LZ_CLK(LZS_SELECT)
       }
       if (bl == slot) {
         ksel = sel;
@@ -366,6 +418,7 @@ __global__ void __launch_bounds__(LZ_THREADS, 3)
         ksel = kism = 0;
         __syncwarp();
       }
+      LZ_CLK(LZS_BATCH)
     }
   }
   if (lane == 0) {
@@ -379,6 +432,8 @@ __global__ void __launch_bounds__(LZ_THREADS, 3)
     uint32_t *gh = reinterpret_cast<uint32_t *>(hist + (size_t)chunk * ZB_WARPS_PER_CHUNK * ZB_HIST_SYMS);
     for (int i = tid; i < ZB_WARPS_PER_CHUNK * ZB_HIST_WORDS; i += LZ_THREADS) gh[i] = hist_all[i];
   }
+  LZ_CLK(LZS_BARRIER)
+  LZ_CLK_PUBLISH()
   if (tid == 0) {
     uint32_t raw = 0;
     uint64_t a = 0, b = 0;
@@ -389,7 +444,7 @@ __global__ void __launch_bounds__(LZ_THREADS, 3)
     }
     ZbChunkCheck cc;
     cc.crc_raw = raw;
-    cc.adler = zb_adler_from_sums(a % ZB_ADLER_MOD, b % ZB_ADLER_MOD, len);
+    cc.adler = (CK & ZB_CK_ADLER) ? zb_adler_from_sums(a % ZB_ADLER_MOD, b % ZB_ADLER_MOD, len) : 0u;
     chk[chunk] = cc;
   }
 }
@@ -1183,13 +1238,25 @@ size_t zb_lz2_table_bytes(int *grid_out) {
   if (grid_out) *grid_out = grid;
   return (size_t)grid * LZ2_TABLES_PER_CTA * LZ2_BUCKETS * sizeof(uint2);
 }
+// the k_lz instance for a level's matcher (MODE) and a format's checksum (CK)
+typedef void (*ZbLzKernel)(const uint8_t *, const ZbChunkDesc *, uint2 *, uint32_t *, uint16_t *, ZbChunkCheck *,
+                           const ZbCrcTables *);
+static ZbLzKernel zb_lz_kernel(int mode, int data_format) {
+  const int ck = data_format == ZB_DF_GZIP ? ZB_CK_CRC : data_format == ZB_DF_ZLIB ? ZB_CK_ADLER : 0;
+  if (mode) return ck == ZB_CK_CRC ? k_lz<1, ZB_CK_CRC> : ck == ZB_CK_ADLER ? k_lz<1, ZB_CK_ADLER> : k_lz<1, 0>;
+  return ck == ZB_CK_CRC ? k_lz<0, ZB_CK_CRC> : ck == ZB_CK_ADLER ? k_lz<0, ZB_CK_ADLER> : k_lz<0, 0>;
+}
 // function attributes are per device: zb200_init calls this once for the ctx's device
 cudaError_t zb_setup_deflate_attrs() {
-  cudaError_t e = cudaFuncSetAttribute(k_lz<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, LZ_SM_TOTAL);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(k_lz<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, LZ_SM_TOTAL);
-  // three CTAs of 75 KiB: ask for the largest shared-memory carve-out
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(k_lz<0>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(k_lz<1>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  cudaError_t e = cudaSuccess;
+  static const int fmts[3] = {ZB_DF_GZIP, ZB_DF_ZLIB, ZB_DF_DEFLATE};
+  for (int mode = 0; mode < 2; mode++)
+    for (int f = 0; f < 3; f++) {
+      const ZbLzKernel k = zb_lz_kernel(mode, fmts[f]);
+      if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, LZ_SM_TOTAL);
+      // three CTAs of 75 KiB: ask for the largest shared-memory carve-out
+      if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+    }
   if (e == cudaSuccess) e = cudaFuncSetAttribute(k_lz2, cudaFuncAttributeMaxDynamicSharedMemorySize, LZ2_SM_TOTAL);
   // load the remaining kernels now rather than at their first launch (see zb_setup_inflate_attrs)
   cudaFuncAttributes fa;
@@ -1207,10 +1274,9 @@ cudaError_t zb_launch_lz(const ZbCompressWork &w, cudaStream_t s) {
     if ((uint32_t)grid > w.n_chunks) grid = (int)w.n_chunks;
     k_lz2<<<grid, LZ_THREADS, LZ2_SM_TOTAL, s>>>(w.src, w.desc, w.masks, w.recs, w.hist, w.chk, w.tabs, w.lz2_tables,
                                                  w.n_chunks, zb_lz2_params(w.level));
-  } else if (w.level == -2 || w.level == 0) {
-    k_lz<0><<<w.n_chunks, LZ_THREADS, LZ_SM_TOTAL, s>>>(w.src, w.desc, w.masks, w.recs, w.hist, w.chk, w.tabs);
   } else {
-    k_lz<1><<<w.n_chunks, LZ_THREADS, LZ_SM_TOTAL, s>>>(w.src, w.desc, w.masks, w.recs, w.hist, w.chk, w.tabs);
+    const ZbLzKernel k = zb_lz_kernel((w.level == -2 || w.level == 0) ? 0 : 1, w.data_format);
+    k<<<w.n_chunks, LZ_THREADS, LZ_SM_TOTAL, s>>>(w.src, w.desc, w.masks, w.recs, w.hist, w.chk, w.tabs);
   }
   return cudaGetLastError();
 }

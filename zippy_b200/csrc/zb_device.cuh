@@ -121,7 +121,10 @@ struct ZbCheck {
   uint64_t a_sum, b_sum;
 };
 // FULL = the piece size with the fast path, QOFF = where its quarter shifts x^(8 * FULL/4 * k), k = 0..3, sit in lane_mul.
-template <uint32_t FULL = ZB_SUB_BYTES, int QOFF = 41>
+// WANT = which sums are computed (ZB_CK_CRC | ZB_CK_ADLER); the other fields of the result are 0.
+#define ZB_CK_CRC 1
+#define ZB_CK_ADLER 2
+template <uint32_t FULL = ZB_SUB_BYTES, int QOFF = 41, int WANT = ZB_CK_CRC | ZB_CK_ADLER>
 __device__ __forceinline__ ZbCheck zb_warp_checksums(const uint8_t *base, uint32_t off, uint32_t n,
                                                      const uint32_t *tab, const uint32_t *lane_mul, uint32_t ts = 1u) {
   const int lane = zb_lane();
@@ -139,16 +142,19 @@ __device__ __forceinline__ ZbCheck zb_warp_checksums(const uint8_t *base, uint32
     for (uint32_t k = 0; k < QR; k++) {
       const uint32_t w0 = zb_ld32_unaligned(base, o + 128u * k), w1 = zb_ld32_unaligned(base, o + 128u * (QR + k));
       const uint32_t w2 = zb_ld32_unaligned(base, o + 128u * (2u * QR + k)), w3 = zb_ld32_unaligned(base, o + 128u * (3u * QR + k));
-      if (k) {
-        r0 = zb_mul1024(tab, r0);
-        r1 = zb_mul1024(tab, r1);
-        r2 = zb_mul1024(tab, r2);
-        r3 = zb_mul1024(tab, r3);
+      if (WANT & ZB_CK_CRC) {
+        if (k) {
+          r0 = zb_mul1024(tab, r0);
+          r1 = zb_mul1024(tab, r1);
+          r2 = zb_mul1024(tab, r2);
+          r3 = zb_mul1024(tab, r3);
+        }
+        r0 ^= w0;
+        r1 ^= w1;
+        r2 ^= w2;
+        r3 ^= w3;
       }
-      r0 ^= w0;
-      r1 ^= w1;
-      r2 ^= w2;
-      r3 ^= w3;
+      if (!(WANT & ZB_CK_ADLER)) continue;
       const uint32_t s0 = __dp4a(w0, 0x01010101u, 0u), s1 = __dp4a(w1, 0x01010101u, 0u);
       const uint32_t s2 = __dp4a(w2, 0x01010101u, 0u), s3 = __dp4a(w3, 0x01010101u, 0u);
       a += s0 + s1 + s2 + s3;
@@ -158,12 +164,18 @@ __device__ __forceinline__ ZbCheck zb_warp_checksums(const uint8_t *base, uint32
       b -= (uint64_t)(__dp4a(w0, 0x03020100u, 0u) + __dp4a(w1, 0x03020100u, 0u) + __dp4a(w2, 0x03020100u, 0u) +
                       __dp4a(w3, 0x03020100u, 0u));
     }
-    uint32_t r = zb_gf2_mul(r0, lane_mul[QOFF + 3]) ^ zb_gf2_mul(r1, lane_mul[QOFF + 2]) ^ zb_gf2_mul(r2, lane_mul[QOFF + 1]) ^ r3;
-    r = zb_gf2_mul(r, lane_mul[32 - lane]);
     ZbCheck out;
-    out.crc_raw = zb_warp_xor(r);
-    out.a_sum = zb_warp_sum64((uint64_t)a);
-    out.b_sum = zb_warp_sum64(b);
+    out.crc_raw = 0;
+    out.a_sum = out.b_sum = 0;
+    if (WANT & ZB_CK_CRC) {
+      uint32_t r = zb_gf2_mul(r0, lane_mul[QOFF + 3]) ^ zb_gf2_mul(r1, lane_mul[QOFF + 2]) ^ zb_gf2_mul(r2, lane_mul[QOFF + 1]) ^ r3;
+      r = zb_gf2_mul(r, lane_mul[32 - lane]);
+      out.crc_raw = zb_warp_xor(r);
+    }
+    if (WANT & ZB_CK_ADLER) {
+      out.a_sum = zb_warp_sum64((uint64_t)a);
+      out.b_sum = zb_warp_sum64(b);
+    }
     return out;
   }
   const uint32_t rows = n >> 7, tail = n & 127u;
@@ -204,18 +216,24 @@ __device__ __forceinline__ ZbCheck zb_warp_checksums(const uint8_t *base, uint32
       b += (uint64_t)(rem - i) * byte;
     }
   }
-  crc = zb_warp_xor(crc);
-  crc_tail = zb_warp_xor(crc_tail);
-  crc_rem = __shfl_sync(ZB_FULL, crc_rem, 0);
   ZbCheck out;
-  uint32_t raw = crc;
-  if (tail) {
-    raw = zb_gf2_mul(crc, zb_xpow8(tail));
-    if (rem) raw ^= zb_gf2_mul(crc_tail, zb_xpow8(rem)) ^ crc_rem;
-    else raw ^= crc_tail;
+  out.crc_raw = 0;
+  out.a_sum = out.b_sum = 0;
+  if (WANT & ZB_CK_CRC) {
+    crc = zb_warp_xor(crc);
+    crc_tail = zb_warp_xor(crc_tail);
+    crc_rem = __shfl_sync(ZB_FULL, crc_rem, 0);
+    uint32_t raw = crc;
+    if (tail) {
+      raw = zb_gf2_mul(crc, zb_xpow8(tail));
+      if (rem) raw ^= zb_gf2_mul(crc_tail, zb_xpow8(rem)) ^ crc_rem;
+      else raw ^= crc_tail;
+    }
+    out.crc_raw = raw;
   }
-  out.crc_raw = raw;
-  out.a_sum = zb_warp_sum64((uint64_t)a);
-  out.b_sum = zb_warp_sum64(b);
+  if (WANT & ZB_CK_ADLER) {
+    out.a_sum = zb_warp_sum64((uint64_t)a);
+    out.b_sum = zb_warp_sum64(b);
+  }
   return out;
 }
