@@ -928,6 +928,15 @@ __global__ void __launch_bounds__(128)
 #define PK_ROW_WORDS 17   // a 32-byte window encodes to at most 32 x 15 bits = 15 words (+ partial)
 #define PK_STG_WORDS (PK_ROW_WORDS * 32 + 4)   // one batch of 32 rows + the carried partial word
 #define PK_EDGES 10       // piece boundaries of a chunk: header+warp 0, warps 1..7, tail, end
+// While a batch's tokens are walked, stg holds only its carried word (stg[0]) and zeros, so the batch's inputs are
+// staged there and zeroed again before pk_append: the literal bytes in 36-byte slots, one per window (an odd word
+// stride: no bank conflicts when the 32 lanes store or read their own windows; the ninth word absorbs the source's
+// misalignment), then the batch's match records (the token loop reads one entry past a window's last record).
+#define PK_LIT_OFF 1
+#define PK_SLOT_WORDS 9
+#define PK_REC_OFF (PK_LIT_OFF + 32 * PK_SLOT_WORDS)
+static_assert(PK_REC_OFF + 32 * ZB_MATCH_SLOTS + 1 <= PK_STG_WORDS, "a batch's staged inputs fit in stg");
+#define PK_CODE_NONE 320  // codes[] entry of zero bits: the second code of an iteration that has none
 
 // Token -> bits, written with plain coalesced stores (no zero-fill, no global atomics).
 // A chunk's stream is a sequence of bit PIECES: [block header + warp 0's tokens], warp 1..7's
@@ -995,9 +1004,23 @@ __device__ __forceinline__ void pk_append(uint32_t *stg, const uint32_t *rows, u
   __syncwarp();
 }
 
-__global__ void __launch_bounds__(LZ_THREADS)
+// Append the n bits of v to a lane's row (acc: the accn < 32 bits of its incomplete word; accn + n < 64).  The
+// low word is stored whether or not it is complete: an incomplete one is stored again when it grows, and the
+// row's length leaves out what lies past its end.
+__device__ __forceinline__ void pk_put(uint32_t *rows, uint32_t v, uint32_t n, uint32_t &acc, uint32_t &accn,
+                                       uint32_t &ri) {
+  const uint32_t lo = acc | (v << accn), hi = __funnelshift_l(v, 0u, accn);
+  accn += n;
+  rows[ri] = lo;
+  ri += accn & 32u;  // row word k of lane i is rows[k * 32 + i]
+  acc = accn >= 32u ? hi : lo;
+  accn &= 31u;
+}
+
+__global__ void __launch_bounds__(LZ_THREADS, 6)  // 6 CTAs (48 warps) per SM: <= 40 registers, 36 KiB shared
     k_pack(ZbCompressWork w) {
-  __shared__ uint32_t codes[288 + 32];  // [0,288) litlen, [288,320) dist: code | len << 16
+  // [0,288) litlen, [288,320) dist, [320] none: code | code length << 16 | (code length + extra bits) << 24
+  __shared__ uint32_t codes[288 + 32 + 1];
   __shared__ uint32_t rows_all[ZB_WARPS_PER_CHUNK * PK_ROW_WORDS * 32];
   __shared__ uint32_t stg_all[ZB_WARPS_PER_CHUNK * PK_STG_WORDS];
   __shared__ PkEdges ed;
@@ -1009,12 +1032,17 @@ __global__ void __launch_bounds__(LZ_THREADS)
   const ZbChunkDesc d = w.desc[chunk];
   const ZbCodebook *cb = &w.cb[chunk];
   const uint32_t len = d.len;
-  const int tid = (int)threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int tid = (int)threadIdx.x, lane = tid & 31;
+  const int warp = (int)__reduce_max_sync(ZB_FULL, (uint32_t)tid >> 5);  // known warp-uniform: see k_lz
   const uint32_t btype = cb->block_type;
   const uint64_t out0 = w.chunk_off[chunk];  // byte offset of this chunk's deflate bytes
   const uint8_t *src = w.src + d.src_off;
 
-  for (int i = tid; i < 320; i += LZ_THREADS) codes[i] = i < 288 ? cb->ll[i] : cb->dd[i - 288];
+  for (int i = tid; i <= PK_CODE_NONE; i += LZ_THREADS) {
+    const uint32_t e = i < 288 ? cb->ll[i] : i < 320 ? cb->dd[i - 288] : 0u, clen = e >> 16;
+    const uint32_t xb = i > 256 && i < 288 ? zb_len_extra_bits(i - 257) : i >= 288 && i < 320 ? zb_dist_extra_bits(i - 288) : 0;
+    codes[i] = (e & 0xffffu) | clen << 16 | (clen + xb) << 24;
+  }
   for (int i = tid; i < ZB_WARPS_PER_CHUNK * PK_STG_WORDS; i += LZ_THREADS) stg_all[i] = 0u;
 
   // ---- framing bytes (zippy.nim:21-42, 50-58, 60-78): every byte written explicitly ----
@@ -1100,6 +1128,7 @@ __global__ void __launch_bounds__(LZ_THREADS)
       const uint2 *gmask = w.masks + (size_t)chunk * ZB_WINDOWS_PER_CHUNK;
       const uint32_t *grecs = w.recs + (size_t)chunk * ZB_RECS_PER_CHUNK + (size_t)warp * ZB_RECS_PER_SUB;
       const uint32_t nwin = (b1 - b0 + 31u) >> 5;
+      const uint32_t mis = (uint32_t)(uintptr_t)(src + b0) & 3u;  // the same for every batch (1 KiB apart)
       uint32_t rec_base = 0;
       for (uint32_t wbase = 0; wbase < nwin; wbase += 32) {
         if (wbase && (wbase & (ZB_REC_PIECE_WINDOWS - 1u)) == 0u) {  // the next 4 KiB piece: its own dense record stream
@@ -1120,61 +1149,56 @@ __global__ void __launch_bounds__(LZ_THREADS)
           const uint32_t t = __shfl_up_sync(ZB_FULL, rincl, o);
           if (lane >= o) rincl += t;
         }
-        const uint32_t *wrec = grecs + rec_base + rincl - nmatch;
-        rec_base += __shfl_sync(ZB_FULL, rincl, 31);
-        const uint8_t *wdata = src + ((size_t)win << 5);
-        uint64_t acc = 0;
-        uint32_t accn = 0, nw = 0, mcnt = 0;
-        while (s) {
-          const uint32_t bit = (uint32_t)(__ffs((int)s) - 1);
-          s &= s - 1;
-          // literal and match tokens share the first code (literal / length symbol): one lookup, one append,
-          // whatever mix of tokens the 32 lanes hold in this iteration; only the distance part is a branch
-          const bool is_m = (im >> bit) & 1u;
-          const uint32_t rec = is_m ? wrec[mcnt] : 0u;
-          mcnt += is_m ? 1u : 0u;
-          const uint32_t lc = rec & 31u;
-          const uint32_t sym = is_m ? 257u + lc : (uint32_t)wdata[bit];
-          const uint32_t e1 = codes[sym];
-          uint32_t v1 = e1 & 0xffffu, n1 = e1 >> 16;
-          if (is_m) {
-            v1 |= ((rec >> 5) & 31u) << n1;
-            n1 += (uint32_t)zb_len_extra_bits((int)lc);
-          } else if (s) {
-            // two literals in a row leave as one append (<= 30 bits): the all-literal windows are the ones that
-            // set the iteration count of the warp
-            const uint32_t bit2 = (uint32_t)(__ffs((int)s) - 1);
-            if (!((im >> bit2) & 1u)) {
-              const uint32_t e = codes[wdata[bit2]];
-              v1 |= (e & 0xffffu) << n1;
-              n1 += e >> 16;
-              s &= s - 1;
-            }
+        const uint32_t rtot = __shfl_sync(ZB_FULL, rincl, 31);
+        // ---- stage the batch's bytes (from the word that holds its first byte) and records in stg ----
+        {
+          const uint32_t bbase = b0 + (wbase << 5);
+          const uint32_t *pw = reinterpret_cast<const uint32_t *>(src + bbase - mis);
+          const uint32_t nword = min(1024u, b1 - bbase) + mis;  // 4 * (words to load) covers this many bytes
+#pragma unroll 1
+          for (uint32_t k = (uint32_t)lane; 4u * k < nword; k += 32) {
+            const uint32_t v = __ldg(pw + k);
+            uint32_t *q = stg + PK_LIT_OFF + k + (k >> 3);  // word k % 8 of slot k / 8
+            if (k < 256u) *q = v;
+            if (k && (k & 7u) == 0u) q[-1] = v;            // and the ninth word of the slot before
           }
-          acc |= (uint64_t)v1 << accn;
-          accn += n1;
-          if (accn >= 32) {
-            rows[nw * 32 + lane] = (uint32_t)acc;
-            nw++;
-            acc >>= 32;
-            accn -= 32;
-          }
-          if (is_m) {
-            const uint32_t dc = (rec >> 10) & 31u;
-            const uint32_t e2 = codes[288 + dc];
-            acc |= (uint64_t)((e2 & 0xffffu) | ((rec >> 15) << (e2 >> 16))) << accn;
-            accn += (e2 >> 16) + (uint32_t)zb_dist_extra_bits((int)dc);
-            if (accn >= 32) {
-              rows[nw * 32 + lane] = (uint32_t)acc;
-              nw++;
-              acc >>= 32;
-              accn -= 32;
-            }
-          }
+          const uint32_t *brec = grecs + rec_base;
+#pragma unroll 1
+          for (uint32_t k = (uint32_t)lane; k < rtot; k += 32) stg[PK_REC_OFF + k] = brec[k];
         }
-        if (accn) rows[nw * 32 + lane] = (uint32_t)acc;
+        rec_base += rtot;
         __syncwarp();
-        pk_append(stg, rows, nw * 32u + accn, bitcur, sw0, piece_start, dstw_rel, &ed);
+        // ---- one lane per window: every iteration emits two codes with their extra bits, the same operations
+        //      whatever token the lane holds.  A match: length code, distance code.  A literal followed by a
+        //      literal: both (the all-literal windows set the warp's iteration count).  A lone literal: it and
+        //      the zero-bit code ----
+        const uint8_t *lit = reinterpret_cast<const uint8_t *>(stg + PK_LIT_OFF + lane * PK_SLOT_WORDS) + mis;
+        uint32_t ri = PK_REC_OFF + rincl - nmatch;  // stg[ri]: the lane's next record
+        uint32_t wi = (uint32_t)lane, acc = 0, accn = 0;  // rows[wi]: the lane's incomplete row word
+        while (s) {
+          const uint32_t t1 = s & (0u - s);
+          s ^= t1;
+          const uint32_t t2 = s & (0u - s);  // 0: t1 is the last token
+          // both bytes are read whatever the tokens are (t2 = 0 reads lit[-1], inside stg): no branch
+          const uint32_t l1 = lit[31 - __clz(t1)], l2 = lit[31 - __clz(t2)];
+          const uint32_t r = stg[ri];
+          const bool is_m = (im & t1) != 0u;
+          const bool pair = t2 != 0u && (im & (t1 | t2)) == 0u;
+          s ^= pair ? t2 : 0u;
+          ri += is_m ? 1u : 0u;
+          const uint32_t rec = is_m ? r : 0u;
+          const uint32_t sym1 = is_m ? 257u + (rec & 31u) : l1;
+          const uint32_t sym2 = is_m ? 288u + ((rec >> 10) & 31u) : pair ? l2 : PK_CODE_NONE;
+          const uint32_t e1 = codes[sym1], e2 = codes[sym2];
+          pk_put(rows, (e1 & 0xffffu) | ((rec >> 5) & 31u) << __byte_perm(e1, 0u, 0x4442), e1 >> 24, acc, accn, wi);
+          pk_put(rows, (e2 & 0xffffu) | (rec >> 15) << __byte_perm(e2, 0u, 0x4442), e2 >> 24, acc, accn, wi);
+        }
+        rows[wi] = acc;
+        __syncwarp();
+        for (uint32_t k = (uint32_t)lane; k < PK_REC_OFF - PK_LIT_OFF + rtot; k += 32) stg[PK_LIT_OFF + k] = 0u;
+        __syncwarp();
+        // wi - lane = 32 x the complete words = their bits
+        pk_append(stg, rows, wi - (uint32_t)lane + accn, bitcur, sw0, piece_start, dstw_rel, &ed);
       }
     }
     // the piece's last, partial word (shared with its successor)
@@ -1186,7 +1210,7 @@ __global__ void __launch_bounds__(LZ_THREADS)
     const uint32_t e = codes[256];
     uint32_t pos = B0 + cb->eob_bit_start;
     unsigned long long tv = (unsigned long long)(e & 0xffffu);
-    uint32_t nb = e >> 16;
+    uint32_t nb = e >> 24;
     if (!cb->is_final) {
       nb += 3u;
       nb += (8u - ((pos + nb) & 7u)) & 7u;   // to the byte boundary
