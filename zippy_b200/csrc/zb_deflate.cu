@@ -594,7 +594,7 @@ __device__ __forceinline__ void lz2_extend(const Lz2Pos &P, const uint8_t *data,
     hp = np;
     hc = nq;
   }
-  if (mc < LZ_LANE_CAP) mc = min(mc, P.limit);
+  mc = min(mc, P.limit);  // bytes past the sub-chunk end (another member's, stale shared memory) never count
   if (mc > m) {
     m = mc;
     dist = d;
