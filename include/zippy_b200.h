@@ -145,6 +145,36 @@ int zb200_inflate_batch_crc32(zb200_ctx *ctx, const uint8_t *src_base, const uin
 int zb200_checksum_batch(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n,
                          int kind, uint32_t *out);
 
+/* ---- streaming compression: one gzip / zlib / raw member from input that arrives piece by piece ----
+ * What a stream emits, concatenated, is byte for byte what zb200_compress_batch writes for the whole input as
+ * one member (same level, format and fname_len), whatever the sizes of the writes.
+ *  - begin: level -2..9, data_format GZIP / ZLIB / DEFLATE, fname_len 0..25 (gzip FNAME letters, as
+ *    fname_lens in compress_batch; ignored for the other formats).  An invalid level or format fails with
+ *    ZB200_ERR_INVALID_LEVEL / ZB200_ERR_INVALID_FORMAT, an invalid fname_len with ZB200_ERR_ARG.
+ *  - The stream's state lives on the host inside the stream object: the pending input, the last 32 KiB of
+ *    input already compressed (the LZ levels' history), the running CRC-32 / Adler-32 and 64-bit byte count,
+ *    whether the header went out.  There is no device memory per stream; the kernels use the ctx's scratch.
+ *    Several streams may be open on one ctx, interleaved with each other and with any other call on it; calls
+ *    on one ctx serialise as always.  Free every stream of a ctx before zb200_shutdown.
+ *  - Chunking is the one-shot call's: 64 KiB chunks from the start of the member.  A chunk is compressed only
+ *    once it is known not to be the last, so a stream always holds back 1..65536 bytes (none only when nothing
+ *    was written); finish compresses what is held back as the last chunk, then writes the trailer.  A stream
+ *    with no input finishes as the empty member.  The header goes out with the first emitted bytes.
+ *  - write launches kernels only once a batch of input is pending (64 MiB, tools/bench_compress_stream.py);
+ *    smaller writes are only buffered and emit nothing.  *dst_len receives what was emitted.
+ *  - bound(st, len): the most bytes the next write of `len` bytes (or finish: len = 0) can emit.
+ *  - A write or finish after finish: ZB200_ERR_ARG.  ZB200_ERR_DST_TOO_SMALL consumes nothing and leaves the
+ *    stream as it was: retry with bound() bytes.  After a CUDA failure every later call reports it.
+ *  - Members of 4 GiB and more work: the byte count is 64-bit, gzip ISIZE is the total mod 2^32.
+ *  - free: at any time, finished or not. */
+typedef struct zb200_compress_stream zb200_compress_stream;
+int zb200_compress_stream_begin(zb200_ctx *ctx, int level, int data_format, int fname_len, zb200_compress_stream **out);
+size_t zb200_compress_stream_bound(const zb200_compress_stream *st, size_t len);
+int zb200_compress_stream_write(zb200_compress_stream *st, const uint8_t *src, size_t len,
+                                uint8_t *dst, size_t dst_cap, size_t *dst_len);
+int zb200_compress_stream_finish(zb200_compress_stream *st, uint8_t *dst, size_t dst_cap, size_t *dst_len);
+void zb200_compress_stream_free(zb200_compress_stream *st);
+
 /* ---- device-resident variants (pointers prefixed d_ are device memory on ctx's device;
  * offsets / statuses / sizes stay host arrays).  Used when the data already lives in HBM
  * (bench.py's `value`) and by the multi-GPU sharded path.  The call returns after the

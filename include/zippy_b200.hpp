@@ -193,4 +193,40 @@ inline std::vector<std::string> compressBatch(const std::vector<std::string> &it
   return res;
 }
 
+// One member compressed from input that arrives piece by piece (zb200_compress_stream_*, no reference
+// counterpart): what write() and finish() return, concatenated, is the member compressBatch writes for the whole
+// input with the same FNAME length.  Small writes are gathered and return "".  fnameLen < 0 with gzip draws the
+// FNAME length at random, as compress() does; ctx nullptr is this thread's default context.
+class CompressStream {
+ public:
+  explicit CompressStream(int level = DefaultCompression, CompressedDataFormat dataFormat = dfGzip, int fnameLen = -1,
+                          zb200_ctx *ctx = nullptr) {
+    if (fnameLen < 0) fnameLen = dataFormat == dfGzip ? (int)(std::random_device()() % 26) : 0;
+    detail::check(zb200_compress_stream_begin(ctx ? ctx : detail::ctx(), level, dataFormat, fnameLen, &st_));
+  }
+  ~CompressStream() { zb200_compress_stream_free(st_); }
+  CompressStream(const CompressStream &) = delete;
+  CompressStream &operator=(const CompressStream &) = delete;
+
+  std::string write(const void *src, size_t len) {
+    std::string out(zb200_compress_stream_bound(st_, len), '\0');
+    size_t n = 0;
+    detail::check(zb200_compress_stream_write(st_, static_cast<const uint8_t *>(src), len,
+                                              reinterpret_cast<uint8_t *>(&out[0]), out.size(), &n));
+    out.resize(n);
+    return out;
+  }
+  std::string write(const std::string &data) { return write(data.data(), data.size()); }
+  std::string finish() {
+    std::string out(zb200_compress_stream_bound(st_, 0), '\0');
+    size_t n = 0;
+    detail::check(zb200_compress_stream_finish(st_, reinterpret_cast<uint8_t *>(&out[0]), out.size(), &n));
+    out.resize(n);
+    return out;
+  }
+
+ private:
+  zb200_compress_stream *st_ = nullptr;
+};
+
 }  // namespace zippy

@@ -240,3 +240,49 @@ proc inflateBatchCrc32*(items: openArray[string], sizes: openArray[int]): seq[(s
   for i in 0 ..< items.len:
     check st[i]
     result.add (dst[dofs[i].int ..< (dofs[i] + lens[i]).int], crcs[i])
+
+# ---- streaming compression (no counterpart in zippy.nim): one member from input that arrives piece by
+# piece; what write and finish return, concatenated, is compressBatch(@[whole input]) with the same FNAME ----
+type Zb200CompressStream = pointer
+proc zb200_compress_stream_begin(ctx: Zb200Ctx, level, dataFormat, fnameLen: cint,
+                                 st: ptr Zb200CompressStream): cint {.importc, cdecl, dynlib: lib.}
+proc zb200_compress_stream_bound(st: Zb200CompressStream, len: csize_t): csize_t {.importc, cdecl, dynlib: lib.}
+proc zb200_compress_stream_write(st: Zb200CompressStream, src: pointer, len: csize_t, dst: pointer, dstCap: csize_t,
+                                 dstLen: ptr csize_t): cint {.importc, cdecl, dynlib: lib.}
+proc zb200_compress_stream_finish(st: Zb200CompressStream, dst: pointer, dstCap: csize_t,
+                                  dstLen: ptr csize_t): cint {.importc, cdecl, dynlib: lib.}
+proc zb200_compress_stream_free(st: Zb200CompressStream) {.importc, cdecl, dynlib: lib.}
+
+type CompressStream* = object
+  st: Zb200CompressStream
+
+proc newCompressStream*(level = DefaultCompression, dataFormat = dfGzip,
+                        fnameLen = -1): CompressStream {.raises: [ZippyError].} =
+  ## fnameLen < 0 with dfGzip draws the FNAME length at random, as compress does (zippy.nim:28-42)
+  var k = fnameLen
+  if k < 0:
+    k = 0
+    if dataFormat == dfGzip:
+      var urand: array[1, uint8]
+      if not urandom(urand):
+        raise newException(ZippyError, "Failed to generate random number")
+      k = (urand[0] mod 26).int
+  check zb200_compress_stream_begin(getCtx(), level.cint, dataFormat.cint, k.cint, result.st.addr)
+
+proc write*(s: var CompressStream, data: string): string {.raises: [ZippyError].} =
+  ## small writes are gathered on the host and return ""
+  result = newString(zb200_compress_stream_bound(s.st, data.len.csize_t).int + 1)
+  var n: csize_t
+  check zb200_compress_stream_write(s.st, data.cstring, data.len.csize_t, result[0].addr, result.len.csize_t, n.addr)
+  result.setLen(n.int)
+
+proc finish*(s: var CompressStream): string {.raises: [ZippyError].} =
+  result = newString(zb200_compress_stream_bound(s.st, 0).int + 1)
+  var n: csize_t
+  check zb200_compress_stream_finish(s.st, result[0].addr, result.len.csize_t, n.addr)
+  result.setLen(n.int)
+
+proc close*(s: var CompressStream) =
+  if s.st != nil:
+    zb200_compress_stream_free(s.st)
+    s.st = nil

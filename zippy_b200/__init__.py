@@ -8,7 +8,8 @@ Same names, argument meaning and error behaviour as the reference module
     crc32(src) / adler32(src) -> int
     ZippyError, dfDetect/dfZlib/dfGzip/dfDeflate, NoCompression/BestSpeed/...
 
-plus the batch forms that make a GPU worthwhile (no reference counterpart).  All codec
+plus the batch forms that make a GPU worthwhile and CompressStream, one member compressed from input
+that arrives in pieces (no reference counterpart).  All codec
 work happens in libzippy_b200.so's CUDA kernels; this module only owns buffers, draws the
 reference's random gzip FNAME length (zippy.nim:28-42) and maps status codes to ZippyError.
 There is no CPU fallback: without the library or a CUDA device every call raises.
@@ -26,7 +27,8 @@ NoCompression, BestSpeed, BestCompression = 0, 1, 9                    # common.
 DefaultCompression, HuffmanOnly = -1, -2
 
 __all__ = ["compress", "uncompress", "crc32", "adler32", "deflate", "inflate", "compress_batch", "uncompress_batch",
-           "uncompressed_sizes", "checksum_batch", "ZippyError", "Context", "MultiGpu", "dfDetect", "dfZlib", "dfGzip",
+           "uncompressed_sizes", "checksum_batch", "ZippyError", "Context", "CompressStream", "MultiGpu", "dfDetect",
+           "dfZlib", "dfGzip",
            "dfDeflate", "NoCompression", "BestSpeed", "BestCompression", "DefaultCompression", "HuffmanOnly"]
 
 
@@ -315,6 +317,57 @@ class Context:
         v = ctypes.c_uint32(0)
         _check(self._h, _native.lib().zb200_adler32(self._h, src.ctypes.data, src.size, ctypes.byref(v)))
         return v.value
+
+
+class CompressStream:
+    """One gzip / zlib / raw member written piece by piece (zb200_compress_stream_*): the concatenation of what
+    write() and finish() return is exactly compress_batch([whole input]) with the same FNAME length.  Input is
+    gathered until a batch is pending, so most small writes return b"".  With gzip and fname_len=None the FNAME
+    length is drawn at random, as compress() does (zippy.nim:28-42)."""
+
+    def __init__(self, level=DefaultCompression, dataFormat=dfGzip, fname_len=None, ctx=None):
+        if fname_len is None:
+            fname_len = os.urandom(1)[0] % 26 if dataFormat == dfGzip else 0
+        self._ctx = ctx if ctx is not None else default_context()
+        self._h = ctypes.c_void_p()
+        _check(self._ctx._h, _native.lib().zb200_compress_stream_begin(self._ctx._h, level, dataFormat, fname_len,
+                                                                       ctypes.byref(self._h)))
+
+    def _out(self, n):
+        """-> (a destination for the next call that takes n input bytes, its length word)"""
+        if not self._h:
+            raise ZippyError(22, "the stream is closed")
+        return np.empty(int(_native.lib().zb200_compress_stream_bound(self._h, n)) + 8, dtype=np.uint8), ctypes.c_size_t(0)
+
+    def write(self, data):
+        src = _as_u8(data)
+        out, m = self._out(src.size)
+        _check(self._ctx._h, _native.lib().zb200_compress_stream_write(self._h, src.ctypes.data, src.size, out.ctypes.data,
+                                                                       out.size, ctypes.byref(m)))
+        return out[:m.value].tobytes()
+
+    def finish(self):
+        out, m = self._out(0)
+        _check(self._ctx._h, _native.lib().zb200_compress_stream_finish(self._h, out.ctypes.data, out.size,
+                                                                        ctypes.byref(m)))
+        return out[:m.value].tobytes()
+
+    def close(self):
+        if self._h:
+            _native.lib().zb200_compress_stream_free(self._h)
+            self._h = ctypes.c_void_p()
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
 
 
 class MultiGpu:

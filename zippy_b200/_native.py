@@ -56,6 +56,11 @@ SYMBOLS = {
                                               c_intp]),
     "zb200_uncompress_sizes_device": (c_int, [ctypes.c_void_p, c_u8p, c_u64p, c_size_t, c_int, c_u64p, c_intp]),
     "zb200_checksum_batch_device": (c_int, [ctypes.c_void_p, c_u8p, c_u64p, c_size_t, c_int, ctypes.c_void_p]),
+    "zb200_compress_stream_begin": (c_int, [ctypes.c_void_p, c_int, c_int, c_int, ctypes.POINTER(ctypes.c_void_p)]),
+    "zb200_compress_stream_bound": (c_size_t, [ctypes.c_void_p, c_size_t]),
+    "zb200_compress_stream_write": (c_int, [ctypes.c_void_p, c_u8p, c_size_t, c_u8p, c_size_t, ctypes.POINTER(c_size_t)]),
+    "zb200_compress_stream_finish": (c_int, [ctypes.c_void_p, c_u8p, c_size_t, ctypes.POINTER(c_size_t)]),
+    "zb200_compress_stream_free": (None, [ctypes.c_void_p]),
     "zb200_mgpu_init": (c_int, [ctypes.c_void_p, c_int, ctypes.POINTER(ctypes.c_void_p)]),
     "zb200_mgpu_shutdown": (None, [ctypes.c_void_p]),
     "zb200_mgpu_device_count": (c_int, [ctypes.c_void_p]),

@@ -57,6 +57,10 @@ StreamMemOps load_stream_memops() {
 
 constexpr size_t kMaxChunksPerGroup = 32768;  // device-resident batches: 2 GiB of input per launch group
 constexpr size_t kHostGroupChunks = 4096;     // host batches: 256 MiB groups so transfers overlap the kernels
+// A compress stream launches once this much input is pending: smaller writes are gathered, as every launch costs
+// five kernels and a sync.  Of 16 / 64 / 256 MiB, 64 was the fastest at levels 1 and Default on one H100 80GB HBM3
+// at 700 W (tools/bench_compress_stream.py, DESIGN.md section 8 "Compress streams").
+constexpr size_t ZB_STREAM_BATCH_BYTES = 64u << 20;
 
 }  // namespace
 
@@ -159,6 +163,8 @@ struct zb200_ctx {
   DevBuf desc, member_first, fname, masks, recs, hist, chk, cb, chunk_off, member_off, member_check, member_isize;
   DevBuf src_off, dst_off, out_len, status, expect, kind, counter, ck_out, ck_pieces, ck_first, ck_piece_out, ck_partials;
   DevBuf in_stage, out_stage, lz2_tables;
+  DevBuf carry;             // a compress stream's member carry: [0] in, [1] out
+  size_t stream_batch_bytes = ZB_STREAM_BATCH_BYTES;  // pending input at which a stream write launches
   DevBuf seg_src, seg_dst, seg_len, seg_status, seg_kind, seg_expect, seg_cand, skip_mask;  // large-member segments
   DevBuf mark_scratch, mark_segs, seg_bits;  // speculative segments of a large member (uint16 symbols, descriptors)
   DevBuf mark_win;          // window resolve scratch of the joint segments: group window maps (uint16) + incoming windows
@@ -187,6 +193,20 @@ struct zb200_ctx {
   zb200_timing timing;
   std::string last_err;
   std::mutex mu;
+};
+
+// One member compressed from input that arrives piece by piece.  All of its state is on the host; the
+// kernels run on its ctx's scratch, so any number of streams and other calls can share a ctx.
+struct zb200_compress_stream {
+  zb200_ctx *ctx = nullptr;
+  int level = 0, data_format = 0;
+  uint8_t fname_len = 0;
+  size_t batch_bytes = 0;      // launch once this much input is pending
+  std::vector<uint8_t> buf;    // [history | pending input]: pending starts at a chunk boundary of the member
+  size_t hist = 0;             // bytes of history (the LZ levels: the last <= 32 KiB already compressed)
+  ZbMemberCarry carry{0u, 1u, 0ull};  // the input compressed so far: raw CRC-32, Adler-32, bytes
+  bool head_done = false, finished = false;
+  int err = ZB200_OK;          // a CUDA failure: the stream is unusable
 };
 
 namespace {
@@ -368,14 +388,26 @@ struct Group {
   uint64_t bound;       // output bound of the group
 };
 
+// One launch of a compress stream (zb200_compress_stream_*): a run of whole chunks of ONE member that
+// continues what earlier launches compressed.  The source holds `hist` bytes of the member's preceding input
+// in front of the run (k_lz2's history for the first chunk); `head`: the run starts the member (header);
+// `last`: the run ends it (BFINAL, trailer).  carry_in is the member's bytes before the run, carry_out
+// receives the bytes through its end.
+struct StreamPart {
+  uint32_t hist;
+  bool head, last;
+  ZbMemberCarry carry_in, carry_out;
+};
+
 // ---- compress: device-resident (h_src == h_dst == nullptr) or pipelined host buffers ----
 // With host buffers the batch is cut into groups and H2D(g+1) || kernels(g) || D2H(g-1) run
 // on three streams; each group's output offset is chained on the device (out_base_ptr), so
 // the only host waits are for the small per-group offset arrays that size the D2H copies.
+// sp (host buffers, n == 1 only): the member is one part of a stream; null for every batch call.
 int compress_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint8_t *h_src, const uint64_t *src_offsets,
                     size_t n, int level, int data_format, const uint8_t *fname_lens, uint8_t *d_dst,
                     size_t dst_cap, uint8_t *h_dst, size_t h_dst_cap, uint64_t *dst_offsets, int *statuses,
-                    size_t max_group_chunks) {
+                    size_t max_group_chunks, StreamPart *sp = nullptr) {
   if (level < -2 || level > 9) return ZB200_ERR_INVALID_LEVEL;
   if (data_format != ZB200_DF_GZIP && data_format != ZB200_DF_ZLIB && data_format != ZB200_DF_DEFLATE)
     return ZB200_ERR_INVALID_FORMAT;
@@ -392,7 +424,9 @@ int compress_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint8_t *h_src, 
   ctx->timing.n_chunks = 0;
   dst_offsets[0] = 0;
   if (n == 0) return ZB200_OK;
-  const uint64_t src_lo = src_offsets[0];  // d_src holds [src_lo, src_hi) rebased to 0 when staging from the host
+  const uint64_t hist = sp ? sp->hist : 0;
+  const bool head = !sp || sp->head, last = !sp || sp->last;
+  const uint64_t src_lo = src_offsets[0] - hist;  // d_src holds [src_lo, src_hi) rebased to 0 when staging from the host
   const bool src_pageable = h_src && is_pageable(h_src + src_lo), dst_pageable = h_dst && is_pageable(h_dst);
 
   // ---- plan: groups, descriptors ----
@@ -426,8 +460,8 @@ int compress_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint8_t *h_src, 
         d.src_off = src_offsets[m1] - (h_src ? src_lo : 0) + (uint64_t)k * ZB_CHUNK_BYTES;
         d.len = (uint32_t)std::min<uint64_t>(ZB_CHUNK_BYTES, len - (uint64_t)k * ZB_CHUNK_BYTES);
         d.member = (uint32_t)(m1 - m0);
-        d.flags = (k == 0 ? ZB_CHUNK_FIRST : 0u) | (k == nc - 1 ? ZB_CHUNK_LAST : 0u);
-        d.pad = (level == -1 || level >= 2) ? (uint32_t)std::min<uint64_t>(32768, (uint64_t)k * ZB_CHUNK_BYTES) : 0u;
+        d.flags = (k == 0 ? ZB_CHUNK_FIRST | (head ? ZB_CHUNK_HEAD : 0u) : 0u) | (k == nc - 1 && last ? ZB_CHUNK_LAST : 0u);
+        d.pad = (level == -1 || level >= 2) ? (uint32_t)std::min<uint64_t>(32768, hist + (uint64_t)k * ZB_CHUNK_BYTES) : 0u;
         desc.push_back(d);
       }
       g.bound += zb200_compress_bound((size_t)len, data_format) + 64;
@@ -437,7 +471,7 @@ int compress_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint8_t *h_src, 
     g.nc = desc.size() - g.c0;
     chunks_left -= std::min(chunks_left, g.nc);
     first.push_back((uint32_t)g.nc);
-    g.in_lo = src_offsets[m0] - src_lo;
+    g.in_lo = m0 == 0 ? 0 : src_offsets[m0] - src_lo;  // the first group also copies a stream's history
     g.in_hi = src_offsets[m1] - src_lo;
     max_nc = std::max(max_nc, g.nc);
     max_nm = std::max(max_nm, g.m1 - g.m0);
@@ -460,13 +494,16 @@ int compress_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint8_t *h_src, 
   ENSURE(ctx->member_check, max_nm * sizeof(uint32_t));
   ENSURE(ctx->member_isize, max_nm * sizeof(uint32_t));
   if (level == -1 || level >= 2) ENSURE(ctx->lz2_tables, zb_lz2_table_bytes(nullptr));
+  if (sp) ENSURE(ctx->carry, 2 * sizeof(ZbMemberCarry));
   {
-    int rc = ensure_pinned(ctx, nfirst * sizeof(uint64_t) + 64);
+    int rc = ensure_pinned(ctx, nfirst * sizeof(uint64_t) + sizeof(ZbMemberCarry) + 64);
     if (rc) return rc;
     rc = ensure_group_events(ctx, 3 * ng + 1);
     if (rc) return rc;
   }
   uint64_t *pin_off = (uint64_t *)ctx->pin;
+  ZbMemberCarry *pin_carry = (ZbMemberCarry *)(pin_off + nfirst);  // a stream's carry-out comes back behind the offsets
+  ZbMemberCarry *d_carry = (ZbMemberCarry *)ctx->carry.p;          // [0] in, [1] out
 
   cudaStream_t s = ctx->stream;
   cudaStream_t sh = h_src ? ctx->h2d_stream : s, sd = h_dst ? ctx->d2h_stream : s;
@@ -474,6 +511,7 @@ int compress_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint8_t *h_src, 
   CK(cudaMemcpyAsync(ctx->member_first.p, first.data(), nfirst * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
   if (fname_lens && data_format == ZB200_DF_GZIP)
     CK(cudaMemcpyAsync(ctx->fname.p, fname_lens, n, cudaMemcpyHostToDevice, s));
+  if (sp) CK(cudaMemcpyAsync(d_carry, &sp->carry_in, sizeof(ZbMemberCarry), cudaMemcpyHostToDevice, s));
   CK(cudaMemsetAsync(ctx->group_end.p, 0, sizeof(uint64_t), s));
   if (h_src || h_dst) {
     // the transfer streams must not run ahead of the setup above
@@ -500,6 +538,8 @@ int compress_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint8_t *h_src, 
     w.member_off = (uint64_t *)ctx->member_off.p + g.first0;
     w.member_check = (uint32_t *)ctx->member_check.p;
     w.member_isize = (uint32_t *)ctx->member_isize.p;
+    w.carry_in = sp ? d_carry : nullptr;
+    w.carry_out = sp ? d_carry + 1 : nullptr;
     w.tabs = ctx->d_tabs;
     w.lz2_tables = (uint2 *)ctx->lz2_tables.p;
     w.n_chunks = (uint32_t)g.nc;
@@ -559,6 +599,7 @@ int compress_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint8_t *h_src, 
                        cudaMemcpyDeviceToDevice, s));
     CK(cudaMemcpyAsync(pin_off + g.first0, w.member_off, (w.n_members + 1) * sizeof(uint64_t),
                        cudaMemcpyDeviceToHost, s));
+    if (sp) CK(cudaMemcpyAsync(pin_carry, w.carry_out, sizeof(ZbMemberCarry), cudaMemcpyDeviceToHost, s));
     CK(cudaEventRecord(ctx->gev[3 * gi + 2], s));
     if (timed) CK(cudaEventRecord(ctx->ev[4], s));
     CK(zb_launch_pack(w, s));
@@ -586,12 +627,43 @@ int compress_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint8_t *h_src, 
   if (h_src) CK(cudaStreamSynchronize(sh));
   if (h_dst) CK(cudaStreamSynchronize(sd));
   if (total_out > dst_cap) return ZB200_ERR_DST_TOO_SMALL;
+  if (sp) sp->carry_out = *pin_carry;
   // per-kernel times: measured on the first group, scaled to the batch by chunk count
   const float scale = groups[0].nc ? (float)nc_all / (float)groups[0].nc : 1.f;
   ctx->timing.lz_ms = ev_ms(ctx->ev[0], ctx->ev[1]) * scale;
   ctx->timing.huff_ms = ev_ms(ctx->ev[1], ctx->ev[2]) * scale;
   ctx->timing.scan_ms = ev_ms(ctx->ev[2], ctx->ev[3]) * scale;
   ctx->timing.pack_ms = ev_ms(ctx->ev[4], ctx->ev[5]) * scale;
+  return ZB200_OK;
+}
+
+// Compress the stream's next `nbytes` pending bytes (whole chunks unless `last`) into dst; ctx locked.  On
+// success the carry advances and the compressed input leaves the buffer (its last 32 KiB stay as history);
+// on failure nothing changes.
+int stream_run(zb200_compress_stream *st, size_t nbytes, bool last, uint8_t *dst, size_t dst_cap, size_t *dst_len) {
+  zb200_ctx *ctx = st->ctx;
+  if (!dst) return ZB200_ERR_DST_TOO_SMALL;  // every run emits at least one byte
+  const size_t in_end = st->hist + nbytes;
+  ENSURE(ctx->in_stage, in_end + 64);
+  ENSURE(ctx->out_stage, zb200_compress_bound(nbytes, st->data_format) + 128);
+  const uint64_t offs[2] = {st->hist, in_end};
+  uint64_t dst_offs[2] = {0, 0};
+  StreamPart sp;
+  sp.hist = (uint32_t)st->hist;
+  sp.head = !st->head_done;
+  sp.last = last;
+  sp.carry_in = st->carry;
+  int rc = compress_locked(ctx, (const uint8_t *)ctx->in_stage.p, st->buf.data(), offs, 1, st->level, st->data_format,
+                           &st->fname_len, (uint8_t *)ctx->out_stage.p, ctx->out_stage.cap & ~(size_t)3, dst, dst_cap,
+                           dst_offs, nullptr, ctx->host_group_chunks, &sp);
+  if (rc) return rc;
+  *dst_len = (size_t)dst_offs[1];
+  st->carry = sp.carry_out;
+  st->head_done = true;
+  const bool lz = st->level == -1 || st->level >= 2;
+  const size_t keep = lz ? std::min<size_t>(32768, in_end) : 0;
+  st->buf.erase(st->buf.begin(), st->buf.begin() + (in_end - keep));
+  st->hist = keep;
   return ZB200_OK;
 }
 
@@ -1804,6 +1876,10 @@ int zb200_init(int device, zb200_ctx **out) {
     long v = atol(e);
     if (v > 0) ctx->dev_group_chunks = ctx->host_group_chunks = (size_t)v;
   }
+  if (const char *e = getenv("ZB200_STREAM_BATCH_BYTES")) {  // test hook: compress streams launch at this much pending input
+    long long v = atoll(e);
+    if (v > 0) ctx->stream_batch_bytes = (size_t)v;
+  }
   if (const char *e = getenv("ZB200_BIG_MEMBER_BYTES")) {  // test hook: segment path for small members too
     long long v = atoll(e);
     if (v > 0) {
@@ -1856,7 +1932,7 @@ void zb200_shutdown(zb200_ctx *ctx) {
   DevBuf *bufs[] = {&ctx->desc, &ctx->member_first, &ctx->fname, &ctx->masks, &ctx->recs, &ctx->hist, &ctx->chk,
                     &ctx->cb, &ctx->chunk_off, &ctx->member_off, &ctx->member_check, &ctx->member_isize,
                     &ctx->src_off, &ctx->dst_off, &ctx->out_len, &ctx->status, &ctx->expect, &ctx->kind,
-                    &ctx->counter, &ctx->ck_out, &ctx->ck_pieces, &ctx->ck_first, &ctx->ck_piece_out, &ctx->ck_partials, &ctx->in_stage, &ctx->out_stage, &ctx->lz2_tables,
+                    &ctx->counter, &ctx->ck_out, &ctx->ck_pieces, &ctx->ck_first, &ctx->ck_piece_out, &ctx->ck_partials, &ctx->in_stage, &ctx->out_stage, &ctx->lz2_tables, &ctx->carry,
                     &ctx->seg_src, &ctx->seg_dst, &ctx->seg_len, &ctx->seg_status, &ctx->seg_kind, &ctx->seg_expect, &ctx->seg_cand, &ctx->skip_mask, &ctx->order, &ctx->mark_scratch, &ctx->mark_segs, &ctx->seg_bits, &ctx->mark_win, &ctx->gate};
   for (DevBuf *b : bufs)
     if (b->p) cudaFree(b->p);
@@ -2000,6 +2076,82 @@ int zb200_compress_batch_h2d(zb200_ctx *ctx, const uint8_t *src_base, const uint
     return ZB200_OK;
   });
 }
+
+// ---- compress streams ----
+int zb200_compress_stream_begin(zb200_ctx *ctx, int level, int data_format, int fname_len, zb200_compress_stream **out) {
+  return guarded(ctx, [&]() -> int {
+    if (!ctx || !out) return ZB200_ERR_ARG;
+    *out = nullptr;
+    if (level < -2 || level > 9) return ZB200_ERR_INVALID_LEVEL;
+    if (data_format != ZB200_DF_GZIP && data_format != ZB200_DF_ZLIB && data_format != ZB200_DF_DEFLATE)
+      return ZB200_ERR_INVALID_FORMAT;
+    if (fname_len < 0 || fname_len > 25) return ZB200_ERR_ARG;
+    zb200_compress_stream *st = new zb200_compress_stream();
+    st->ctx = ctx;
+    st->level = level;
+    st->data_format = data_format;
+    st->fname_len = (uint8_t)fname_len;
+    {
+      std::lock_guard<std::mutex> lk(ctx->mu);
+      st->batch_bytes = ctx->stream_batch_bytes;
+    }
+    st->buf.reserve(65536);  // a non-null source even for an empty member
+    *out = st;
+    return ZB200_OK;
+  });
+}
+
+size_t zb200_compress_stream_bound(const zb200_compress_stream *st, size_t len) {
+  return st ? zb200_compress_bound(st->buf.size() - st->hist + len, st->data_format) : 0;
+}
+
+int zb200_compress_stream_write(zb200_compress_stream *st, const uint8_t *src, size_t len, uint8_t *dst, size_t dst_cap,
+                                size_t *dst_len) {
+  if (!st) return ZB200_ERR_ARG;
+  zb200_ctx *ctx = st->ctx;
+  return guarded(ctx, [&]() -> int {
+    if (!dst_len || (len && !src)) return ZB200_ERR_ARG;
+    *dst_len = 0;
+    if (st->err) return st->err;
+    if (st->finished) return ZB200_ERR_ARG;
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    DeviceGuard g(ctx->device);
+    memset(&ctx->timing, 0, sizeof(ctx->timing));
+    const size_t old = st->buf.size(), pending = old - st->hist + len;
+    st->buf.insert(st->buf.end(), src, src + len);
+    // launch with enough input gathered, holding back 1..65536 bytes: the chunk that may turn out to be the last
+    if (pending < st->batch_bytes || pending <= ZB_CHUNK_BYTES) return ZB200_OK;
+    const int rc = stream_run(st, (pending - 1) / ZB_CHUNK_BYTES * ZB_CHUNK_BYTES, false, dst, dst_cap, dst_len);
+    if (rc) {
+      st->buf.resize(old);  // nothing consumed
+      if (rc == ZB200_ERR_CUDA) st->err = rc;
+    }
+    return rc;
+  });
+}
+
+int zb200_compress_stream_finish(zb200_compress_stream *st, uint8_t *dst, size_t dst_cap, size_t *dst_len) {
+  if (!st) return ZB200_ERR_ARG;
+  zb200_ctx *ctx = st->ctx;
+  return guarded(ctx, [&]() -> int {
+    if (!dst_len) return ZB200_ERR_ARG;
+    *dst_len = 0;
+    if (st->err) return st->err;
+    if (st->finished) return ZB200_ERR_ARG;
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    DeviceGuard g(ctx->device);
+    memset(&ctx->timing, 0, sizeof(ctx->timing));
+    const int rc = stream_run(st, st->buf.size() - st->hist, true, dst, dst_cap, dst_len);
+    if (rc == ZB200_ERR_CUDA) st->err = rc;
+    if (rc) return rc;
+    st->finished = true;
+    std::vector<uint8_t>().swap(st->buf);
+    st->hist = 0;
+    return ZB200_OK;
+  });
+}
+
+void zb200_compress_stream_free(zb200_compress_stream *st) { delete st; }
 
 // second half of the sharded path: once the size exchange has told a rank where its shard lands in
 // the concatenated stream, its device-resident members go straight to that place in host memory

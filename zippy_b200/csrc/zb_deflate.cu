@@ -846,7 +846,7 @@ __global__ void __launch_bounds__(SCAN_THREADS)
       flags = d.flags;
       member = d.member;
       sz = w.cb[c].total_bytes;
-      if (flags & ZB_CHUNK_FIRST) {
+      if (flags & ZB_CHUNK_HEAD) {
         head = frame_head_bytes(w.data_format, w.fname_len, member);
         sz += head;
       }
@@ -885,7 +885,8 @@ __global__ void __launch_bounds__(SCAN_THREADS)
 
 // whole-member checksums: one warp per member.  Each lane folds a contiguous run of the member's
 // chunks (raw(A||B) = raw(A) * x^(8|B|) + raw(B); Adler by its closed form), then a shuffle tree
-// folds the 32 runs, so a member of 16384 chunks (1 GiB) is not combined serially.
+// folds the 32 runs, so a member of 16384 chunks (1 GiB) is not combined serially.  A carry-in (the
+// member's bytes before this launch) goes in front; the trailer value and ISIZE are of the whole.
 __global__ void __launch_bounds__(128)
     k_member_check(ZbCompressWork w) {
   const uint32_t m = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31u;
@@ -915,6 +916,19 @@ __global__ void __launch_bounds__(128)
     }
   }
   if (lane == 0) {
+    if (w.carry_in) {
+      const ZbMemberCarry ci = w.carry_in[m];
+      if (w.data_format == ZB_DF_ZLIB) ad = zb_adler32_combine(ci.adler, ad, bytes);
+      else if (w.data_format == ZB_DF_GZIP) raw = zb_gf2_mul(ci.crc_raw, zb_xpow8_t(w.tabs->pow2, bytes)) ^ raw;
+      bytes += ci.bytes;
+    }
+    if (w.carry_out) {
+      ZbMemberCarry co;
+      co.crc_raw = raw;
+      co.adler = ad;
+      co.bytes = bytes;
+      w.carry_out[m] = co;
+    }
     uint32_t v = 0;
     if (w.data_format == ZB_DF_ZLIB) v = ad;
     else if (w.data_format == ZB_DF_GZIP)
@@ -1046,7 +1060,7 @@ __global__ void __launch_bounds__(LZ_THREADS, 6)  // 6 CTAs (48 warps) per SM: <
   for (int i = tid; i < ZB_WARPS_PER_CHUNK * PK_STG_WORDS; i += LZ_THREADS) stg_all[i] = 0u;
 
   // ---- framing bytes (zippy.nim:21-42, 50-58, 60-78): every byte written explicitly ----
-  if (tid == 32 && (d.flags & ZB_CHUNK_FIRST)) {
+  if (tid == 32 && (d.flags & ZB_CHUNK_HEAD)) {
     uint8_t *h = w.dst + w.member_off[d.member];
     if (w.data_format == ZB_DF_GZIP) {
       h[0] = 31; h[1] = 139; h[2] = 8; h[3] = 8;  // FNAME flag set, as the reference does

@@ -12,11 +12,21 @@ struct ZbChunkDesc {
   uint64_t src_off;   // byte offset of the chunk in the source buffer
   uint32_t len;       // 0..65536
   uint32_t member;    // index of the input this chunk belongs to
-  uint32_t flags;     // bit0: first chunk of its member, bit1: last chunk
+  uint32_t flags;     // ZB_CHUNK_*
   uint32_t pad;       // k_lz2: bytes of the member's preceding data staged as history (<= 32768)
 };
-#define ZB_CHUNK_FIRST 1u
-#define ZB_CHUNK_LAST 2u
+#define ZB_CHUNK_FIRST 1u  // first chunk of its member in this launch group: places member_off
+#define ZB_CHUNK_LAST 2u   // last chunk of its member: BFINAL, then the trailer
+#define ZB_CHUNK_HEAD 4u   // the member's gzip / zlib header goes in front of this chunk (a stream's later
+                           // launches continue a member whose header an earlier launch wrote: FIRST without HEAD)
+
+// The part of a member compressed before this launch (a compress stream): raw CRC-32 and Adler-32 of its
+// bytes and their count.  The empty prefix is {0, 1, 0}.
+struct ZbMemberCarry {
+  uint32_t crc_raw;
+  uint32_t adler;
+  uint64_t bytes;
+};
 
 struct ZbChunkCheck {
   uint32_t crc_raw;   // init-0 CRC of the chunk bytes
@@ -40,6 +50,8 @@ struct ZbCompressWork {
   uint64_t *member_off;        // [n_members + 1] output offsets (member_off[n] = total)
   uint32_t *member_check;      // [n_members] crc32 (gzip) or adler32 (zlib) of the whole member
   uint32_t *member_isize;      // [n_members] input size mod 2^32 (gzip ISIZE)
+  const ZbMemberCarry *carry_in;  // [n_members] or null (= the empty prefix): folded in front of each member's chunks
+  ZbMemberCarry *carry_out;       // [n_members] or null: carry_in followed by this launch's chunks
   uint64_t out_base;           // byte offset in dst where this group's first member starts ...
   const uint64_t *out_base_ptr;// ... or, when non-null, a device word holding it (the previous group's end),
                                // so consecutive groups can be enqueued without a host round trip
