@@ -4,12 +4,14 @@
     python tools/lz1_model.py [--blocks N]
 
 Replays the kernel's parse on the first N C2 blocks (bench.py's offsets): 4 KiB pieces, a fresh 2048-entry
-table per piece pre-seeded with the 2 KiB before it, one probe per position, the 4-byte verify, the extension
-by 4 bytes per step up to the 32-byte lane cap, and the greedy chain "match -> first candidate at or after
-its end".  Same-hash stores of one window resolve as "highest lane wins" (the GPU leaves that to the
-hardware; it does not change these statistics).  Prints, per entered window: lanes that pass the 4-byte
-check, extension steps (max over the warp and summed over lanes), matches the chain selects and windows
-whose last match hits the lane cap.  Those numbers size the stages tools/lz1_stages.py times.
+table per piece pre-seeded with the 2 KiB before it (in the second 32 KiB phase only the 1 KiB of the first phase
+that is staged again: the piece at 32768 gets 1 KiB), one probe per position, the 4-byte verify (with at least
+4 bytes left before the piece end), the extension by 4 bytes per step up to the 32-byte lane cap, and the greedy
+chain "match -> first candidate at or after its end".  Same-hash stores of one window resolve as "highest lane
+wins".  Prints, per entered window: lanes that pass the 4-byte check, extension steps (max over the warp and
+summed over lanes), matches the chain selects and windows whose last match hits the lane cap.  Those numbers
+size the stages tools/lz1_stages.py times.  tests/test_gpu_lz1_model.py checks them against the token-exact
+model tests/native/lz1_model.c.
 """
 import argparse
 import os
@@ -19,24 +21,25 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 PIECE, PRESEED, CAP, MAX_MATCH, MAX_DIST = 4096, 2048, 32, 258, 32768
+PHASE, PHASE_HIST = 32768, 1024
 
 
 def lz_hash(v):
     return ((v * 0x9E3779B1) & 0xffffffff) >> 21
 
 
-def model(blocks):
-    from tests import util
-    T = util.text_corpus(util.load_corpus())
+def window_stats(blocks):
+    """Per-window work of the parse of `blocks` (each 64 KiB of text without NUL bytes), summed."""
     B = 65536
     tot = dict(windows=0, entered=0, verified=0, ext_steps_warp=0, ext_steps_lanes=0, chain=0, cap=0)
-    for i in range(blocks):
-        o = util._sm64(0xC2 + i) % (len(T) - B)
-        d = T[o:o + B] + b"\0" * 400
+    for blk in blocks:
+        assert len(blk) == B
+        d = blk + b"\0" * 400
         w4 = [int.from_bytes(d[p:p + 4], "little") for p in range(B)]
         for pb in range(0, B, PIECE):
             tab = {}
-            for p in range(max(0, pb - PRESEED), pb):
+            sbase = PHASE - PHASE_HIST if pb >= PHASE else 0
+            for p in range(pb - min(PRESEED, pb - sbase), pb):
                 tab[lz_hash(w4[p])] = p
             entry, b1 = pb, pb + PIECE
             for wb in range(pb, b1, 32):
@@ -53,7 +56,7 @@ def model(blocks):
                 for l in range(32):
                     p, c = wb + l, cand[l]
                     lim = min(MAX_MATCH, b1 - p)
-                    if c < p and p - c <= MAX_DIST and p >= entry and lim >= 3 and w4[p] == w4[c]:
+                    if c < p and p - c <= MAX_DIST and p >= entry and lim >= 4 and w4[p] == w4[c]:
                         m, steps = 4, 0
                         for k in range(1, CAP // 4):
                             steps += 1
@@ -90,7 +93,9 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--blocks", type=int, default=24)
     args = ap.parse_args()
-    tot = model(args.blocks)
+    from tests import util
+    T = util.text_corpus(util.load_corpus())
+    tot = window_stats([util.c2_block(T, i) for i in range(args.blocks)])
     n = tot["entered"]
     print("%d C2 blocks: %d windows, %d entered" % (args.blocks, tot["windows"], n))
     for k in ("verified", "ext_steps_warp", "ext_steps_lanes", "chain", "cap"):

@@ -364,8 +364,8 @@ __global__ void __launch_bounds__(LZ_THREADS, 3)
           __syncwarp();
           // make the outcome independent of the arbitration: the highest position wins (every round strictly
           // raises the entry, so it ends).  Slows the kernel; off by default because the
-          // arbitration IS a fixed function of the instruction's addresses on this hardware -- the full-size
-          // run-to-run test (tests/test_gpu_fullsize.py) is what holds that claim to account
+          // arbitration IS fixed on this hardware: the lowest lane lands, which tests/test_gpu_lz1_model.py
+          // asserts token by token (and this variant's tokens under the highest-position rule)
           for (;;) {
             const bool lost = can && table[h] < (uint16_t)p;
             if (!__any_sync(ZB_FULL, lost)) break;
