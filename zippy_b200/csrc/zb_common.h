@@ -112,6 +112,32 @@ ZB_HD uint32_t zb_len_base(int code) {
   return ((4u + (uint32_t)(code & 3)) << ((code >> 2) - 1)) + 3;
 }
 
+// The same codes without branches (the parse converts every match with these): code and extra value of a match
+// length 3..258 / a distance 1..32768.  With e = the code's extra bits, code = 4e + (v >> e) for v = len - 3 and
+// 2e + (v >> e) for v = d - 1 (e = 0 covers the codes without extra bits); the extra value is v's low e bits.
+ZB_HD uint32_t zb_hibit(uint32_t v) {  // index of the highest set bit of v | 1
+#if defined(__CUDA_ARCH__)
+  return 31u - (uint32_t)__clz((int)(v | 1u));
+#else
+  return 31u - (uint32_t)__builtin_clz(v | 1u);
+#endif
+}
+ZB_HD uint32_t zb_len_code_bf(uint32_t len, uint32_t &extra) {
+  const uint32_t v = len - 3u;
+  const int h = (int)zb_hibit(v) - 2;
+  const uint32_t e = h > 0 ? (uint32_t)h : 0u;
+  const bool top = len == 258u;  // 258 has its own code, 28, with no extra bits
+  extra = top ? 0u : v & ((1u << e) - 1u);
+  return top ? 28u : 4u * e + (v >> e);
+}
+ZB_HD uint32_t zb_dist_code_bf(uint32_t d, uint32_t &extra) {
+  const uint32_t v = d - 1u;
+  const int h = (int)zb_hibit(v) - 1;
+  const uint32_t e = h > 0 ? (uint32_t)h : 0u;
+  extra = v & ((1u << e) - 1u);
+  return 2u * e + (v >> e);
+}
+
 ZB_HD uint32_t zb_brev16(uint32_t v, int len) {  // reverse the low `len` bits (len<=16)
   if (len == 0) return 0u;
 #if defined(__CUDA_ARCH__)

@@ -74,9 +74,10 @@ __device__ __forceinline__ uint32_t low_mask(uint32_t n) { return shl_clamp(1u, 
 // Final match record consumed by k_pack: length code | length extra value << 5 |
 // distance code << 10 | distance extra value << 15.
 __device__ __forceinline__ uint32_t lz_final_rec(uint32_t mlen, uint32_t dist, int &lc, int &dc) {
-  lc = zb_len_code(mlen);
-  dc = zb_dist_code(dist);
-  return (uint32_t)lc | ((mlen - zb_len_base(lc)) << 5) | ((uint32_t)dc << 10) | ((dist - zb_dist_base(dc)) << 15);
+  uint32_t le, de;
+  lc = (int)zb_len_code_bf(mlen, le);
+  dc = (int)zb_dist_code_bf(dist, de);
+  return (uint32_t)lc | (le << 5) | ((uint32_t)dc << 10) | (de << 15);
 }
 
 
@@ -107,6 +108,11 @@ __device__ __forceinline__ void lz_select(const uint8_t *data, uint32_t off0, ui
     }
     ism = vis;
     const int lastm = 31 - __clz((int)ism);
+    // the coverage before the lane-cap extension: a capped last match covers every position after it whether the
+    // extension clips it to the piece or not (the piece end is nvalid, which sel masks), so this reduce need not
+    // wait for the extension and runs alongside the shuffle below
+    const uint32_t cov = (ism & lbit) ? (low_mask(endp) & ~low_mask((uint32_t)lane)) : 0u;
+    const uint32_t covered = __reduce_or_sync(ZB_FULL, cov);
     uint32_t mlast = __shfl_sync(ZB_FULL, m, lastm);
     if (mlast >= LZ_LANE_CAP) {
       const uint32_t md = __shfl_sync(ZB_FULL, dist, lastm);
@@ -125,8 +131,6 @@ __device__ __forceinline__ void lz_select(const uint8_t *data, uint32_t off0, ui
       mlast = min(mlast, min((uint32_t)ZB_MAX_MATCH, b1 - pos));
       if (lane == lastm) m = mlast;
     }
-    const uint32_t cov = (ism & lbit) ? (low_mask((uint32_t)lane + m) & ~low_mask((uint32_t)lane)) : 0u;
-    const uint32_t covered = __reduce_or_sync(ZB_FULL, cov);
     sel = ism | (~covered & ~low_mask(cur) & low_mask(nvalid));
     endw = (uint32_t)lastm + mlast;
     if (ism & lbit) {
@@ -144,7 +148,10 @@ __device__ __forceinline__ void lz_select(const uint8_t *data, uint32_t off0, ui
 // of the windows' match counts places them, and the packer recomputes the same prefix from the masks.
 // (Eight fixed slots per window made every record a 4-byte write into its own 32-byte sector: 2.3x the
 // algorithmic DRAM traffic.)  The parts of a window split its literals by position and its matches round-robin.
-template <int LPW>
+// LITS = false: the caller has counted the literals already (k_lz<1> does it in the window loop, one atomic per
+// lane and window instead of a loop here of one LDS + atomic per literal, as long as the busiest part's).
+// Matches convert without branches (lz_final_rec).
+template <int LPW, bool LITS>
 __device__ __forceinline__ void lz_batch_pass(const uint8_t *wdata, bool active, uint32_t ksel, uint32_t kism,
                                               const uint32_t *ring_win, uint32_t *whist, uint2 *gmask_w,
                                               uint32_t *grecs_piece, uint32_t &rec_base) {
@@ -153,7 +160,7 @@ __device__ __forceinline__ void lz_batch_pass(const uint8_t *wdata, bool active,
   if (active && part == 0) *gmask_w = make_uint2(ksel, kism);
   const uint32_t im = active ? kism : 0u;
   const uint32_t pm = (0xffffffffu >> (32 - 32 / LPW)) << (part * (32 / LPW));
-  uint32_t s = active ? (ksel & ~kism & pm) : 0u;  // this part's literal tokens
+  uint32_t s = (LITS && active) ? (ksel & ~kism & pm) : 0u;  // this part's literal tokens
   while (s) {
     const uint32_t bit = (uint32_t)(__ffs((int)s) - 1);
     s &= s - 1;
@@ -345,13 +352,14 @@ __global__ void __launch_bounds__(LZ_THREADS, 3)
         const uint32_t p = wb + (uint32_t)lane;
         const uint32_t nvalid = min(32u, b1 - wb);
         const uint32_t cur = entry - wb;
-        uint32_t m = 0, c = 0;
+        uint32_t m = 0, c = 0, lit = 0;
         if (MODE == 1) {
           // this lane's 4 bytes; the word pair stays in registers for the compare below
           const uint32_t *wp = reinterpret_cast<const uint32_t *>(data) + ((doff + p) >> 2);
           const uint32_t sp = ((doff + p) & 3u) * 8u;
           const uint32_t p0 = wp[0], p1 = wp[1];
           const uint32_t v = __funnelshift_r(p0, p1, sp);
+          lit = v & 255u;
           const bool can = (p + 4 <= len);
           const uint32_t h = lz_hash(v);
           c = table[h];
@@ -377,23 +385,38 @@ __global__ void __launch_bounds__(LZ_THREADS, 3)
           // a match may not cross the piece end (another warp starts its own parse there)
           const uint32_t limit = p < b1 ? min((uint32_t)ZB_MAX_MATCH, b1 - p) : 0u;
           if (can && c < p && p - c <= ZB_MAX_DIST && p >= entry && limit >= ZB_MIN_MATCH) {
-            // unaligned compare, 4 bytes per step, carrying the upper word of each side
+            // unaligned compare, 8 bytes per step, carrying the upper word of each side; the first step's four words
+            // are loaded with the 4-byte check and every step loads the next one's, so a lane waits for one round of
+            // shared-memory loads per 8 bytes (4 before)
             const uint32_t *wc = reinterpret_cast<const uint32_t *>(data) + ((doff + c) >> 2);
             const uint32_t sc = ((doff + c) & 3u) * 8u;
             uint32_t hp = p1, hc = wc[1];
+            uint32_t np = wp[2], nq = wc[2], np2 = wp[3], nq2 = wc[3];
             if (__funnelshift_r(wc[0], hc, sc) == v) {
               m = 4;
 #pragma unroll 1
-              for (int k = 2; k <= LZ_LANE_CAP / 4; k++) {
-                const uint32_t np = wp[k], nq = wc[k];
+              for (int k = 2;; k += 2) {
                 const uint32_t x = __funnelshift_r(hp, np, sp) ^ __funnelshift_r(hc, nq, sc);
+                const uint32_t x2 = __funnelshift_r(np, np2, sp) ^ __funnelshift_r(nq, nq2, sc);
                 if (x) {
                   m += (uint32_t)(__ffs((int)x) - 1) >> 3;
                   break;
                 }
-                m += 4;
-                hp = np;
-                hc = nq;
+                if (k == LZ_LANE_CAP / 4) {
+                  m += 4;
+                  break;
+                }
+                if (x2) {
+                  m += 4u + ((uint32_t)(__ffs((int)x2) - 1) >> 3);
+                  break;
+                }
+                m += 8;
+                hp = np2;
+                hc = nq2;
+                np = wp[k + 2];
+                nq = wc[k + 2];
+                np2 = wp[k + 3];
+                nq2 = wc[k + 3];
               }
               if (m < LZ_LANE_CAP) m = min(m, limit);
             }
@@ -403,6 +426,8 @@ __global__ void __launch_bounds__(LZ_THREADS, 3)
         uint32_t endw;
         lz_select(data, doff, wb, b1, cur, nvalid, m, p - c, ring + slot * ZB_MATCH_SLOTS, sel, ism, endw);
         entry = wb + max(endw, nvalid);
+        // level 1 counts the window's literals here, one atomic per lane, from the byte the probe already holds
+        if (MODE == 1 && ((sel & ~ism) >> lane & 1u)) atomicAdd(&whist[lit >> 1], 1u << ((lit & 1u) * 16u));
         LZ_CLK(LZS_SELECT)
       }
       if (bl == slot) {
@@ -413,7 +438,7 @@ __global__ void __launch_bounds__(LZ_THREADS, 3)
       if (slot == LZ_BATCH_WINDOWS - 1u || wb + 32 >= b1) {
         __syncwarp();
         const uint32_t bwin = win - slot + bl;  // this lane's window
-        lz_batch_pass<LZ_BATCH_LPW>(data + (uint32_t)(doff + (bwin << 5)), bl <= slot, ksel, kism, ring + bl * ZB_MATCH_SLOTS,
+        lz_batch_pass<LZ_BATCH_LPW, MODE != 1>(data + (uint32_t)(doff + (bwin << 5)), bl <= slot, ksel, kism, ring + bl * ZB_MATCH_SLOTS,
                                     whist, gmask + bwin, grecs, rec_base);
         ksel = kism = 0;
         __syncwarp();
@@ -778,7 +803,7 @@ __global__ void __launch_bounds__(LZ_THREADS, 2)
         if (slot == LZ2_RING_WINDOWS - 1u || wb + 32 >= b1) {
           __syncwarp();
           const uint32_t bwin = win - slot + bl;  // four lanes per window
-          lz_batch_pass<32 / LZ2_RING_WINDOWS>(data + off0 + (bwin << 5), bl <= slot, ksel, kism, ring + bl * ZB_MATCH_SLOTS,
+          lz_batch_pass<32 / LZ2_RING_WINDOWS, true>(data + off0 + (bwin << 5), bl <= slot, ksel, kism, ring + bl * ZB_MATCH_SLOTS,
                                                whist, gmask + bwin,
                                                grecs + ((wb & ~(uint32_t)(ZB_REC_PIECE_BYTES - 1u)) >> 2), rec_base);
           ksel = kism = 0;
