@@ -175,6 +175,41 @@ int zb200_compress_stream_write(zb200_compress_stream *st, const uint8_t *src, s
 int zb200_compress_stream_finish(zb200_compress_stream *st, uint8_t *dst, size_t dst_cap, size_t *dst_len);
 void zb200_compress_stream_free(zb200_compress_stream *st);
 
+/* ---- streaming decompression: one gzip / zlib / raw member from compressed input that arrives piece by piece ----
+ * Whatever the sizes of the writes (empty ones included), everything read from a stream, concatenated, is
+ * byte for byte what zippy.uncompress(whole input, data_format) returns, and the stream's final status is that
+ * call's status.  One exception: a member whose output exceeds 4 GiB - 33 KiB and that uncompress can only decode
+ * serially (no parallel segments) ends there with ZB200_ERR_DST_TOO_SMALL; a stream has no such limit and decodes it.
+ *  - begin: data_format DETECT, GZIP, ZLIB or DEFLATE (anything else: ZB200_ERR_INVALID_FORMAT).  Raw streams
+ *    start at byte 0 (there is no `pos`).
+ *  - write consumes all of src; *avail (may be NULL) receives the decoded bytes now waiting to be read.  finish
+ *    says the input has ended: it decodes what is held, then checks the trailer, checksum before size.
+ *    read moves up to dst_cap waiting bytes into dst (*dst_len: how many); it works after finish too.
+ *  - What depends on the input's length waits until the length is known: nothing about the header is decided
+ *    before 19 bytes have arrived (or finish), and the last 8 (gzip) / 4 (zlib) bytes are always held back as the
+ *    possible trailer.  As in uncompress, bytes between the final block and the trailer are ignored, and so is
+ *    anything after a raw stream's final block.  A second gzip member is not decoded (the reference rejects it).
+ *  - Errors: once a write or finish fails, every later call (read included) returns the same status.  Bytes read
+ *    before that come only from blocks that decoded completely; for a truncated member they are a prefix of its
+ *    output.  A write or finish after finish: ZB200_ERR_ARG.
+ *  - The stream's state lives on the host inside the stream object: the compressed input not decoded yet (from a
+ *    block boundary on), the last 32 KiB of output, the running CRC-32 / Adler-32 and 64-bit output count (ISIZE is
+ *    compared mod 2^32), the wrapper, the decoded bytes not read yet.  There is no device memory per stream; the
+ *    kernels use the ctx's scratch.  Several streams may be open on one ctx, interleaved with each other and with any
+ *    other call on it; calls on one ctx serialise as always.  Free every stream of a ctx before zb200_shutdown.
+ *  - write launches kernels only once a batch of compressed input is pending (64 MiB,
+ *    tools/bench_decompress_stream.py); smaller writes are only buffered.  One launch reads at most twice that much
+ *    input and produces at most about 1 GiB (more only when a single block is larger); a large write is decoded by
+ *    as many launches as it needs before it returns.
+ *  - Decoded bytes stay in the stream until read: read after every write.
+ *  - free: at any time, finished or not. */
+typedef struct zb200_decompress_stream zb200_decompress_stream;
+int zb200_decompress_stream_begin(zb200_ctx *ctx, int data_format, zb200_decompress_stream **out);
+int zb200_decompress_stream_write(zb200_decompress_stream *st, const uint8_t *src, size_t len, size_t *avail);
+int zb200_decompress_stream_finish(zb200_decompress_stream *st, size_t *avail);
+int zb200_decompress_stream_read(zb200_decompress_stream *st, uint8_t *dst, size_t dst_cap, size_t *dst_len);
+void zb200_decompress_stream_free(zb200_decompress_stream *st);
+
 /* ---- device-resident variants (pointers prefixed d_ are device memory on ctx's device;
  * offsets / statuses / sizes stay host arrays).  Used when the data already lives in HBM
  * (bench.py's `value`) and by the multi-GPU sharded path.  The call returns after the

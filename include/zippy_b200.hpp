@@ -229,4 +229,40 @@ class CompressStream {
   zb200_compress_stream *st_ = nullptr;
 };
 
+// One member decoded from compressed input that arrives piece by piece (zb200_decompress_stream_*, no reference
+// counterpart): what write() and finish() return, concatenated, is uncompress(whole input, dataFormat); a bad input
+// throws the ZippyError uncompress throws.  Small writes are gathered and return "".  ctx nullptr is this thread's
+// default context.
+class DecompressStream {
+ public:
+  explicit DecompressStream(CompressedDataFormat dataFormat = dfDetect, zb200_ctx *ctx = nullptr) {
+    detail::check(zb200_decompress_stream_begin(ctx ? ctx : detail::ctx(), dataFormat, &st_));
+  }
+  ~DecompressStream() { zb200_decompress_stream_free(st_); }
+  DecompressStream(const DecompressStream &) = delete;
+  DecompressStream &operator=(const DecompressStream &) = delete;
+
+  std::string write(const void *src, size_t len) {
+    size_t avail = 0;
+    detail::check(zb200_decompress_stream_write(st_, static_cast<const uint8_t *>(src), len, &avail));
+    return drain(avail);
+  }
+  std::string write(const std::string &data) { return write(data.data(), data.size()); }
+  std::string finish() {
+    size_t avail = 0;
+    detail::check(zb200_decompress_stream_finish(st_, &avail));
+    return drain(avail);
+  }
+
+ private:
+  std::string drain(size_t avail) {
+    std::string out(avail, '\0');
+    size_t n = 0;
+    detail::check(zb200_decompress_stream_read(st_, reinterpret_cast<uint8_t *>(&out[0]), out.size(), &n));
+    out.resize(n);
+    return out;
+  }
+  zb200_decompress_stream *st_ = nullptr;
+};
+
 }  // namespace zippy

@@ -286,3 +286,44 @@ proc close*(s: var CompressStream) =
   if s.st != nil:
     zb200_compress_stream_free(s.st)
     s.st = nil
+
+# ---- streaming decompression (no counterpart in zippy.nim): one member from compressed input that arrives piece
+# by piece; what write and finish return, concatenated, is uncompress(whole input, dataFormat), and a bad input
+# raises uncompress's ZippyError message (strerror of the same status) ----
+type Zb200DecompressStream = pointer
+proc zb200_decompress_stream_begin(ctx: Zb200Ctx, dataFormat: cint,
+                                   st: ptr Zb200DecompressStream): cint {.importc, cdecl, dynlib: lib.}
+proc zb200_decompress_stream_write(st: Zb200DecompressStream, src: pointer, len: csize_t,
+                                   avail: ptr csize_t): cint {.importc, cdecl, dynlib: lib.}
+proc zb200_decompress_stream_finish(st: Zb200DecompressStream, avail: ptr csize_t): cint {.importc, cdecl, dynlib: lib.}
+proc zb200_decompress_stream_read(st: Zb200DecompressStream, dst: pointer, dstCap: csize_t,
+                                  dstLen: ptr csize_t): cint {.importc, cdecl, dynlib: lib.}
+proc zb200_decompress_stream_free(st: Zb200DecompressStream) {.importc, cdecl, dynlib: lib.}
+
+type DecompressStream* = object
+  st: Zb200DecompressStream
+
+proc newDecompressStream*(dataFormat = dfDetect): DecompressStream {.raises: [ZippyError].} =
+  check zb200_decompress_stream_begin(getCtx(), dataFormat.cint, result.st.addr)
+
+proc drain(s: var DecompressStream, avail: csize_t): string {.raises: [ZippyError].} =
+  result = newString(avail.int + 1)
+  var n: csize_t
+  check zb200_decompress_stream_read(s.st, result[0].addr, avail, n.addr)
+  result.setLen(n.int)
+
+proc write*(s: var DecompressStream, data: string): string {.raises: [ZippyError].} =
+  ## small writes are gathered on the host and return ""
+  var avail: csize_t
+  check zb200_decompress_stream_write(s.st, data.cstring, data.len.csize_t, avail.addr)
+  s.drain(avail)
+
+proc finish*(s: var DecompressStream): string {.raises: [ZippyError].} =
+  var avail: csize_t
+  check zb200_decompress_stream_finish(s.st, avail.addr)
+  s.drain(avail)
+
+proc close*(s: var DecompressStream) =
+  if s.st != nil:
+    zb200_decompress_stream_free(s.st)
+    s.st = nil

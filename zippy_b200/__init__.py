@@ -8,8 +8,9 @@ Same names, argument meaning and error behaviour as the reference module
     crc32(src) / adler32(src) -> int
     ZippyError, dfDetect/dfZlib/dfGzip/dfDeflate, NoCompression/BestSpeed/...
 
-plus the batch forms that make a GPU worthwhile and CompressStream, one member compressed from input
-that arrives in pieces (no reference counterpart).  All codec
+plus the batch forms that make a GPU worthwhile, CompressStream, one member compressed from input
+that arrives in pieces, and DecompressStream, one member decoded from compressed input that arrives in pieces
+(no reference counterparts).  All codec
 work happens in libzippy_b200.so's CUDA kernels; this module only owns buffers, draws the
 reference's random gzip FNAME length (zippy.nim:28-42) and maps status codes to ZippyError.
 There is no CPU fallback: without the library or a CUDA device every call raises.
@@ -27,7 +28,8 @@ NoCompression, BestSpeed, BestCompression = 0, 1, 9                    # common.
 DefaultCompression, HuffmanOnly = -1, -2
 
 __all__ = ["compress", "uncompress", "crc32", "adler32", "deflate", "inflate", "compress_batch", "uncompress_batch",
-           "uncompressed_sizes", "checksum_batch", "ZippyError", "Context", "CompressStream", "MultiGpu", "dfDetect",
+           "uncompressed_sizes", "checksum_batch", "ZippyError", "Context", "CompressStream", "DecompressStream",
+           "MultiGpu", "dfDetect",
            "dfZlib", "dfGzip",
            "dfDeflate", "NoCompression", "BestSpeed", "BestCompression", "DefaultCompression", "HuffmanOnly"]
 
@@ -355,6 +357,59 @@ class CompressStream:
     def close(self):
         if self._h:
             _native.lib().zb200_compress_stream_free(self._h)
+            self._h = ctypes.c_void_p()
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class DecompressStream:
+    """One gzip / zlib / raw member decoded from compressed input that arrives in pieces (zb200_decompress_stream_*):
+    the concatenation of what write() and finish() return is exactly uncompress(whole input, dataFormat), and a bad
+    input raises the ZippyError uncompress raises (at the latest from finish()).  Input is gathered until a batch is
+    pending, so most small writes return b""."""
+
+    def __init__(self, dataFormat=dfDetect, ctx=None):
+        self._ctx = ctx if ctx is not None else default_context()
+        self._h = ctypes.c_void_p()
+        _check(self._ctx._h, _native.lib().zb200_decompress_stream_begin(self._ctx._h, dataFormat, ctypes.byref(self._h)))
+
+    def _handle(self):
+        if not self._h:
+            raise ZippyError(22, "the stream is closed")
+        return self._h
+
+    def _drain(self, avail):
+        out = np.empty(avail, dtype=np.uint8)
+        m = ctypes.c_size_t(0)
+        _check(self._ctx._h, _native.lib().zb200_decompress_stream_read(self._handle(), out.ctypes.data, avail,
+                                                                        ctypes.byref(m)))
+        return out[:m.value].tobytes()
+
+    def write(self, data):
+        src = _as_u8(data)
+        avail = ctypes.c_size_t(0)
+        _check(self._ctx._h, _native.lib().zb200_decompress_stream_write(self._handle(), src.ctypes.data, src.size,
+                                                                         ctypes.byref(avail)))
+        return self._drain(avail.value)
+
+    def finish(self):
+        avail = ctypes.c_size_t(0)
+        _check(self._ctx._h, _native.lib().zb200_decompress_stream_finish(self._handle(), ctypes.byref(avail)))
+        return self._drain(avail.value)
+
+    def close(self):
+        if self._h:
+            _native.lib().zb200_decompress_stream_free(self._h)
             self._h = ctypes.c_void_p()
 
     def __enter__(self):

@@ -61,6 +61,10 @@ constexpr size_t kHostGroupChunks = 4096;     // host batches: 256 MiB groups so
 // five kernels and a sync.  Of 16 / 64 / 256 MiB, 64 was the fastest at levels 1 and Default on one H100 80GB HBM3
 // at 700 W (tools/bench_compress_stream.py, DESIGN.md section 8 "Compress streams").
 constexpr size_t ZB_STREAM_BATCH_BYTES = 64u << 20;
+// A decompress stream launches once this much compressed payload is pending (tools/bench_decompress_stream.py,
+// DESIGN.md section 8 "Decompress streams"), and one launch produces at most about kDstreamMaxOut bytes.
+constexpr size_t ZB_DSTREAM_BATCH_BYTES = 64u << 20;
+constexpr uint64_t kDstreamMaxOut = 1ull << 30;
 
 }  // namespace
 
@@ -165,6 +169,8 @@ struct zb200_ctx {
   DevBuf in_stage, out_stage, lz2_tables;
   DevBuf carry;             // a compress stream's member carry: [0] in, [1] out
   size_t stream_batch_bytes = ZB_STREAM_BATCH_BYTES;  // pending input at which a stream write launches
+  size_t dstream_batch_bytes = ZB_DSTREAM_BATCH_BYTES;  // pending compressed input at which a decompress stream launches
+  bool dstream_log = false;
   DevBuf seg_src, seg_dst, seg_len, seg_status, seg_kind, seg_expect, seg_cand, skip_mask;  // large-member segments
   DevBuf mark_scratch, mark_segs, seg_bits;  // speculative segments of a large member (uint16 symbols, descriptors)
   DevBuf mark_win;          // window resolve scratch of the joint segments: group window maps (uint16) + incoming windows
@@ -207,6 +213,31 @@ struct zb200_compress_stream {
   ZbMemberCarry carry{0u, 1u, 0ull};  // the input compressed so far: raw CRC-32, Adler-32, bytes
   bool head_done = false, finished = false;
   int err = ZB200_OK;          // a CUDA failure: the stream is unusable
+};
+
+// One member decoded from compressed input that arrives piece by piece.  All of its state is on the host; the
+// kernels run on its ctx's scratch, so any number of streams and other calls can share a ctx.
+struct zb200_decompress_stream {
+  zb200_ctx *ctx = nullptr;
+  int data_format = 0;         // as requested (DETECT too)
+  int fmt = -1;                // the resolved format once the header is decided, -1 before
+  size_t batch_bytes = 0;      // a write launches once this much compressed payload is pending
+  std::vector<uint8_t> in;     // held input: in[in_head ..) are member bytes from in_off on, from a block boundary on
+  size_t in_head = 0;          // in[0 .. in_head) is decoded already (dropped once it is half of the vector)
+  uint64_t in_off = 0;
+  uint32_t bit0 = 0;           // the decode resumes at bit bit0 of in[in_head]
+  uint64_t total_in = 0;       // member bytes written
+  uint8_t tail[8] = {};        // the last 8 member bytes written (the trailer once the input has ended)
+  std::vector<uint8_t> win;    // the last 32 KiB of output in front of the resume point (when base_out > 0)
+  uint64_t base_out = 0;       // output position of the resume point: 0, or >= 32768 (see dstream_run)
+  uint64_t out_total = 0;      // output produced so far (64-bit; gzip ISIZE is compared mod 2^32)
+  uint32_t check = 0;          // CRC-32 (gzip) or Adler-32 (zlib) of that output
+  std::vector<uint8_t> q;      // decoded bytes not read yet: q[q_head ..)
+  size_t q_head = 0;
+  bool done = false;           // the final block is decoded: the rest of the payload is ignored
+  bool finished = false;
+  bool log = false;            // env ZB200_DSTREAM_LOG: one line per launch on stderr (which decode path ran)
+  int err = ZB200_OK;          // once a write or finish failed, every later call reports it
 };
 
 namespace {
@@ -1333,6 +1364,372 @@ int inflate_big_members(zb200_ctx *ctx, const uint8_t *d_src, const uint64_t *sr
   return ZB200_OK;
 }
 
+// ---- decompress streams (zb200_decompress_stream_*) ----
+// The wrapper waits until the input's length can no longer change its verdict: zb_parse_wrapper decides DETECT
+// with len > 18 / len > 6 and checks the gzip header's length against len, so a header is decided once 19 bytes
+// are held and zb_parse_wrapper accepts them, or when it rejects them for anything but their length, or at
+// finish (`final`).  Raw streams start at byte 0 at once.
+int dstream_header(zb200_decompress_stream *st, bool final) {
+  if (st->data_format != ZB200_DF_DEFLATE && !final && st->total_in < 19) return ZB200_OK;
+  uint64_t pos = 0;
+  uint32_t kind = 0, expect = 0, isize = 0;
+  uint8_t dummy = 0;
+  const int r = zb_parse_wrapper(st->in.empty() ? &dummy : st->in.data(), st->in.size(), st->data_format, 0, pos, kind,
+                                 expect, isize);
+  if (r == ZB200_ERR_UNCOMPRESS && !final) return ZB200_OK;   // a gzip header longer than what is held so far
+  if (r) return r;
+  st->fmt = (int)kind;
+  st->check = kind == ZB200_DF_ZLIB ? 1u : 0u;   // Adler-32 / CRC-32 of no bytes
+  st->in.erase(st->in.begin(), st->in.begin() + (ptrdiff_t)pos);
+  st->in_off = pos;
+  st->bit0 = 0;
+  return ZB200_OK;
+}
+
+uint64_t dstream_reserve(const zb200_decompress_stream *st) {
+  return st->fmt == ZB200_DF_GZIP ? 8 : st->fmt == ZB200_DF_ZLIB ? 4 : 0;
+}
+
+// A dynamic block header is at most 14 + 19 * 3 + 320 * 14 bits.  Its decode reads bits past the input as zeros and
+// rejects some headers before it asks whether it ran past the end, so an error in a block that starts less than this
+// before the end of the input received so far is only believed at finish.
+constexpr uint64_t kDstreamHeaderBits = 1024 * 8;
+
+// One launch of a decompress stream (ctx locked): decode the held input from the resume point, bits [bit0, end),
+// where end is the payload received so far (`last`: everything, the trailer included, as uncompress reads it).
+//  1. Boundaries: this library's joints / zlib flushes (k_find_sync), else dynamic-block starts (k_find_blocks),
+//     at least 16 KiB apart.  Segments [b_i, b_i+1) are CLOSED (they must end on the next boundary without a
+//     final block); the last one is OPEN: it stops where the input runs out and says where to resume.
+//  2. A counting pass, then the uint16 marker decode of the segments that fit in kDstreamMaxOut, then the window
+//     resolve with the carried 32 KiB in front of the launch's output (dst = [window | output]).
+//  3. The bytes go to the stream's queue; their checksum is folded into the running one, and the last 32 KiB, the
+//     resume point and the output count are carried, all together once nothing can fail any more.
+// One launch stages at most max(2 x the batching threshold, 64 KiB) of held input (one large write is decoded in
+// several launches, each copying only its own slice); it takes the whole rest only if that slice holds no complete
+// block (`uncapped`).
+// Anything irregular (a closed segment that fails or misses its boundary, a bad marker, a marker before the start of
+// the stream, an error in the open segment of several) redoes the launch as ONE open segment from bit0: the serial
+// decode with the carried window, whose verdict is the reference's.  Until 32 KiB of output exist the resume point
+// stays at the payload start (base_out = 0): a window shorter than 32 KiB would let a distance reach before the
+// stream's start, which only a decode from the start rejects; the bytes already produced are not emitted twice.
+// `progress`: the output or the resume point moved.  Returns a decode status (the stream's verdict) or a CUDA one.
+int dstream_run(zb200_decompress_stream *st, bool last_in, bool &progress, bool uncapped = false) {
+  progress = false;
+  zb200_ctx *ctx = st->ctx;
+  cudaStream_t s = ctx->stream;
+  const uint8_t *held = st->in.data() + st->in_head;
+  const uint64_t held_n = st->in.size() - st->in_head;
+  const uint64_t resv = dstream_reserve(st);
+  uint64_t pay_end = st->total_in - resv > st->in_off ? st->total_in - resv - st->in_off : 0;  // local bytes
+  const uint64_t max_in = std::max<uint64_t>(2 * (uint64_t)st->batch_bytes, 65536);
+  const bool capped = !uncapped && (last_in ? held_n : pay_end) > max_in;
+  bool last = last_in;
+  if (capped) {   // a slice of the input: where it ends is not the end of the input
+    pay_end = max_in;
+    last = false;
+  }
+  const uint64_t dec_end = last ? held_n : pay_end;
+  const uint64_t lo_bit = st->bit0, end_bit = dec_end * 8ull, pay_bit = pay_end * 8ull;
+  if (!last && pay_bit <= lo_bit) return ZB200_OK;
+  const uint64_t min_gap = std::max<uint64_t>(16384ull * 8ull, (pay_bit - std::min(pay_bit, lo_bit)) / 60000ull);
+  ENSURE(ctx->in_stage, dec_end + 64);
+  ENSURE(ctx->counter, 128);
+  const uint8_t *d_src = (const uint8_t *)ctx->in_stage.p;
+  int rc = h2d_copy(ctx, (uint8_t *)ctx->in_stage.p, held, dec_end, s, true);
+  if (rc) return rc;
+  uint32_t *d_cnt = (uint32_t *)ctx->counter.p + 8;
+  uint64_t *d_resume = (uint64_t *)ctx->counter.p + 8;   // bytes 64..79
+  int *d_bad = (int *)((uint32_t *)ctx->counter.p + 12);
+  // 1. boundaries
+  std::vector<uint64_t> bits(1, lo_bit);
+  const char *path = "serial";
+  if (pay_bit > lo_bit + 2 * min_gap) {
+    const uint64_t lo = (lo_bit + 7) / 8;
+    uint32_t cap = (uint32_t)std::min<uint64_t>((pay_end - lo) / 32 + 64, 1u << 24);
+    ENSURE(ctx->seg_cand, (size_t)cap * 8 + 16);
+    uint32_t cnt = 0;
+    CK(zb_launch_find_sync(d_src, lo, pay_end, (uint64_t *)ctx->seg_cand.p, cap, d_cnt, s));
+    CK(cudaMemcpyAsync(&cnt, d_cnt, 4, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    ctx->timing.kernel_launches += 1;
+    std::vector<uint64_t> cand;
+    if (cnt > 0 && cnt <= cap) {
+      cand.resize(cnt);
+      CK(cudaMemcpyAsync(cand.data(), ctx->seg_cand.p, (size_t)cnt * 8, cudaMemcpyDeviceToHost, s));
+      CK(cudaStreamSynchronize(s));
+      std::sort(cand.begin(), cand.end());
+      for (uint64_t c : cand)
+        if (c * 8 >= bits.back() + min_gap && c * 8 < pay_bit) bits.push_back(c * 8);
+      path = "joints";
+    }
+    if (bits.size() < 2) {
+      cap = (uint32_t)std::min<uint64_t>((pay_end - lo) / 64 + 1024, 1u << 24);
+      ENSURE(ctx->seg_cand, (size_t)cap * 8 + 16);
+      CK(zb_launch_find_blocks(d_src, lo_bit, pay_bit, pay_end, (uint64_t *)ctx->seg_cand.p, cap, d_cnt, s));
+      CK(cudaMemcpyAsync(&cnt, d_cnt, 4, cudaMemcpyDeviceToHost, s));
+      CK(cudaStreamSynchronize(s));
+      ctx->timing.kernel_launches += 1;
+      if (cnt > 0 && cnt <= cap) {
+        cand.resize(cnt);
+        CK(cudaMemcpyAsync(cand.data(), ctx->seg_cand.p, (size_t)cnt * 8, cudaMemcpyDeviceToHost, s));
+        CK(cudaStreamSynchronize(s));
+        std::sort(cand.begin(), cand.end());
+        for (uint64_t c : cand)
+          if (c >= bits.back() + min_gap && c + min_gap / 4 < pay_bit) bits.push_back(c);
+        path = "blocks";
+      }
+    }
+    if (bits.size() < 2) path = "serial";
+  }
+  ZbInflateWork w;
+  memset(&w, 0, sizeof(w));
+  w.src = d_src;
+  w.seg_limit = dec_end;
+  w.tabs = ctx->d_tabs;
+  w.data_format = ZB200_DF_DEFLATE;
+  w.seg_mode = 1;
+  w.seg_win0 = st->base_out > 0;
+  std::vector<uint64_t> sl, sb;
+  std::vector<int> sst;
+  std::vector<uint32_t> sk;
+  uint64_t res[2] = {0, 0};
+  // one decode launch over the first n segments, the last of them ending at bit `last_end`: counting with the last
+  // one open, or marker symbols (every segment closed)
+  auto pass = [&](size_t n, bool count, uint64_t last_end) -> int {
+    sb.resize(2 * n);
+    for (size_t i = 0; i < n; i++) {
+      sb[2 * i] = bits[i];
+      sb[2 * i + 1] = i + 1 < n ? bits[i + 1] : last_end;
+    }
+    ENSURE(ctx->seg_bits, 2 * n * 8);
+    ENSURE(ctx->seg_len, n * 8);
+    ENSURE(ctx->seg_status, n * 4);
+    ENSURE(ctx->seg_kind, n * 4);
+    ENSURE(ctx->seg_expect, n * 4);
+    CK(cudaMemcpyAsync(ctx->seg_bits.p, sb.data(), 2 * n * 8, cudaMemcpyHostToDevice, s));
+    res[0] = bits[n - 1];
+    res[1] = 0;
+    if (count) CK(cudaMemcpyAsync(d_resume, res, 16, cudaMemcpyHostToDevice, s));
+    w.seg_bits = (const uint64_t *)ctx->seg_bits.p;
+    w.dst = count ? nullptr : (uint8_t *)ctx->mark_scratch.p;
+    w.dst_off = (const uint64_t *)ctx->seg_dst.p;
+    w.out_len = (uint64_t *)ctx->seg_len.p;
+    w.status = (int *)ctx->seg_status.p;
+    w.expect = (uint32_t *)ctx->seg_expect.p;
+    w.kind = (uint32_t *)ctx->seg_kind.p;
+    w.counter = (uint32_t *)ctx->counter.p + 4;
+    w.n = (uint32_t)n;
+    w.count_only = count ? 1 : 0;
+    w.mark = count ? 0 : 1;
+    w.resume = count ? d_resume : nullptr;
+    CK(zb_launch_inflate(w, s));
+    sl.resize(n);
+    sst.resize(n);
+    sk.resize(n);
+    CK(cudaMemcpyAsync(sl.data(), ctx->seg_len.p, n * 8, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(sst.data(), ctx->seg_status.p, n * 4, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(sk.data(), ctx->seg_kind.p, n * 4, cudaMemcpyDeviceToHost, s));
+    if (count) CK(cudaMemcpyAsync(res, d_resume, 16, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    ctx->timing.kernel_launches += 1;
+    return ZB200_OK;
+  };
+  // The open segment decodes up to lim_bit: the input's end, or (once) less of it when one serial segment would
+  // produce more than kDstreamMaxOut (DEFLATE expands at most 1032:1, so 1 MiB of input stays near the bound).
+  uint64_t lim_bit = end_bit;
+  bool lim_last = last, cut = false;
+  const uint64_t cut_bits = 8ull * (kDstreamMaxOut / 1032);
+  for (;;) {
+    const size_t S = bits.size();
+    // 2. the counting pass
+    rc = pass(S, true, lim_bit);
+    if (rc) return rc;
+    bool irregular = false;
+    for (size_t i = 0; i + 1 < S; i++)
+      irregular = irregular || sst[i] != ZB200_OK || sk[i] != 0 || sl[i] > 0xf0000000ull;
+    // the open segment: its complete output, where it stopped, whether that was the final block
+    uint64_t open_n = 0, open_stop = 0;
+    bool open_fin = false;
+    if (!irregular) {
+      const int os = sst[S - 1];
+      int err = ZB200_OK;
+      if (os == ZB200_OK) {
+        open_fin = sk[S - 1] != 0;
+        open_n = sl[S - 1];
+        open_stop = lim_bit;   // not final: the input is used up at a block boundary
+        if (!open_fin && lim_last) err = ZB200_ERR_END_OF_BUFFER;   // the reference reads one more block header
+      } else {
+        open_n = res[1];
+        open_stop = res[0];
+        const bool ran_out = os == ZB200_ERR_DST_TOO_SMALL || (os == ZB200_ERR_END_OF_BUFFER && !lim_last) ||
+                             (!lim_last && lim_bit - std::min(lim_bit, res[0]) < kDstreamHeaderBits);
+        if (!ran_out) err = os;
+      }
+      if (err) {
+        if (S == 1) return err;
+        irregular = true;
+      }
+    }
+    if (irregular) {
+      if (S == 1) return ZB200_ERR_UNCOMPRESS;
+      bits.resize(1);
+      path = "fallback";
+      continue;
+    }
+    if (S == 1 && !cut && open_n > kDstreamMaxOut && lim_bit > lo_bit + cut_bits) {
+      cut = true;
+      lim_bit = lo_bit + cut_bits;
+      lim_last = false;
+      continue;
+    }
+    if (S == 1 && cut && lim_bit != end_bit && open_stop == lo_bit && !open_fin) {   // one block longer than that
+      lim_bit = end_bit;
+      lim_last = last;
+      continue;
+    }
+    // 3. what fits in one launch's output: whole segments, the first one always
+    std::vector<uint64_t> size(S);
+    for (size_t i = 0; i + 1 < S; i++) size[i] = sl[i];
+    size[S - 1] = open_n;
+    size_t T = 0;
+    uint64_t tot = 0;
+    while (T < S && (T == 0 || tot + size[T] <= kDstreamMaxOut)) tot += size[T++];
+    const bool with_open = T == S;
+    const uint64_t stop = with_open ? open_stop : bits[T];
+    const bool fin = with_open && open_fin;
+    // 4. marker decode of segments [0, T), all closed now, into [32768 markers | output] each
+    std::vector<ZbMarkSegHost> segs(T);
+    std::vector<uint64_t> dof(T + 1);
+    const uint64_t W = st->base_out > 0 ? 32768 : 0;
+    uint64_t se = 0, de = W;
+    for (size_t i = 0; i < T; i++) {
+      se += 32768ull;
+      segs[i].scr = se;
+      segs[i].dst = de;
+      segs[i].n = (uint32_t)size[i];
+      segs[i].pad = 0;
+      dof[i] = se;
+      se += size[i];
+      de += size[i];
+    }
+    dof[T] = se;
+    ENSURE(ctx->mark_scratch, (size_t)se * 2 + 64);
+    ENSURE(ctx->mark_segs, T * sizeof(ZbMarkSegHost) + 16);
+    ENSURE(ctx->seg_dst, (T + 1) * 8);
+    CK(cudaMemcpyAsync(ctx->seg_dst.p, dof.data(), (T + 1) * 8, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(ctx->mark_segs.p, segs.data(), T * sizeof(ZbMarkSegHost), cudaMemcpyHostToDevice, s));
+    CK(zb_launch_mark_prefill((uint16_t *)ctx->mark_scratch.p, ctx->mark_segs.p, (uint32_t)T, s));
+    ctx->timing.kernel_launches += 1;
+    rc = pass(T, false, fin ? lim_bit : stop);
+    if (rc) return rc;
+    for (size_t i = 0; i < T && !irregular; i++)
+      irregular = sst[i] != ZB200_OK || sl[i] != size[i] || (sk[i] != 0) != (fin && i + 1 == T);
+    if (irregular) {
+      if (S == 1) return ZB200_ERR_UNCOMPRESS;
+      bits.resize(1);
+      path = "fallback";
+      continue;
+    }
+    uint64_t total = 0;
+    for (size_t i = 0; i < T; i++) total += segs[i].n;
+    // 5. resolve against the carried window in front of the output
+    ENSURE(ctx->out_stage, W + total + 64);
+    uint8_t *d_out = (uint8_t *)ctx->out_stage.p;
+    if (W) CK(cudaMemcpyAsync(d_out, st->win.data(), W, cudaMemcpyHostToDevice, s));
+    CK(cudaMemsetAsync(d_bad, 0, 4, s));
+    uint32_t max_n = 0;
+    for (size_t i = 0; i < T; i++) max_n = std::max(max_n, segs[i].n);
+    const uint32_t gsz = std::max<uint32_t>(1u, (uint32_t)std::ceil(std::sqrt((double)T)));
+    const size_t ngroups = (T + gsz - 1) / gsz;
+    ENSURE(ctx->mark_win, ngroups * 32768ull * 3);
+    CK(zb_launch_resolve_groups((uint16_t *)ctx->mark_scratch.p, ctx->mark_segs.p, (uint32_t)T, max_n, gsz, 0, W,
+                                (uint16_t *)ctx->mark_win.p, (uint8_t *)ctx->mark_win.p + ngroups * 65536ull, d_out,
+                                d_bad, s));
+    ctx->timing.kernel_launches += 4;
+    int bad = 0;
+    CK(cudaMemcpyAsync(&bad, d_bad, 4, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    if (bad) {
+      if (S == 1) return ZB200_ERR_UNCOMPRESS;
+      bits.resize(1);
+      path = "fallback";
+      continue;
+    }
+    // 6. emit what was not emitted before, fold its checksum in, carry the window and the resume point
+    const uint64_t skip = st->out_total - st->base_out;
+    const uint64_t fresh = total > skip ? total - skip : 0;
+    uint32_t check = st->check;
+    if (fresh && st->fmt != ZB200_DF_DEFLATE) {
+      const uint64_t offs[2] = {0, fresh};
+      ZbChecksumWork cw;
+      memset(&cw, 0, sizeof(cw));
+      rc = upload_pieces(ctx, offs, 1, cw);
+      if (rc) return rc;
+      ENSURE(ctx->src_off, 16);
+      ENSURE(ctx->ck_out, 4);
+      CK(cudaMemcpyAsync(ctx->src_off.p, offs, 16, cudaMemcpyHostToDevice, s));
+      cw.src = d_out + W + skip;
+      cw.off = (const uint64_t *)ctx->src_off.p;
+      cw.out = (uint32_t *)ctx->ck_out.p;
+      cw.kind = st->fmt == ZB200_DF_ZLIB ? 1 : 0;
+      CK(zb_launch_checksum(cw, s));
+      uint32_t c = 0;
+      CK(cudaMemcpyAsync(&c, ctx->ck_out.p, 4, cudaMemcpyDeviceToHost, s));
+      CK(cudaStreamSynchronize(s));
+      ctx->timing.kernel_launches += 2;
+      check = st->fmt == ZB200_DF_ZLIB ? zb_adler32_combine(check, c, fresh) : zb_crc32_combine(check, c, fresh);
+    }
+    const uint64_t new_base = st->base_out + total;
+    const bool advance = fin || new_base >= 32768;
+    std::vector<uint8_t> nwin;
+    if (advance && !fin) nwin.resize(std::min<uint64_t>(32768, W + total));
+    const size_t q0 = st->q.size();
+    if (fresh) {
+      if (st->q_head && st->q_head * 2 >= q0) {   // drop what was read
+        st->q.erase(st->q.begin(), st->q.begin() + (ptrdiff_t)st->q_head);
+        st->q_head = 0;
+      }
+      st->q.resize(st->q.size() + fresh);   // (a failure from here on is the stream's error: the bytes are never read)
+      rc = d2h_copy(ctx, st->q.data() + (st->q.size() - fresh), d_out + W + skip, fresh, s, true);
+      if (rc) return rc;
+    }
+    if (!nwin.empty())
+      CK(cudaMemcpyAsync(nwin.data(), d_out + W + total - nwin.size(), nwin.size(), cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    rc = d2h_flush(ctx);
+    if (rc) return rc;
+    // nothing can fail from here on: commit the launch
+    ctx->timing.d2h_bytes += fresh;
+    if (st->log)
+      fprintf(stderr, "zb200 dstream: path=%s segs=%zu taken=%zu out=%llu final=%d\n", path, S, T,
+              (unsigned long long)total, (int)fin);
+    progress = fresh > 0 || (advance && stop > lo_bit) || fin;
+    if (capped && !progress) return dstream_run(st, last_in, progress, true);   // no complete block in the slice
+    st->check = check;
+    st->out_total = std::max(st->out_total, new_base);
+    if (fin) {
+      st->done = true;
+      std::vector<uint8_t>().swap(st->in);
+      std::vector<uint8_t>().swap(st->win);
+      st->in_head = 0;
+      st->in_off = st->total_in;
+      st->bit0 = 0;
+      st->base_out = new_base;
+    } else if (advance) {
+      st->in_head += stop / 8;
+      if (st->in_head * 2 >= st->in.size()) {   // drop the decoded input: amortised, one large write is not moved per launch
+        st->in.erase(st->in.begin(), st->in.begin() + (ptrdiff_t)st->in_head);
+        st->in_head = 0;
+      }
+      st->in_off += stop / 8;
+      st->bit0 = (uint32_t)(stop & 7);
+      st->base_out = new_base;
+      st->win.swap(nwin);
+    }
+    return ZB200_OK;
+  }
+}
+
 // Work-queue order of one inflate launch: a member is decoded by one 8-lane group from start to end,
 // so a long member that is fetched late finishes long after everything else (the tail of the launch).
 // Members much longer than the average go first, longest first; the rest keep their order.
@@ -1880,6 +2277,11 @@ int zb200_init(int device, zb200_ctx **out) {
     long long v = atoll(e);
     if (v > 0) ctx->stream_batch_bytes = (size_t)v;
   }
+  if (const char *e = getenv("ZB200_DSTREAM_BATCH_BYTES")) {  // test hook: decompress streams launch at this much pending input
+    long long v = atoll(e);
+    if (v > 0) ctx->dstream_batch_bytes = (size_t)v;
+  }
+  if (const char *e = getenv("ZB200_DSTREAM_LOG")) ctx->dstream_log = atoi(e) != 0;  // test hook: the decode path of every launch
   if (const char *e = getenv("ZB200_BIG_MEMBER_BYTES")) {  // test hook: segment path for small members too
     long long v = atoll(e);
     if (v > 0) {
@@ -2152,6 +2554,128 @@ int zb200_compress_stream_finish(zb200_compress_stream *st, uint8_t *dst, size_t
 }
 
 void zb200_compress_stream_free(zb200_compress_stream *st) { delete st; }
+
+// ---- decompress streams ----
+int zb200_decompress_stream_begin(zb200_ctx *ctx, int data_format, zb200_decompress_stream **out) {
+  return guarded(ctx, [&]() -> int {
+    if (!ctx || !out) return ZB200_ERR_ARG;
+    *out = nullptr;
+    if (data_format < ZB200_DF_DETECT || data_format > ZB200_DF_DEFLATE) return ZB200_ERR_INVALID_FORMAT;
+    zb200_decompress_stream *st = new zb200_decompress_stream();
+    st->ctx = ctx;
+    st->data_format = data_format;
+    {
+      std::lock_guard<std::mutex> lk(ctx->mu);
+      st->batch_bytes = ctx->dstream_batch_bytes;
+      st->log = ctx->dstream_log;
+    }
+    if (data_format == ZB200_DF_DEFLATE) dstream_header(st, false);
+    *out = st;
+    return ZB200_OK;
+  });
+}
+
+static size_t dstream_avail(const zb200_decompress_stream *st) { return st->q.size() - st->q_head; }
+
+int zb200_decompress_stream_write(zb200_decompress_stream *st, const uint8_t *src, size_t len, size_t *avail) {
+  if (!st) return ZB200_ERR_ARG;
+  zb200_ctx *ctx = st->ctx;
+  bool entered = false;   // past the argument checks: any failure (a host allocation too) is the stream's error
+  const int rc = guarded(ctx, [&]() -> int {
+    if (len && !src) return ZB200_ERR_ARG;
+    if (avail) *avail = 0;
+    if (st->err) return st->err;
+    if (st->finished) return ZB200_ERR_ARG;
+    entered = true;
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    DeviceGuard g(ctx->device);
+    memset(&ctx->timing, 0, sizeof(ctx->timing));
+    // the member's last 8 bytes (its trailer, if this is the end), then the input itself unless the payload is over
+    for (size_t i = len > 8 ? len - 8 : 0; i < len; i++) {
+      memmove(st->tail, st->tail + 1, 7);
+      st->tail[7] = src[i];
+    }
+    st->total_in += len;
+    if (!st->done) st->in.insert(st->in.end(), src, src + len);
+    int rc = ZB200_OK;
+    if (st->fmt < 0) rc = dstream_header(st, false);
+    while (!rc && st->fmt >= 0 && !st->done) {
+      const uint64_t resv = dstream_reserve(st), held = st->in_off + resv;
+      const uint64_t pending = st->total_in > held ? st->total_in - held : 0;
+      if (pending < st->batch_bytes || pending * 8 <= st->bit0) break;
+      bool progress = false;
+      rc = dstream_run(st, false, progress);
+      if (!progress) break;
+    }
+    if (!rc && avail) *avail = dstream_avail(st);
+    return rc;
+  });
+  if (rc && entered) {
+    st->err = rc;
+    if (avail) *avail = 0;
+  }
+  return rc;
+}
+
+int zb200_decompress_stream_finish(zb200_decompress_stream *st, size_t *avail) {
+  if (!st) return ZB200_ERR_ARG;
+  zb200_ctx *ctx = st->ctx;
+  bool entered = false;   // as in zb200_decompress_stream_write
+  const int rc = guarded(ctx, [&]() -> int {
+    if (avail) *avail = 0;
+    if (st->err) return st->err;
+    if (st->finished) return ZB200_ERR_ARG;
+    entered = true;
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    DeviceGuard g(ctx->device);
+    memset(&ctx->timing, 0, sizeof(ctx->timing));
+    int rc = st->fmt < 0 ? dstream_header(st, true) : ZB200_OK;
+    while (!rc && !st->done) {
+      bool progress = false;
+      rc = dstream_run(st, true, progress);
+      if (!rc && !progress && !st->done) rc = ZB200_ERR_UNCOMPRESS;
+    }
+    // the trailer, checksum then size (gzip.nim:80-88, zippy.nim:154-162)
+    if (!rc && st->fmt == ZB200_DF_GZIP) {
+      if (zb_ld_le32(st->tail) != st->check) rc = ZB200_ERR_CHECKSUM;
+      else if (zb_ld_le32(st->tail + 4) != (uint32_t)st->out_total) rc = ZB200_ERR_SIZE;
+    } else if (!rc && st->fmt == ZB200_DF_ZLIB) {
+      const uint8_t *t = st->tail + 4;
+      const uint32_t expect = ((uint32_t)t[0] << 24) | ((uint32_t)t[1] << 16) | ((uint32_t)t[2] << 8) | t[3];
+      if (expect != st->check) rc = ZB200_ERR_CHECKSUM;
+    }
+    if (rc) return rc;
+    st->finished = true;
+    std::vector<uint8_t>().swap(st->in);
+    std::vector<uint8_t>().swap(st->win);
+    st->in_head = 0;
+    if (avail) *avail = dstream_avail(st);
+    return ZB200_OK;
+  });
+  if (rc && entered) {
+    st->err = rc;
+    if (avail) *avail = 0;
+  }
+  return rc;
+}
+
+int zb200_decompress_stream_read(zb200_decompress_stream *st, uint8_t *dst, size_t dst_cap, size_t *dst_len) {
+  if (!st || !dst_len) return ZB200_ERR_ARG;
+  *dst_len = 0;
+  if (st->err) return st->err;
+  const size_t n = std::min(dst_cap, dstream_avail(st));
+  if (n && !dst) return ZB200_ERR_ARG;
+  if (n) memcpy(dst, st->q.data() + st->q_head, n);
+  st->q_head += n;
+  if (st->q_head == st->q.size()) {
+    st->q.clear();
+    st->q_head = 0;
+  }
+  *dst_len = n;
+  return ZB200_OK;
+}
+
+void zb200_decompress_stream_free(zb200_decompress_stream *st) { delete st; }
 
 // second half of the sharded path: once the size exchange has told a rank where its shard lands in
 // the concatenated stream, its device-resident members go straight to that place in host memory

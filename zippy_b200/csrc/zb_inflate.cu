@@ -831,6 +831,13 @@ __global__ void __launch_bounds__(INF_THREADS, INF_MIN_CTAS)
       fin = true;  // the segment's input is used up at a block boundary
       done = ZB_OK;
     } else if (g.st == ST_BLOCK) {
+      if (COUNT_ONLY && w.resume && g.idx + 1u == w.n && lane == 0) {
+        // the open segment of a decompress stream: where it resumes if this block does not complete.  (A segment
+        // whose input is used up at a block boundary ends in the branch above, with status ZB_OK: it resumes there.
+        // The marker pass decodes that segment again as a closed one, up to the block boundary found here.)
+        w.resume[0] = (uint64_t)(reinterpret_cast<const uint8_t *>(g.b.gbase) - w.src) * 8ull + br_consumed_abs(g.b);
+        w.resume[1] = g.op;
+      }
       int r = begin_block<COUNT_ONLY, OutT>(g, gs);
       if (r >= 0) {
         fin = true;

@@ -114,6 +114,12 @@ struct ZbInflateWork {
   const uint32_t *gate_ready;  // device word
   uint32_t *gate_done;         // device [n_gates], zeroed before the launch
   uint32_t n_gates;
+  // With seg_bits and count_only: null, or device [2] -- the last segment (n - 1) is then OPEN, the input a
+  // decompress stream has received so far.  At every block start of that segment its lane 0 stores the block's
+  // absolute bit position in src ([0]) and the segment's output count there ([1]).  When the segment stops with
+  // ZB_ERR_END_OF_BUFFER (the input ran out) or ZB_ERR_DST_TOO_SMALL (the count ran out), its output up to [1] is
+  // complete and the stream resumes decoding at bit [0].
+  uint64_t *resume;
 };
 cudaError_t zb_launch_inflate(const ZbInflateWork &w, cudaStream_t s);
 // positions just past every byte sequence 00 00 ff ff (the empty stored block that byte-aligns a
