@@ -166,12 +166,28 @@ int zb200_checksum_batch(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t
  *  - A write or finish after finish: ZB200_ERR_ARG.  ZB200_ERR_DST_TOO_SMALL consumes nothing and leaves the
  *    stream as it was: retry with bound() bytes.  After a CUDA failure every later call reports it.
  *  - Members of 4 GiB and more work: the byte count is 64-bit, gzip ISIZE is the total mod 2^32.
+ *  - flush(st, mode): emit everything written so far (the header too if it has not gone out), so that every byte
+ *    written can be decoded from what has been emitted.  mode is ZB200_SYNC_FLUSH or ZB200_FULL_FLUSH (zlib's
+ *    Z_SYNC_FLUSH / Z_FULL_FLUSH); anything else, or a flush after finish: ZB200_ERR_ARG.  The flush offsets cut
+ *    the member into flush segments, each cut into 64 KiB chunks from its own start; a segment's last chunk may be
+ *    short and ends, like every chunk but the member's last, in the byte-aligning empty stored block 00 00 ff ff.
+ *    Levels -1 and 2..9 see min(32 KiB, bytes since the member start or the last FULL flush) of history: a sync
+ *    flush keeps the history, a full flush drops it (no match reaches back across it, and a raw inflater started
+ *    right after it decodes the rest).  Levels 0, 1 and -2 have no history, so both modes write the same bytes.
+ *    The member's bytes depend only on the input, the flush offsets and modes, level, format and fname_len --
+ *    never on the write sizes or the batching threshold.  Without a flush, or with sync flushes only at multiples
+ *    of 64 KiB, they are compress_batch's bytes.  A flush with nothing written since the last flush (or begin)
+ *    emits nothing and changes nothing; finish right after a flush writes the empty final block (03 00, at
+ *    level 0 the empty stored block) and the trailer.  bound(st, 0) also bounds what a flush emits;
+ *    ZB200_ERR_DST_TOO_SMALL and CUDA failures behave as for write.
  *  - free: at any time, finished or not. */
+enum { ZB200_SYNC_FLUSH = 2, ZB200_FULL_FLUSH = 3 };
 typedef struct zb200_compress_stream zb200_compress_stream;
 int zb200_compress_stream_begin(zb200_ctx *ctx, int level, int data_format, int fname_len, zb200_compress_stream **out);
 size_t zb200_compress_stream_bound(const zb200_compress_stream *st, size_t len);
 int zb200_compress_stream_write(zb200_compress_stream *st, const uint8_t *src, size_t len,
                                 uint8_t *dst, size_t dst_cap, size_t *dst_len);
+int zb200_compress_stream_flush(zb200_compress_stream *st, int mode, uint8_t *dst, size_t dst_cap, size_t *dst_len);
 int zb200_compress_stream_finish(zb200_compress_stream *st, uint8_t *dst, size_t dst_cap, size_t *dst_len);
 void zb200_compress_stream_free(zb200_compress_stream *st);
 
@@ -201,11 +217,20 @@ void zb200_compress_stream_free(zb200_compress_stream *st);
  *    tools/bench_decompress_stream.py); smaller writes are only buffered.  One launch reads at most twice that much
  *    input and produces at most about 1 GiB (more only when a single block is larger); a large write is decoded by
  *    as many launches as it needs before it returns.
- *  - Decoded bytes stay in the stream until read: read after every write.
+ *  - drain decodes now, whatever the batching threshold, every block that is complete in the input received so
+ *    far, and *avail (may be NULL) receives the bytes waiting to be read.  A block that ends inside the bytes held
+ *    back as the possible trailer counts too, so after a sender's sync or full flush (this library's, zlib's) a
+ *    drain yields everything written up to it.  If the input does end there, the member has no final block
+ *    before its trailer and finish reports uncompress's error.  Before the header is decided (19 member bytes,
+ *    and for gzip the whole header and 9 bytes more) drain decodes nothing.  As for write, an error in a block that starts
+ *    less than 1 KiB before the end of the input so far is only believed at finish.  drain after finish:
+ *    ZB200_ERR_ARG; a failure is the stream's error, as for write.
+ *  - Decoded bytes stay in the stream until read: read after every write or drain.
  *  - free: at any time, finished or not. */
 typedef struct zb200_decompress_stream zb200_decompress_stream;
 int zb200_decompress_stream_begin(zb200_ctx *ctx, int data_format, zb200_decompress_stream **out);
 int zb200_decompress_stream_write(zb200_decompress_stream *st, const uint8_t *src, size_t len, size_t *avail);
+int zb200_decompress_stream_drain(zb200_decompress_stream *st, size_t *avail);
 int zb200_decompress_stream_finish(zb200_decompress_stream *st, size_t *avail);
 int zb200_decompress_stream_read(zb200_decompress_stream *st, uint8_t *dst, size_t dst_cap, size_t *dst_len);
 void zb200_decompress_stream_free(zb200_decompress_stream *st);

@@ -217,6 +217,15 @@ class CompressStream {
     return out;
   }
   std::string write(const std::string &data) { return write(data.data(), data.size()); }
+  // Emit everything written so far (ZB200_SYNC_FLUSH keeps the history, ZB200_FULL_FLUSH drops it): the
+  // bytes returned so far decode to the bytes written so far.  "" when nothing was written since the last flush.
+  std::string flush(int mode = ZB200_SYNC_FLUSH) {
+    std::string out(zb200_compress_stream_bound(st_, 0), '\0');
+    size_t n = 0;
+    detail::check(zb200_compress_stream_flush(st_, mode, reinterpret_cast<uint8_t *>(&out[0]), out.size(), &n));
+    out.resize(n);
+    return out;
+  }
   std::string finish() {
     std::string out(zb200_compress_stream_bound(st_, 0), '\0');
     size_t n = 0;
@@ -245,17 +254,24 @@ class DecompressStream {
   std::string write(const void *src, size_t len) {
     size_t avail = 0;
     detail::check(zb200_decompress_stream_write(st_, static_cast<const uint8_t *>(src), len, &avail));
-    return drain(avail);
+    return take(avail);
   }
   std::string write(const std::string &data) { return write(data.data(), data.size()); }
+  // Decode every block that is complete in the input so far, whatever the batching threshold: after a sender's
+  // flush, everything it wrote up to the flush.
+  std::string drain() {
+    size_t avail = 0;
+    detail::check(zb200_decompress_stream_drain(st_, &avail));
+    return take(avail);
+  }
   std::string finish() {
     size_t avail = 0;
     detail::check(zb200_decompress_stream_finish(st_, &avail));
-    return drain(avail);
+    return take(avail);
   }
 
  private:
-  std::string drain(size_t avail) {
+  std::string take(size_t avail) {
     std::string out(avail, '\0');
     size_t n = 0;
     detail::check(zb200_decompress_stream_read(st_, reinterpret_cast<uint8_t *>(&out[0]), out.size(), &n));

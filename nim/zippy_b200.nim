@@ -249,9 +249,15 @@ proc zb200_compress_stream_begin(ctx: Zb200Ctx, level, dataFormat, fnameLen: cin
 proc zb200_compress_stream_bound(st: Zb200CompressStream, len: csize_t): csize_t {.importc, cdecl, dynlib: lib.}
 proc zb200_compress_stream_write(st: Zb200CompressStream, src: pointer, len: csize_t, dst: pointer, dstCap: csize_t,
                                  dstLen: ptr csize_t): cint {.importc, cdecl, dynlib: lib.}
+proc zb200_compress_stream_flush(st: Zb200CompressStream, mode: cint, dst: pointer, dstCap: csize_t,
+                                 dstLen: ptr csize_t): cint {.importc, cdecl, dynlib: lib.}
 proc zb200_compress_stream_finish(st: Zb200CompressStream, dst: pointer, dstCap: csize_t,
                                   dstLen: ptr csize_t): cint {.importc, cdecl, dynlib: lib.}
 proc zb200_compress_stream_free(st: Zb200CompressStream) {.importc, cdecl, dynlib: lib.}
+
+const
+  SyncFlush* = 2   ## zlib's Z_SYNC_FLUSH: emit everything written, keep the history
+  FullFlush* = 3   ## zlib's Z_FULL_FLUSH: emit everything written, drop the history
 
 type CompressStream* = object
   st: Zb200CompressStream
@@ -276,6 +282,13 @@ proc write*(s: var CompressStream, data: string): string {.raises: [ZippyError].
   check zb200_compress_stream_write(s.st, data.cstring, data.len.csize_t, result[0].addr, result.len.csize_t, n.addr)
   result.setLen(n.int)
 
+proc flush*(s: var CompressStream, mode = SyncFlush): string {.raises: [ZippyError].} =
+  ## everything written so far; "" when nothing was written since the last flush
+  result = newString(zb200_compress_stream_bound(s.st, 0).int + 1)
+  var n: csize_t
+  check zb200_compress_stream_flush(s.st, mode.cint, result[0].addr, result.len.csize_t, n.addr)
+  result.setLen(n.int)
+
 proc finish*(s: var CompressStream): string {.raises: [ZippyError].} =
   result = newString(zb200_compress_stream_bound(s.st, 0).int + 1)
   var n: csize_t
@@ -295,6 +308,7 @@ proc zb200_decompress_stream_begin(ctx: Zb200Ctx, dataFormat: cint,
                                    st: ptr Zb200DecompressStream): cint {.importc, cdecl, dynlib: lib.}
 proc zb200_decompress_stream_write(st: Zb200DecompressStream, src: pointer, len: csize_t,
                                    avail: ptr csize_t): cint {.importc, cdecl, dynlib: lib.}
+proc zb200_decompress_stream_drain(st: Zb200DecompressStream, avail: ptr csize_t): cint {.importc, cdecl, dynlib: lib.}
 proc zb200_decompress_stream_finish(st: Zb200DecompressStream, avail: ptr csize_t): cint {.importc, cdecl, dynlib: lib.}
 proc zb200_decompress_stream_read(st: Zb200DecompressStream, dst: pointer, dstCap: csize_t,
                                   dstLen: ptr csize_t): cint {.importc, cdecl, dynlib: lib.}
@@ -306,7 +320,7 @@ type DecompressStream* = object
 proc newDecompressStream*(dataFormat = dfDetect): DecompressStream {.raises: [ZippyError].} =
   check zb200_decompress_stream_begin(getCtx(), dataFormat.cint, result.st.addr)
 
-proc drain(s: var DecompressStream, avail: csize_t): string {.raises: [ZippyError].} =
+proc take(s: var DecompressStream, avail: csize_t): string {.raises: [ZippyError].} =
   result = newString(avail.int + 1)
   var n: csize_t
   check zb200_decompress_stream_read(s.st, result[0].addr, avail, n.addr)
@@ -316,12 +330,18 @@ proc write*(s: var DecompressStream, data: string): string {.raises: [ZippyError
   ## small writes are gathered on the host and return ""
   var avail: csize_t
   check zb200_decompress_stream_write(s.st, data.cstring, data.len.csize_t, avail.addr)
-  s.drain(avail)
+  s.take(avail)
+
+proc drain*(s: var DecompressStream): string {.raises: [ZippyError].} =
+  ## every block complete in the input so far: after a sender's flush, everything written up to it
+  var avail: csize_t
+  check zb200_decompress_stream_drain(s.st, avail.addr)
+  s.take(avail)
 
 proc finish*(s: var DecompressStream): string {.raises: [ZippyError].} =
   var avail: csize_t
   check zb200_decompress_stream_finish(s.st, avail.addr)
-  s.drain(avail)
+  s.take(avail)
 
 proc close*(s: var DecompressStream) =
   if s.st != nil:

@@ -26,12 +26,14 @@ from . import _native
 dfDetect, dfZlib, dfGzip, dfDeflate = 0, 1, 2, 3                       # common.nim:4-5
 NoCompression, BestSpeed, BestCompression = 0, 1, 9                    # common.nim:7-12
 DefaultCompression, HuffmanOnly = -1, -2
+SyncFlush, FullFlush = 2, 3                                            # zlib's Z_SYNC_FLUSH / Z_FULL_FLUSH
 
 __all__ = ["compress", "uncompress", "crc32", "adler32", "deflate", "inflate", "compress_batch", "uncompress_batch",
            "uncompressed_sizes", "checksum_batch", "ZippyError", "Context", "CompressStream", "DecompressStream",
            "MultiGpu", "dfDetect",
            "dfZlib", "dfGzip",
-           "dfDeflate", "NoCompression", "BestSpeed", "BestCompression", "DefaultCompression", "HuffmanOnly"]
+           "dfDeflate", "NoCompression", "BestSpeed", "BestCompression", "DefaultCompression", "HuffmanOnly",
+           "SyncFlush", "FullFlush"]
 
 
 class ZippyError(Exception):
@@ -348,6 +350,15 @@ class CompressStream:
                                                                        out.size, ctypes.byref(m)))
         return out[:m.value].tobytes()
 
+    def flush(self, mode=SyncFlush):
+        """Emit everything written so far: what the stream has returned decodes to everything written.  SyncFlush
+        keeps the compression history, FullFlush drops it so a raw inflater can start right after.  Returns b""
+        when nothing was written since the last flush (zlib's Z_SYNC_FLUSH / Z_FULL_FLUSH)."""
+        out, m = self._out(0)
+        _check(self._ctx._h, _native.lib().zb200_compress_stream_flush(self._h, mode, out.ctypes.data, out.size,
+                                                                       ctypes.byref(m)))
+        return out[:m.value].tobytes()
+
     def finish(self):
         out, m = self._out(0)
         _check(self._ctx._h, _native.lib().zb200_compress_stream_finish(self._h, out.ctypes.data, out.size,
@@ -388,7 +399,7 @@ class DecompressStream:
             raise ZippyError(22, "the stream is closed")
         return self._h
 
-    def _drain(self, avail):
+    def _take(self, avail):
         out = np.empty(avail, dtype=np.uint8)
         m = ctypes.c_size_t(0)
         _check(self._ctx._h, _native.lib().zb200_decompress_stream_read(self._handle(), out.ctypes.data, avail,
@@ -400,12 +411,20 @@ class DecompressStream:
         avail = ctypes.c_size_t(0)
         _check(self._ctx._h, _native.lib().zb200_decompress_stream_write(self._handle(), src.ctypes.data, src.size,
                                                                          ctypes.byref(avail)))
-        return self._drain(avail.value)
+        return self._take(avail.value)
+
+    def drain(self):
+        """Decode every block that is complete in the input so far, whatever the batching threshold: after a
+        sender's flush, everything it wrote up to the flush -- once the header is decided: raw streams at once,
+        otherwise after 19 member bytes and, for gzip, the whole header and 9 bytes more."""
+        avail = ctypes.c_size_t(0)
+        _check(self._ctx._h, _native.lib().zb200_decompress_stream_drain(self._handle(), ctypes.byref(avail)))
+        return self._take(avail.value)
 
     def finish(self):
         avail = ctypes.c_size_t(0)
         _check(self._ctx._h, _native.lib().zb200_decompress_stream_finish(self._handle(), ctypes.byref(avail)))
-        return self._drain(avail.value)
+        return self._take(avail.value)
 
     def close(self):
         if self._h:

@@ -59,10 +59,12 @@ SYMBOLS = {
     "zb200_compress_stream_begin": (c_int, [ctypes.c_void_p, c_int, c_int, c_int, ctypes.POINTER(ctypes.c_void_p)]),
     "zb200_compress_stream_bound": (c_size_t, [ctypes.c_void_p, c_size_t]),
     "zb200_compress_stream_write": (c_int, [ctypes.c_void_p, c_u8p, c_size_t, c_u8p, c_size_t, ctypes.POINTER(c_size_t)]),
+    "zb200_compress_stream_flush": (c_int, [ctypes.c_void_p, c_int, c_u8p, c_size_t, ctypes.POINTER(c_size_t)]),
     "zb200_compress_stream_finish": (c_int, [ctypes.c_void_p, c_u8p, c_size_t, ctypes.POINTER(c_size_t)]),
     "zb200_compress_stream_free": (None, [ctypes.c_void_p]),
     "zb200_decompress_stream_begin": (c_int, [ctypes.c_void_p, c_int, ctypes.POINTER(ctypes.c_void_p)]),
     "zb200_decompress_stream_write": (c_int, [ctypes.c_void_p, c_u8p, c_size_t, ctypes.POINTER(c_size_t)]),
+    "zb200_decompress_stream_drain": (c_int, [ctypes.c_void_p, ctypes.POINTER(c_size_t)]),
     "zb200_decompress_stream_finish": (c_int, [ctypes.c_void_p, ctypes.POINTER(c_size_t)]),
     "zb200_decompress_stream_read": (c_int, [ctypes.c_void_p, c_u8p, c_size_t, ctypes.POINTER(c_size_t)]),
     "zb200_decompress_stream_free": (None, [ctypes.c_void_p]),

@@ -208,8 +208,9 @@ struct zb200_compress_stream {
   int level = 0, data_format = 0;
   uint8_t fname_len = 0;
   size_t batch_bytes = 0;      // launch once this much input is pending
-  std::vector<uint8_t> buf;    // [history | pending input]: pending starts at a chunk boundary of the member
-  size_t hist = 0;             // bytes of history (the LZ levels: the last <= 32 KiB already compressed)
+  std::vector<uint8_t> buf;    // [history | pending input]: pending starts at a chunk boundary of its flush segment
+  size_t hist = 0;             // bytes of history (the LZ levels: the last <= 32 KiB compressed since the member
+                               // start or the last full flush)
   ZbMemberCarry carry{0u, 1u, 0ull};  // the input compressed so far: raw CRC-32, Adler-32, bytes
   bool head_done = false, finished = false;
   int err = ZB200_OK;          // a CUDA failure: the stream is unusable
@@ -419,9 +420,10 @@ struct Group {
   uint64_t bound;       // output bound of the group
 };
 
-// One launch of a compress stream (zb200_compress_stream_*): a run of whole chunks of ONE member that
-// continues what earlier launches compressed.  The source holds `hist` bytes of the member's preceding input
-// in front of the run (k_lz2's history for the first chunk); `head`: the run starts the member (header);
+// One launch of a compress stream (zb200_compress_stream_*): a run of chunks of ONE member that continues
+// what earlier launches compressed; only the run's last chunk may be short (the end of a flush segment, or of
+// the member).  The source holds `hist` bytes (0..32768) of the member's preceding input in front of the run
+// (k_lz2's history for the first chunk); `head`: the run starts the member (header);
 // `last`: the run ends it (BFINAL, trailer).  carry_in is the member's bytes before the run, carry_out
 // receives the bytes through its end.
 struct StreamPart {
@@ -668,10 +670,12 @@ int compress_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint8_t *h_src, 
   return ZB200_OK;
 }
 
-// Compress the stream's next `nbytes` pending bytes (whole chunks unless `last`) into dst; ctx locked.  On
-// success the carry advances and the compressed input leaves the buffer (its last 32 KiB stay as history);
-// on failure nothing changes.
-int stream_run(zb200_compress_stream *st, size_t nbytes, bool last, uint8_t *dst, size_t dst_cap, size_t *dst_len) {
+// Compress the stream's next `nbytes` pending bytes into dst; ctx locked.  They are whole chunks, unless the run
+// ends the member (`last`) or a flush segment (a flush: every pending byte, last = false).  On success the carry
+// advances and the compressed input leaves the buffer: its last 32 KiB stay as history, none after a full flush
+// (`reset`).  On failure nothing changes.
+int stream_run(zb200_compress_stream *st, size_t nbytes, bool last, uint8_t *dst, size_t dst_cap, size_t *dst_len,
+               bool reset = false) {
   zb200_ctx *ctx = st->ctx;
   if (!dst) return ZB200_ERR_DST_TOO_SMALL;  // every run emits at least one byte
   const size_t in_end = st->hist + nbytes;
@@ -692,7 +696,7 @@ int stream_run(zb200_compress_stream *st, size_t nbytes, bool last, uint8_t *dst
   st->carry = sp.carry_out;
   st->head_done = true;
   const bool lz = st->level == -1 || st->level >= 2;
-  const size_t keep = lz ? std::min<size_t>(32768, in_end) : 0;
+  const size_t keep = lz && !reset ? std::min<size_t>(32768, in_end) : 0;
   st->buf.erase(st->buf.begin(), st->buf.begin() + (in_end - keep));
   st->hist = keep;
   return ZB200_OK;
@@ -1413,13 +1417,17 @@ constexpr uint64_t kDstreamHeaderBits = 1024 * 8;
 // stays at the payload start (base_out = 0): a window shorter than 32 KiB would let a distance reach before the
 // stream's start, which only a decode from the start rejects; the bytes already produced are not emitted twice.
 // `progress`: the output or the resume point moved.  Returns a decode status (the stream's verdict) or a CUDA one.
-int dstream_run(zb200_decompress_stream *st, bool last_in, bool &progress, bool uncapped = false) {
+// `drain` (zb200_decompress_stream_drain, not `last_in`): the bytes held back as the possible trailer are decoded
+// too, as payload that may go on: a block that ends inside them counts, and only finish decides where the input
+// ends.  If it does end there, the member has no final block before its trailer, and finish reports the error
+// that uncompress (which reads the trailer as payload as well) reports.
+int dstream_run(zb200_decompress_stream *st, bool last_in, bool &progress, bool drain = false, bool uncapped = false) {
   progress = false;
   zb200_ctx *ctx = st->ctx;
   cudaStream_t s = ctx->stream;
   const uint8_t *held = st->in.data() + st->in_head;
   const uint64_t held_n = st->in.size() - st->in_head;
-  const uint64_t resv = dstream_reserve(st);
+  const uint64_t resv = drain ? 0 : dstream_reserve(st);
   uint64_t pay_end = st->total_in - resv > st->in_off ? st->total_in - resv - st->in_off : 0;  // local bytes
   const uint64_t max_in = std::max<uint64_t>(2 * (uint64_t)st->batch_bytes, 65536);
   const bool capped = !uncapped && (last_in ? held_n : pay_end) > max_in;
@@ -1704,7 +1712,7 @@ int dstream_run(zb200_decompress_stream *st, bool last_in, bool &progress, bool 
       fprintf(stderr, "zb200 dstream: path=%s segs=%zu taken=%zu out=%llu final=%d\n", path, S, T,
               (unsigned long long)total, (int)fin);
     progress = fresh > 0 || (advance && stop > lo_bit) || fin;
-    if (capped && !progress) return dstream_run(st, last_in, progress, true);   // no complete block in the slice
+    if (capped && !progress) return dstream_run(st, last_in, progress, drain, true);   // no complete block in the slice
     st->check = check;
     st->out_total = std::max(st->out_total, new_base);
     if (fin) {
@@ -2532,6 +2540,27 @@ int zb200_compress_stream_write(zb200_compress_stream *st, const uint8_t *src, s
   });
 }
 
+int zb200_compress_stream_flush(zb200_compress_stream *st, int mode, uint8_t *dst, size_t dst_cap, size_t *dst_len) {
+  if (!st) return ZB200_ERR_ARG;
+  zb200_ctx *ctx = st->ctx;
+  return guarded(ctx, [&]() -> int {
+    if (!dst_len) return ZB200_ERR_ARG;
+    *dst_len = 0;
+    if (st->err) return st->err;
+    if (st->finished || (mode != ZB200_SYNC_FLUSH && mode != ZB200_FULL_FLUSH)) return ZB200_ERR_ARG;
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    DeviceGuard g(ctx->device);
+    memset(&ctx->timing, 0, sizeof(ctx->timing));
+    // a write always holds input back, so nothing pending means nothing written since the last flush (or begin)
+    const size_t pending = st->buf.size() - st->hist;
+    if (pending == 0) return ZB200_OK;
+    // the flush segment ends here: its last chunk may be short, and the next segment's chunks start after it
+    const int rc = stream_run(st, pending, false, dst, dst_cap, dst_len, mode == ZB200_FULL_FLUSH);
+    if (rc == ZB200_ERR_CUDA) st->err = rc;
+    return rc;
+  });
+}
+
 int zb200_compress_stream_finish(zb200_compress_stream *st, uint8_t *dst, size_t dst_cap, size_t *dst_len) {
   if (!st) return ZB200_ERR_ARG;
   zb200_ctx *ctx = st->ctx;
@@ -2605,6 +2634,35 @@ int zb200_decompress_stream_write(zb200_decompress_stream *st, const uint8_t *sr
       if (pending < st->batch_bytes || pending * 8 <= st->bit0) break;
       bool progress = false;
       rc = dstream_run(st, false, progress);
+      if (!progress) break;
+    }
+    if (!rc && avail) *avail = dstream_avail(st);
+    return rc;
+  });
+  if (rc && entered) {
+    st->err = rc;
+    if (avail) *avail = 0;
+  }
+  return rc;
+}
+
+int zb200_decompress_stream_drain(zb200_decompress_stream *st, size_t *avail) {
+  if (!st) return ZB200_ERR_ARG;
+  zb200_ctx *ctx = st->ctx;
+  bool entered = false;   // as in zb200_decompress_stream_write
+  const int rc = guarded(ctx, [&]() -> int {
+    if (avail) *avail = 0;
+    if (st->err) return st->err;
+    if (st->finished) return ZB200_ERR_ARG;
+    entered = true;
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    DeviceGuard g(ctx->device);
+    memset(&ctx->timing, 0, sizeof(ctx->timing));
+    int rc = st->fmt < 0 ? dstream_header(st, false) : ZB200_OK;
+    // every complete block of what has arrived, whatever the batching threshold, the held-back tail included
+    while (!rc && st->fmt >= 0 && !st->done && (st->in.size() - st->in_head) * 8 > st->bit0) {
+      bool progress = false;
+      rc = dstream_run(st, false, progress, true);
       if (!progress) break;
     }
     if (!rc && avail) *avail = dstream_avail(st);

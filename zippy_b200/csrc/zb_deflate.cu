@@ -660,7 +660,11 @@ __global__ void __launch_bounds__(LZ_THREADS, 2)
   uint32_t phase = 0;
   for (uint32_t chunk = blockIdx.x; chunk < n_chunks; chunk += gridDim.x) {
     const ZbChunkDesc d = desc[chunk];
-    const uint32_t len = d.len, hb = d.pad;  // pad = bytes of history staged in front of the chunk (a multiple of the segment size)
+    const uint32_t len = d.len, hb = d.pad;  // pad = bytes of history staged in front of the chunk, 0..32768
+    // The segment grid is anchored on the chunk start, so the sub-chunks stay segment-aligned: region position q
+    // lies in segment (q + hg) / 8192, and only segment 0 is partial when hb is not a multiple of 8 KiB (after a
+    // flush).  hg = 0 for every aligned pad.
+    const uint32_t hg = (0u - hb) & (LZ2_SEG_BYTES - 1u);
     const uint8_t *rsrc = src + d.src_off - hb;
     const uint32_t mis = (uint32_t)((uintptr_t)rsrc & 15u);
     const uint32_t off0 = mis + hb;           // chunk position x lives at data[off0 + x]
@@ -702,18 +706,19 @@ __global__ void __launch_bounds__(LZ_THREADS, 2)
 
     // ---- phase 1: static tables of every segment that precedes some sub-chunk of this chunk ----
     {
-      const uint32_t nseg = (rlen + LZ2_SEG_BYTES - 1) / LZ2_SEG_BYTES;  // segments of the region; the last is never history
+      const uint32_t nseg = (hg + rlen + LZ2_SEG_BYTES - 1) / LZ2_SEG_BYTES;  // segments of the region; the last is never history
       for (uint32_t sg = (uint32_t)warp; sg + 1 < nseg; sg += ZB_WARPS_PER_CHUNK) {
         uint2 *tab = stat + (size_t)sg * LZ2_BUCKETS;
         lz2_clear_table(tab, (1 << LZ2_STATIC_BITS) * 2);
         __syncwarp();
         uint16_t *tab16 = reinterpret_cast<uint16_t *>(tab);
-        const uint32_t q0 = sg * LZ2_SEG_BYTES, q1 = q0 + LZ2_SEG_BYTES;  // a full segment (only the last one can be short)
+        // the segment's region positions [q0, q1): a full segment, but segment 0 starts at the region start
+        const uint32_t q0 = sg ? sg * LZ2_SEG_BYTES - hg : 0u, q1 = (sg + 1) * LZ2_SEG_BYTES - hg;
         for (uint32_t s = q0; s < q1; s += 32) {
           const uint32_t q = s + (uint32_t)lane;
           const uint32_t v = zb_ld32_unaligned(data, mis + q);
           const uint32_t hs = lz2_hash_mul(v) >> (32 - LZ2_STATIC_BITS);
-          const bool can = q + 4 <= rlen;
+          const bool can = q + 4 <= rlen && q < q1;
           // lanes of one window that share a hash would store to one entry in one instruction, and which of
           // them lands is up to the hardware: the highest position writes, the others stand back
           const uint32_t grp = __match_any_sync(ZB_FULL, can ? hs : (0x80000000u | (uint32_t)lane));
@@ -726,7 +731,7 @@ __global__ void __launch_bounds__(LZ_THREADS, 2)
 
     // ---- phase 2: parse ----
     if (b0 < len) {
-      const uint32_t myseg = (hb + b0) / LZ2_SEG_BYTES;
+      const uint32_t myseg = (hg + hb + b0) / LZ2_SEG_BYTES;
       uint32_t entry = b0;
       uint32_t ksel = 0, kism = 0;
       uint2 *gmask = masks + (size_t)chunk * ZB_WINDOWS_PER_CHUNK;
