@@ -5,15 +5,17 @@
 //             of the chunk.  Replaces encodeSnappy/encodeFragment (snappy.nim:12-163),
 //             the histogram side of BlockMetadata (internal.nim:128-131) and the
 //             separate crc32/adler32 passes of zippy.nim:47,73.
-//   k_huff  : one thread per chunk: zb_build_codebook (zb_huff.h) -- replaces
-//             huffmanCodes + the dynamic header writer (deflate.nim:13-151, 295-394)
-//             and the stored/fixed/dynamic choice (deflate.nim:274-290).
+//   k_huff  : one warp per chunk, four chunks per CTA, workspace in shared memory
+//             (zb_huff_warp.cuh): the codebook zb_build_codebook (zb_huff.h) writes, built
+//             in parallel stages -- replaces huffmanCodes + the dynamic header writer
+//             (deflate.nim:13-151, 295-394) and the stored/fixed/dynamic choice (deflate.nim:274-290).
 //   k_scan  : exclusive scan of chunk sizes -> output offsets; per-member checksum combine.
 //   k_pack  : token -> bit emission with exact, precomputed bit offsets (replaces the
 //             BitStreamWriter loop, deflate.nim:396-464, bitstreams.nim:84-123) plus the
 //             gzip/zlib framing bytes of zippy.nim:21-78 for batched members.
 #include "zb_device.cuh"
 #include "zb_kernels.h"
+#include "zb_huff_warp.cuh"
 
 #define LZ_THREADS (ZB_WARPS_PER_CHUNK * 32)
 #define LZ_HASH_BITS 11
@@ -839,15 +841,14 @@ __global__ void __launch_bounds__(LZ_THREADS, 2)
 }
 
 // ------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(64)
-    k_huff(const ZbChunkDesc *__restrict__ desc, const uint16_t *__restrict__ hist, ZbCodebook *__restrict__ cb,
-           uint32_t n_chunks, int level) {
-  uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c >= n_chunks) return;
-  ZbChunkDesc d = desc[c];
-  zb_build_codebook(hist + (size_t)c * ZB_WARPS_PER_CHUNK * ZB_HIST_SYMS, d.len, (d.flags & ZB_CHUNK_LAST) ? 1 : 0,
-                    level == 0 ? 0 : -1, &cb[c]);
+// k_huff: zb_huff_warp.cuh
+#if ZB_HUFF_STAGE_CLOCKS
+extern "C" int zb200_huff_stage_clocks(unsigned long long *out) {
+  unsigned long long zero[HWS_N] = {};
+  if (cudaMemcpyFromSymbol(out, zb_huff_stage_clk, sizeof(zero)) != cudaSuccess) return -1;
+  return cudaMemcpyToSymbol(zb_huff_stage_clk, zero, sizeof(zero)) == cudaSuccess ? 0 : -1;
 }
+#endif
 
 // ------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t frame_head_bytes(int fmt, const uint8_t *fname_len, uint32_t m) {
@@ -1350,7 +1351,7 @@ cudaError_t zb_launch_lz(const ZbCompressWork &w, cudaStream_t s) {
 }
 cudaError_t zb_launch_huff(const ZbCompressWork &w, cudaStream_t s) {
   if (w.n_chunks == 0) return cudaSuccess;
-  k_huff<<<(w.n_chunks + 63) / 64, 64, 0, s>>>(w.desc, w.hist, w.cb, w.n_chunks, w.level);
+  k_huff<<<(w.n_chunks + HW_WARPS - 1) / HW_WARPS, HW_WARPS * 32, 0, s>>>(w.desc, w.hist, w.cb, w.n_chunks, w.level);
   return cudaGetLastError();
 }
 cudaError_t zb_launch_scan(const ZbCompressWork &w, cudaStream_t s) {

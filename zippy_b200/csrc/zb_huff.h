@@ -5,8 +5,11 @@
 // with a single-thread, allocation-free formulation: sort used symbols, Moffat-
 // Katajainen in-place minimum-redundancy lengths, Kraft-sum length limiting, canonical
 // LSB-first codes, code-length RLE, and exact bit accounting so the packer never needs
-// a sizing pass.  One GPU thread runs this per chunk (k_huff in zb_deflate.cu); the
-// same code is unit-tested on the CPU (tests/test_host_units.py).
+// a sizing pass.  This is the host builder and the reference: k_huff (zb_huff_warp.cuh) builds
+// the same codebook with one warp per chunk in parallel stages (1.37 ms for C2's 65 536 chunks
+// on an H100 80GB HBM3 at 700 W, against 3.41 ms for this code on one GPU thread per chunk), and
+// tests/test_gpu_huff_identity.py compares the two byte for byte; tests/test_host_units.py pins
+// this code's codebooks.
 #pragma once
 #include "zb_common.h"
 
