@@ -235,6 +235,61 @@ int zb200_decompress_stream_finish(zb200_decompress_stream *st, size_t *avail);
 int zb200_decompress_stream_read(zb200_decompress_stream *st, uint8_t *dst, size_t dst_cap, size_t *dst_len);
 void zb200_decompress_stream_free(zb200_decompress_stream *st);
 
+/* ---- random access into one gzip / zlib / raw member (a seekable index, as zlib's zran.c builds on a CPU) ----
+ * build decodes the member once, with uncompress's verdict (any failure is returned and no index is made), and
+ * records access points.  Segment points: for k = 0, 1, ..., the first block start whose output offset is at least
+ * k * 32768 (duplicates removed; point 0 is the first block, at offset 0).  Window points: for j = 0, 1, ..., the
+ * first segment point at or past j * span; each keeps the 32 KiB of output in front of it.  Every segment point keeps
+ * the CRC-32 of its interval (to the next point; the last one to the end of the member).  The points depend only on
+ * the member.  Random access is only as fine as the member's blocks: this library's members have a point at every
+ * 64 KiB chunk joint, zlib's at its block starts, and a member of one block has one point.
+ *  - build: span a multiple of 32768 and >= 32768 (zran's usual span is 1 << 20), else ZB200_ERR_ARG; a bad
+ *    data_format: ZB200_ERR_INVALID_FORMAT.  The index is host memory and belongs to no ctx: use it with any ctx,
+ *    from any thread, and free it with zb200_index_free.
+ *  - extract_batch reads the n ranges [offsets[i], offsets[i] + lens[i]) of the member's output into
+ *    dst[dst_offsets[i] ..) (dst_offsets has n + 1 entries; slot i holds dst_offsets[i+1] - dst_offsets[i] bytes).
+ *    ZB200_ERR_ARG, before any work: src's length or its first or last 32 bytes differ from the indexed member, a
+ *    range ends past the output, or a slot is too small.  Ranges may be empty and may overlap.  Every range is cut
+ *    at window points; each piece is decoded from its window point through the intervals it needs, and all of these
+ *    chains run in parallel, in launch groups of about 1 GiB of output.  Only the compressed bytes the chains cover
+ *    cross PCIe, with their windows.  statuses[i]: ZB200_OK with the exact bytes, ZB200_ERR_UNCOMPRESS if an
+ *    interval it needs does not decode to its recorded size and end, ZB200_ERR_CHECKSUM if it decodes but its CRC-32
+ *    differs (the gzip / zlib trailer is not read).
+ *  - points copies min(cap, count) points out (any array may be NULL) and returns the count.
+ *  - export writes the index as bytes (dst == NULL: only *len, the size); the same member and span give the same
+ *    bytes on any run and any ctx.  import reads them back; anything malformed (wrong length, magic, version or
+ *    CRC, counts that do not fit, points not strictly increasing in bit and output offset, a window flag that
+ *    breaks the rule above, a window that does not decompress to exactly 32768 bytes) is ZB200_ERR_ARG, and
+ *    nothing is read out of bounds.  Format, all integers little-endian:
+ *      offset  size  field
+ *           0     8  magic "ZB200IDX"
+ *           8     4  version (1)
+ *          12     4  data format (ZB200_DF_ZLIB / _GZIP / _DEFLATE, as resolved by the build)
+ *          16     8  payload start P (byte offset of the raw DEFLATE stream in the member)
+ *          24     8  member length in bytes
+ *          32     8  output size
+ *          40     8  span
+ *          48     8  reserved (0)
+ *          56    32  the member's first 32 bytes (zero-padded if shorter)
+ *          88    32  the member's last 32 bytes (zero-padded if shorter)
+ *         120     8  np: number of segment points (>= 1)
+ *         128     8  nw: number of windows (window points with output offset > 0)
+ *         136  24np  per point: bit position in the member (8), output offset (8), interval CRC-32 (4), window flag (4)
+ *           .   8nw  per window: length of its compressed form
+ *           .     .  the windows in point order, each the raw DEFLATE (level 1) of the 32768 bytes in front of its point
+ *           .     4  CRC-32 of every byte before it */
+typedef struct zb200_index zb200_index;
+int zb200_index_build(zb200_ctx *ctx, const uint8_t *src, size_t len, int data_format, uint64_t span, zb200_index **out);
+int zb200_index_extract_batch(zb200_ctx *ctx, const zb200_index *idx, const uint8_t *src, size_t len,
+                              const uint64_t *offsets, const uint64_t *lens, size_t n, uint8_t *dst,
+                              const uint64_t *dst_offsets, int *statuses);
+uint64_t zb200_index_size(const zb200_index *idx);   /* the member's output size */
+size_t zb200_index_points(const zb200_index *idx, uint64_t *bits, uint64_t *outs, uint32_t *crcs, uint8_t *window,
+                          size_t cap);
+void zb200_index_free(zb200_index *idx);
+int zb200_index_export(zb200_ctx *ctx, const zb200_index *idx, uint8_t *dst, size_t cap, size_t *len);
+int zb200_index_import(zb200_ctx *ctx, const uint8_t *src, size_t len, zb200_index **out);
+
 /* ---- device-resident variants (pointers prefixed d_ are device memory on ctx's device;
  * offsets / statuses / sizes stay host arrays).  Used when the data already lives in HBM
  * (bench.py's `value`) and by the multi-GPU sharded path.  The call returns after the

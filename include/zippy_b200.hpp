@@ -10,6 +10,7 @@
 #include <random>
 #include <stdexcept>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "zippy_b200.h"
@@ -279,6 +280,89 @@ class DecompressStream {
     return out;
   }
   zb200_decompress_stream *st_ = nullptr;
+};
+
+// Random access into one member (zb200_index_*): build once, then read ranges of its output.
+class Index {
+ public:
+  static Index build(const std::string &data, CompressedDataFormat dataFormat = dfDetect, uint64_t span = 1u << 20,
+                     zb200_ctx *ctx = nullptr) {
+    Index ix(ctx);
+    detail::check(zb200_index_build(ix.ctx_, reinterpret_cast<const uint8_t *>(data.data()), data.size(), dataFormat,
+                                    span, &ix.idx_));
+    return ix;
+  }
+  static Index fromBytes(const std::string &buf, zb200_ctx *ctx = nullptr) {
+    Index ix(ctx);
+    detail::check(zb200_index_import(ix.ctx_, reinterpret_cast<const uint8_t *>(buf.data()), buf.size(), &ix.idx_));
+    return ix;
+  }
+  Index(Index &&o) noexcept : ctx_(o.ctx_), idx_(o.idx_) { o.idx_ = nullptr; }
+  Index &operator=(Index &&o) noexcept {
+    std::swap(ctx_, o.ctx_);
+    std::swap(idx_, o.idx_);
+    return *this;
+  }
+  Index(const Index &) = delete;
+  Index &operator=(const Index &) = delete;
+  ~Index() { close(); }
+
+  uint64_t size() const { return zb200_index_size(idx_); }
+  struct Point {
+    uint64_t bit, out;
+    uint32_t crc;
+    bool window;
+  };
+  std::vector<Point> points() const {
+    const size_t n = zb200_index_points(idx_, nullptr, nullptr, nullptr, nullptr, 0);
+    std::vector<uint64_t> b(n), o(n);
+    std::vector<uint32_t> c(n);
+    std::vector<uint8_t> w(n);
+    zb200_index_points(idx_, b.data(), o.data(), c.data(), w.data(), n);
+    std::vector<Point> out(n);
+    for (size_t i = 0; i < n; i++) out[i] = Point{b[i], o[i], c[i], w[i] != 0};
+    return out;
+  }
+  // ranges [offsets[i], offsets[i] + lengths[i]); statuses[i] == 0 where out[i] holds the bytes
+  std::vector<std::string> extractBatch(const std::string &data, const std::vector<uint64_t> &offsets,
+                                        const std::vector<uint64_t> &lengths, std::vector<int> &statuses) const {
+    if (offsets.size() != lengths.size()) detail::check(ZB200_ERR_ARG);
+    const size_t n = offsets.size();
+    std::vector<uint64_t> doff(n + 1, 0);
+    for (size_t i = 0; i < n; i++) doff[i + 1] = doff[i] + lengths[i];
+    std::string buf(doff[n] + 1, '\0');
+    statuses.assign(n, 0);
+    detail::check(zb200_index_extract_batch(ctx_, idx_, reinterpret_cast<const uint8_t *>(data.data()), data.size(),
+                                            offsets.data(), lengths.data(), n, reinterpret_cast<uint8_t *>(&buf[0]),
+                                            doff.data(), statuses.data()));
+    std::vector<std::string> out(n);
+    for (size_t i = 0; i < n; i++)
+      if (statuses[i] == 0) out[i] = buf.substr(doff[i], lengths[i]);
+    return out;
+  }
+  std::string extract(const std::string &data, uint64_t offset, uint64_t length) const {
+    std::vector<int> st;
+    std::vector<std::string> r = extractBatch(data, {offset}, {length}, st);
+    detail::check(st[0]);
+    return r[0];
+  }
+  std::string toBytes() const {
+    size_t n = 0;
+    detail::check(zb200_index_export(ctx_, idx_, nullptr, 0, &n));
+    std::string out(n, '\0');
+    detail::check(zb200_index_export(ctx_, idx_, reinterpret_cast<uint8_t *>(&out[0]), out.size(), &n));
+    out.resize(n);
+    return out;
+  }
+  void close() {
+    zb200_index_free(idx_);
+    idx_ = nullptr;
+  }
+
+ private:
+  explicit Index(zb200_ctx *ctx) : ctx_(ctx ? ctx : detail::ctx()) {}
+  zb200_ctx *ctx_ = nullptr;
+  zb200_index *idx_ = nullptr;
 };
 
 }  // namespace zippy

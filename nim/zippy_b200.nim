@@ -347,3 +347,78 @@ proc close*(s: var DecompressStream) =
   if s.st != nil:
     zb200_decompress_stream_free(s.st)
     s.st = nil
+
+# ---- random access into one member (zb200_index_*): build once, then read ranges of its output ----
+type
+  Zb200Index = pointer
+  Index* = object
+    idx: Zb200Index
+  IndexPoint* = object
+    bit*, output*: uint64
+    crc*: uint32
+    window*: bool
+
+proc zb200_index_build(ctx: Zb200Ctx, src: pointer, len: csize_t, dataFormat: cint, span: uint64,
+                       res: ptr Zb200Index): cint {.importc, cdecl, dynlib: lib.}
+proc zb200_index_extract_batch(ctx: Zb200Ctx, idx: Zb200Index, src: pointer, len: csize_t, offsets, lens: ptr uint64,
+                               n: csize_t, dst: pointer, dstOffsets: ptr uint64,
+                               statuses: ptr cint): cint {.importc, cdecl, dynlib: lib.}
+proc zb200_index_size(idx: Zb200Index): uint64 {.importc, cdecl, dynlib: lib.}
+proc zb200_index_points(idx: Zb200Index, bits, outs: ptr uint64, crcs: ptr uint32, window: ptr uint8,
+                        cap: csize_t): csize_t {.importc, cdecl, dynlib: lib.}
+proc zb200_index_export(ctx: Zb200Ctx, idx: Zb200Index, dst: pointer, cap: csize_t,
+                        len: ptr csize_t): cint {.importc, cdecl, dynlib: lib.}
+proc zb200_index_import(ctx: Zb200Ctx, src: pointer, len: csize_t, res: ptr Zb200Index): cint {.importc, cdecl, dynlib: lib.}
+proc zb200_index_free(idx: Zb200Index) {.importc, cdecl, dynlib: lib.}
+
+proc buildIndex*(data: string, dataFormat = dfDetect, span = 1'u64 shl 20): Index {.raises: [ZippyError].} =
+  check zb200_index_build(getCtx(), data.cstring, data.len.csize_t, dataFormat.cint, span, result.idx.addr)
+
+proc indexFromBytes*(buf: string): Index {.raises: [ZippyError].} =
+  check zb200_index_import(getCtx(), buf.cstring, buf.len.csize_t, result.idx.addr)
+
+proc size*(ix: Index): uint64 = zb200_index_size(ix.idx)
+
+proc points*(ix: Index): seq[IndexPoint] =
+  let n = zb200_index_points(ix.idx, nil, nil, nil, nil, 0).int
+  var bits, outs = newSeq[uint64](n + 1)
+  var crcs = newSeq[uint32](n + 1)
+  var win = newSeq[uint8](n + 1)
+  discard zb200_index_points(ix.idx, bits[0].addr, outs[0].addr, crcs[0].addr, win[0].addr, n.csize_t)
+  for i in 0 ..< n:
+    result.add IndexPoint(bit: bits[i], output: outs[i], crc: crcs[i], window: win[i] != 0)
+
+proc extractBatch*(ix: Index, data: string, offsets, lengths: seq[uint64],
+                   statuses: var seq[cint]): seq[string] {.raises: [ZippyError].} =
+  ## range i is [offsets[i], offsets[i] + lengths[i]); result[i] holds it where statuses[i] == 0
+  if offsets.len != lengths.len: check 22
+  let n = offsets.len
+  var doff = newSeq[uint64](n + 1)
+  for i in 0 ..< n: doff[i + 1] = doff[i] + lengths[i]
+  var buf = newString(doff[n].int + 1)
+  statuses = newSeq[cint](n + 1)
+  var o = offsets & @[0'u64]
+  var l = lengths & @[0'u64]
+  check zb200_index_extract_batch(getCtx(), ix.idx, data.cstring, data.len.csize_t, o[0].addr, l[0].addr, n.csize_t,
+                                  buf[0].addr, doff[0].addr, statuses[0].addr)
+  statuses.setLen(n)
+  for i in 0 ..< n:
+    result.add(if statuses[i] == 0: buf[doff[i].int ..< doff[i + 1].int] else: "")
+
+proc extract*(ix: Index, data: string, offset, length: uint64): string {.raises: [ZippyError].} =
+  var st: seq[cint]
+  let r = ix.extractBatch(data, @[offset], @[length], st)
+  check st[0]
+  r[0]
+
+proc toBytes*(ix: Index): string {.raises: [ZippyError].} =
+  var n: csize_t
+  check zb200_index_export(getCtx(), ix.idx, nil, 0, n.addr)
+  result = newString(n.int + 1)
+  check zb200_index_export(getCtx(), ix.idx, result[0].addr, n + 1, n.addr)
+  result.setLen(n.int)
+
+proc close*(ix: var Index) =
+  if ix.idx != nil:
+    zb200_index_free(ix.idx)
+    ix.idx = nil

@@ -30,7 +30,7 @@ SyncFlush, FullFlush = 2, 3                                            # zlib's 
 
 __all__ = ["compress", "uncompress", "crc32", "adler32", "deflate", "inflate", "compress_batch", "uncompress_batch",
            "uncompressed_sizes", "checksum_batch", "ZippyError", "Context", "CompressStream", "DecompressStream",
-           "MultiGpu", "dfDetect",
+           "MultiGpu", "Index", "dfDetect",
            "dfZlib", "dfGzip",
            "dfDeflate", "NoCompression", "BestSpeed", "BestCompression", "DefaultCompression", "HuffmanOnly",
            "SyncFlush", "FullFlush"]
@@ -506,6 +506,99 @@ class MultiGpu:
         _check(None, L.zb200_mgpu_checksum_batch(self._h, base.ctypes.data, offsets.ctypes.data, n,
                                                   0 if kind == "crc32" else 1, out.ctypes.data))
         return out[:n]
+
+
+class Index:
+    """Random access into one gzip / zlib / raw member (zb200_index_*): access points found by one decode on the
+    GPU, then batches of ranges decoded from the nearest window point.  The index lives in host memory; `ctx` is
+    only the context its calls run on."""
+
+    def __init__(self, handle, ctx):
+        self._h = handle
+        self._ctx = ctx
+
+    @classmethod
+    def build(cls, data, dataFormat=dfDetect, span=1 << 20, ctx=None):
+        ctx = ctx or default_context()
+        src = _as_u8(data)
+        h = ctypes.c_void_p()
+        _check(ctx._h, _native.lib().zb200_index_build(ctx._h, src.ctypes.data, src.size, dataFormat, span,
+                                                       ctypes.byref(h)))
+        return cls(h, ctx)
+
+    def _handle(self):
+        if not self._h:
+            raise ZippyError(22, "the index is closed")
+        return self._h
+
+    @property
+    def size(self):
+        """The member's output size."""
+        return int(_native.lib().zb200_index_size(self._handle()))
+
+    @property
+    def points(self):
+        """dict of numpy arrays, one entry per segment point: bit (position in the member), out (output offset),
+        crc (CRC-32 of the interval up to the next point) and window (1 at window points)."""
+        L, h = _native.lib(), self._handle()
+        n = int(L.zb200_index_points(h, None, None, None, None, 0))
+        bits, outs = np.zeros(n, np.uint64), np.zeros(n, np.uint64)
+        crcs, win = np.zeros(n, np.uint32), np.zeros(n, np.uint8)
+        L.zb200_index_points(h, bits.ctypes.data, outs.ctypes.data, crcs.ctypes.data, win.ctypes.data, n)
+        return {"bit": bits, "out": outs, "crc": crcs, "window": win}
+
+    def extract_batch(self, data, offsets, lengths):
+        """-> (out uint8 array, out_offsets uint64[n+1], statuses int32[n]): range i is
+        out[out_offsets[i]:out_offsets[i+1]] where statuses[i] == 0."""
+        src = _as_u8(data)
+        offsets = np.ascontiguousarray(offsets, dtype=np.uint64).reshape(-1)
+        lengths = np.ascontiguousarray(lengths, dtype=np.uint64).reshape(-1)
+        if offsets.size != lengths.size:
+            raise ZippyError(22, "offsets and lengths differ in length")
+        n = offsets.size
+        out_offs = np.zeros(n + 1, dtype=np.uint64)
+        np.cumsum(lengths, out=out_offs[1:])
+        out = np.empty(int(out_offs[n]) + 1, dtype=np.uint8)
+        st = np.zeros(max(n, 1), dtype=np.int32)
+        _check(self._ctx._h, _native.lib().zb200_index_extract_batch(
+            self._ctx._h, self._handle(), src.ctypes.data, src.size, offsets.ctypes.data, lengths.ctypes.data, n,
+            out.ctypes.data, out_offs.ctypes.data, st.ctypes.data))
+        return out[:int(out_offs[n])], out_offs, st[:n]
+
+    def extract(self, data, offset, length):
+        """The output bytes [offset, offset + length) of the member; raises ZippyError on a bad range or member."""
+        out, _, st = self.extract_batch(data, [offset], [length])
+        if st[0] != 0:
+            raise ZippyError(int(st[0]))
+        return out.tobytes()
+
+    def to_bytes(self):
+        """The index serialised (include/zippy_b200.h documents the format); Index.from_bytes reads it back."""
+        L, h = _native.lib(), self._handle()
+        n = ctypes.c_size_t(0)
+        _check(self._ctx._h, L.zb200_index_export(self._ctx._h, h, None, 0, ctypes.byref(n)))
+        out = np.empty(n.value, dtype=np.uint8)
+        _check(self._ctx._h, L.zb200_index_export(self._ctx._h, h, out.ctypes.data, out.size, ctypes.byref(n)))
+        return out[:n.value].tobytes()
+
+    @classmethod
+    def from_bytes(cls, buf, ctx=None):
+        ctx = ctx or default_context()
+        src = _as_u8(buf)
+        h = ctypes.c_void_p()
+        _check(ctx._h, _native.lib().zb200_index_import(ctx._h, src.ctypes.data, src.size, ctypes.byref(h)))
+        return cls(h, ctx)
+
+    def close(self):
+        if self._h:
+            _native.lib().zb200_index_free(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
 
 
 def host_register(ptr, nbytes):

@@ -68,6 +68,15 @@ SYMBOLS = {
     "zb200_decompress_stream_finish": (c_int, [ctypes.c_void_p, ctypes.POINTER(c_size_t)]),
     "zb200_decompress_stream_read": (c_int, [ctypes.c_void_p, c_u8p, c_size_t, ctypes.POINTER(c_size_t)]),
     "zb200_decompress_stream_free": (None, [ctypes.c_void_p]),
+    "zb200_index_build": (c_int, [ctypes.c_void_p, c_u8p, c_size_t, c_int, ctypes.c_uint64,
+                                  ctypes.POINTER(ctypes.c_void_p)]),
+    "zb200_index_extract_batch": (c_int, [ctypes.c_void_p, ctypes.c_void_p, c_u8p, c_size_t, c_u64p, c_u64p, c_size_t,
+                                          c_u8p, c_u64p, c_intp]),
+    "zb200_index_size": (ctypes.c_uint64, [ctypes.c_void_p]),
+    "zb200_index_points": (c_size_t, [ctypes.c_void_p, c_u64p, c_u64p, ctypes.c_void_p, c_u8p, c_size_t]),
+    "zb200_index_free": (None, [ctypes.c_void_p]),
+    "zb200_index_export": (c_int, [ctypes.c_void_p, ctypes.c_void_p, c_u8p, c_size_t, ctypes.POINTER(c_size_t)]),
+    "zb200_index_import": (c_int, [ctypes.c_void_p, c_u8p, c_size_t, ctypes.POINTER(ctypes.c_void_p)]),
     "zb200_mgpu_init": (c_int, [ctypes.c_void_p, c_int, ctypes.POINTER(ctypes.c_void_p)]),
     "zb200_mgpu_shutdown": (None, [ctypes.c_void_p]),
     "zb200_mgpu_device_count": (c_int, [ctypes.c_void_p]),

@@ -16,6 +16,7 @@
 #include <condition_variable>
 #include <deque>
 #include <functional>
+#include <memory>
 #include <mutex>
 #include <thread>
 #include <string>
@@ -188,6 +189,9 @@ struct zb200_ctx {
   bool big_env = false;
   bool joint_markers = true;       // env ZB200_JOINT_MARKERS=0 turns the marker segments at sync joints off (A/B timing)
   uint32_t mark_window_segs = 8192;  // segments per window of the joint marker decode (env ZB200_MARK_WINDOW_SEGS)
+  DevBuf idx_desc, idx_out;          // index build / extraction: gather descriptors, gathered bytes
+  uint64_t index_group_bytes = kDstreamMaxOut;  // output budget of one extraction launch group (env ZB200_INDEX_GROUP_BYTES)
+  bool index_log = false;            // env ZB200_INDEX_LOG: one stderr line per extraction launch group
   cudaEvent_t ev[10] = {};
   cudaStream_t h2d_stream = nullptr, d2h_stream = nullptr;
   std::vector<cudaEvent_t> gev;   // per-group events (H2D done, compute done, offsets ready)
@@ -1399,6 +1403,59 @@ uint64_t dstream_reserve(const zb200_decompress_stream *st) {
 // before the end of the input received so far is only believed at finish.
 constexpr uint64_t kDstreamHeaderBits = 1024 * 8;
 
+// Segment boundaries of a raw stream in d_src that starts at bit lo_bit and whose payload ends at byte pay_end:
+// bits[0] = lo_bit, then this library's joints / zlib flushes (k_find_sync), else dynamic-block starts
+// (k_find_blocks), at least 16 KiB apart.  They are candidates: every segment [bits[i], bits[i + 1]) still has to
+// decode as a closed segment.  `path` names what was found ("joints", "blocks", or "serial": bits = {lo_bit}).
+int find_segment_bits(zb200_ctx *ctx, const uint8_t *d_src, uint64_t lo_bit, uint64_t pay_end, std::vector<uint64_t> &bits,
+                      const char *&path) {
+  cudaStream_t s = ctx->stream;
+  const uint64_t pay_bit = pay_end * 8ull;
+  const uint64_t min_gap = std::max<uint64_t>(16384ull * 8ull, (pay_bit - std::min(pay_bit, lo_bit)) / 60000ull);
+  bits.assign(1, lo_bit);
+  path = "serial";
+  if (pay_bit <= lo_bit + 2 * min_gap) return ZB200_OK;
+  ENSURE(ctx->counter, 128);
+  uint32_t *d_cnt = (uint32_t *)ctx->counter.p + 8;
+  const uint64_t lo = (lo_bit + 7) / 8;
+  uint32_t cap = (uint32_t)std::min<uint64_t>((pay_end - lo) / 32 + 64, 1u << 24);
+  ENSURE(ctx->seg_cand, (size_t)cap * 8 + 16);
+  uint32_t cnt = 0;
+  CK(zb_launch_find_sync(d_src, lo, pay_end, (uint64_t *)ctx->seg_cand.p, cap, d_cnt, s));
+  CK(cudaMemcpyAsync(&cnt, d_cnt, 4, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  ctx->timing.kernel_launches += 1;
+  std::vector<uint64_t> cand;
+  if (cnt > 0 && cnt <= cap) {
+    cand.resize(cnt);
+    CK(cudaMemcpyAsync(cand.data(), ctx->seg_cand.p, (size_t)cnt * 8, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    std::sort(cand.begin(), cand.end());
+    for (uint64_t c : cand)
+      if (c * 8 >= bits.back() + min_gap && c * 8 < pay_bit) bits.push_back(c * 8);
+    path = "joints";
+  }
+  if (bits.size() < 2) {
+    cap = (uint32_t)std::min<uint64_t>((pay_end - lo) / 64 + 1024, 1u << 24);
+    ENSURE(ctx->seg_cand, (size_t)cap * 8 + 16);
+    CK(zb_launch_find_blocks(d_src, lo_bit, pay_bit, pay_end, (uint64_t *)ctx->seg_cand.p, cap, d_cnt, s));
+    CK(cudaMemcpyAsync(&cnt, d_cnt, 4, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    ctx->timing.kernel_launches += 1;
+    if (cnt > 0 && cnt <= cap) {
+      cand.resize(cnt);
+      CK(cudaMemcpyAsync(cand.data(), ctx->seg_cand.p, (size_t)cnt * 8, cudaMemcpyDeviceToHost, s));
+      CK(cudaStreamSynchronize(s));
+      std::sort(cand.begin(), cand.end());
+      for (uint64_t c : cand)
+        if (c >= bits.back() + min_gap && c + min_gap / 4 < pay_bit) bits.push_back(c);
+      path = "blocks";
+    }
+  }
+  if (bits.size() < 2) path = "serial";
+  return ZB200_OK;
+}
+
 // One launch of a decompress stream (ctx locked): decode the held input from the resume point, bits [bit0, end),
 // where end is the payload received so far (`last`: everything, the trailer included, as uncompress reads it).
 //  1. Boundaries: this library's joints / zlib flushes (k_find_sync), else dynamic-block starts (k_find_blocks),
@@ -1439,56 +1496,18 @@ int dstream_run(zb200_decompress_stream *st, bool last_in, bool &progress, bool 
   const uint64_t dec_end = last ? held_n : pay_end;
   const uint64_t lo_bit = st->bit0, end_bit = dec_end * 8ull, pay_bit = pay_end * 8ull;
   if (!last && pay_bit <= lo_bit) return ZB200_OK;
-  const uint64_t min_gap = std::max<uint64_t>(16384ull * 8ull, (pay_bit - std::min(pay_bit, lo_bit)) / 60000ull);
   ENSURE(ctx->in_stage, dec_end + 64);
   ENSURE(ctx->counter, 128);
   const uint8_t *d_src = (const uint8_t *)ctx->in_stage.p;
   int rc = h2d_copy(ctx, (uint8_t *)ctx->in_stage.p, held, dec_end, s, true);
   if (rc) return rc;
-  uint32_t *d_cnt = (uint32_t *)ctx->counter.p + 8;
   uint64_t *d_resume = (uint64_t *)ctx->counter.p + 8;   // bytes 64..79
   int *d_bad = (int *)((uint32_t *)ctx->counter.p + 12);
   // 1. boundaries
-  std::vector<uint64_t> bits(1, lo_bit);
+  std::vector<uint64_t> bits;
   const char *path = "serial";
-  if (pay_bit > lo_bit + 2 * min_gap) {
-    const uint64_t lo = (lo_bit + 7) / 8;
-    uint32_t cap = (uint32_t)std::min<uint64_t>((pay_end - lo) / 32 + 64, 1u << 24);
-    ENSURE(ctx->seg_cand, (size_t)cap * 8 + 16);
-    uint32_t cnt = 0;
-    CK(zb_launch_find_sync(d_src, lo, pay_end, (uint64_t *)ctx->seg_cand.p, cap, d_cnt, s));
-    CK(cudaMemcpyAsync(&cnt, d_cnt, 4, cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
-    ctx->timing.kernel_launches += 1;
-    std::vector<uint64_t> cand;
-    if (cnt > 0 && cnt <= cap) {
-      cand.resize(cnt);
-      CK(cudaMemcpyAsync(cand.data(), ctx->seg_cand.p, (size_t)cnt * 8, cudaMemcpyDeviceToHost, s));
-      CK(cudaStreamSynchronize(s));
-      std::sort(cand.begin(), cand.end());
-      for (uint64_t c : cand)
-        if (c * 8 >= bits.back() + min_gap && c * 8 < pay_bit) bits.push_back(c * 8);
-      path = "joints";
-    }
-    if (bits.size() < 2) {
-      cap = (uint32_t)std::min<uint64_t>((pay_end - lo) / 64 + 1024, 1u << 24);
-      ENSURE(ctx->seg_cand, (size_t)cap * 8 + 16);
-      CK(zb_launch_find_blocks(d_src, lo_bit, pay_bit, pay_end, (uint64_t *)ctx->seg_cand.p, cap, d_cnt, s));
-      CK(cudaMemcpyAsync(&cnt, d_cnt, 4, cudaMemcpyDeviceToHost, s));
-      CK(cudaStreamSynchronize(s));
-      ctx->timing.kernel_launches += 1;
-      if (cnt > 0 && cnt <= cap) {
-        cand.resize(cnt);
-        CK(cudaMemcpyAsync(cand.data(), ctx->seg_cand.p, (size_t)cnt * 8, cudaMemcpyDeviceToHost, s));
-        CK(cudaStreamSynchronize(s));
-        std::sort(cand.begin(), cand.end());
-        for (uint64_t c : cand)
-          if (c >= bits.back() + min_gap && c + min_gap / 4 < pay_bit) bits.push_back(c);
-        path = "blocks";
-      }
-    }
-    if (bits.size() < 2) path = "serial";
-  }
+  rc = find_segment_bits(ctx, d_src, lo_bit, pay_end, bits, path);
+  if (rc) return rc;
   ZbInflateWork w;
   memset(&w, 0, sizeof(w));
   w.src = d_src;
@@ -2302,6 +2321,11 @@ int zb200_init(int device, zb200_ctx **out) {
     long v = atol(e);
     if (v > 0) ctx->mark_window_segs = (uint32_t)std::min<long>(v, 60000);
   }
+  if (const char *e = getenv("ZB200_INDEX_GROUP_BYTES")) {  // test hook: small launch groups in index extraction
+    long long v = atoll(e);
+    if (v > 0) ctx->index_group_bytes = (uint64_t)v;
+  }
+  if (const char *e = getenv("ZB200_INDEX_LOG")) ctx->index_log = atoi(e) != 0;  // test hook: one line per extraction group
   ctx->memops = load_stream_memops();
   if (const char *e = getenv("ZB200_UNC_GATED")) ctx->gated_unc = atoi(e) != 0;  // test hook: 0 = one launch per group
   if (const char *e = getenv("ZB200_UNC_GROUP_BYTES")) {  // test hook: small pipelined groups in the host uncompress
@@ -2343,7 +2367,8 @@ void zb200_shutdown(zb200_ctx *ctx) {
                     &ctx->cb, &ctx->chunk_off, &ctx->member_off, &ctx->member_check, &ctx->member_isize,
                     &ctx->src_off, &ctx->dst_off, &ctx->out_len, &ctx->status, &ctx->expect, &ctx->kind,
                     &ctx->counter, &ctx->ck_out, &ctx->ck_pieces, &ctx->ck_first, &ctx->ck_piece_out, &ctx->ck_partials, &ctx->in_stage, &ctx->out_stage, &ctx->lz2_tables, &ctx->carry,
-                    &ctx->seg_src, &ctx->seg_dst, &ctx->seg_len, &ctx->seg_status, &ctx->seg_kind, &ctx->seg_expect, &ctx->seg_cand, &ctx->skip_mask, &ctx->order, &ctx->mark_scratch, &ctx->mark_segs, &ctx->seg_bits, &ctx->mark_win, &ctx->gate};
+                    &ctx->seg_src, &ctx->seg_dst, &ctx->seg_len, &ctx->seg_status, &ctx->seg_kind, &ctx->seg_expect, &ctx->seg_cand, &ctx->skip_mask, &ctx->order, &ctx->mark_scratch, &ctx->mark_segs, &ctx->seg_bits, &ctx->mark_win, &ctx->gate,
+                    &ctx->idx_desc, &ctx->idx_out};
   for (DevBuf *b : bufs)
     if (b->p) cudaFree(b->p);
   if (ctx->d_tabs) cudaFree(ctx->d_tabs);
@@ -2997,13 +3022,8 @@ int zb200_checksum_batch(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t
 // was too small) and reports the size; decode_finish copies the bytes to the caller.  Also what gives the
 // reference's answer for a gzip member whose ISIZE understates its content: the data is produced, the CRC
 // is checked, then the size check fails (gzip.nim:80-88), instead of "destination too small".
-int zb200_decode_begin(zb200_ctx *ctx, const uint8_t *src, size_t len, int data_format, size_t pos, size_t *out_len) {
-  return guarded(ctx, [&]() -> int {
-    if (!ctx || !out_len || (len && !src)) return ZB200_ERR_ARG;
-    if (data_format < ZB200_DF_DETECT || data_format > ZB200_DF_DEFLATE) return ZB200_ERR_INVALID_FORMAT;
-    std::lock_guard<std::mutex> lk(ctx->mu);
-    DeviceGuard g(ctx->device);
-    memset(&ctx->timing, 0, sizeof(ctx->timing));
+// decode_begin with the ctx locked: the member staged in in_stage, its output in out_stage (ctx->pending)
+static int decode_begin_locked(zb200_ctx *ctx, const uint8_t *src, size_t len, int data_format, size_t pos, size_t *out_len) {
     ctx->pending = false;
     uint8_t dummy = 0;
     const uint8_t *sp = src ? src : &dummy;
@@ -3040,6 +3060,16 @@ int zb200_decode_begin(zb200_ctx *ctx, const uint8_t *src, size_t len, int data_
       cap = real;
     }
     return ZB200_ERR_UNCOMPRESS;
+}
+
+int zb200_decode_begin(zb200_ctx *ctx, const uint8_t *src, size_t len, int data_format, size_t pos, size_t *out_len) {
+  return guarded(ctx, [&]() -> int {
+    if (!ctx || !out_len || (len && !src)) return ZB200_ERR_ARG;
+    if (data_format < ZB200_DF_DETECT || data_format > ZB200_DF_DEFLATE) return ZB200_ERR_INVALID_FORMAT;
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    DeviceGuard g(ctx->device);
+    memset(&ctx->timing, 0, sizeof(ctx->timing));
+    return decode_begin_locked(ctx, src, len, data_format, pos, out_len);
   });
 }
 
@@ -3121,6 +3151,707 @@ int zb200_adler32(zb200_ctx *ctx, const void *src, size_t len, uint32_t *out) {
   uint64_t so[2] = {0, len};
   uint8_t dummy = 0;
   return zb200_checksum_batch(ctx, src ? (const uint8_t *)src : &dummy, so, 1, 1, out);
+}
+
+}  // extern "C"
+
+// ---- random access (zb200_index_*) ----
+// Segment points: for k = 0, 1, ..., the first block start whose output offset is >= k * 32768 (duplicates removed).
+// Window points: for j = 0, 1, ..., the first segment point whose output offset is >= j * span; each keeps the 32 KiB
+// of output in front of it.  Every segment point keeps the CRC-32 of its interval (up to the next point, the last one
+// to the end of the member).  All of it is host memory, tied to no ctx.
+struct zb200_index {
+  int fmt = 0;
+  uint64_t payload = 0, len = 0, size = 0, span = 0;
+  uint8_t head[32] = {}, tail[32] = {};
+  std::vector<uint64_t> bit, out;   // per point: absolute bit position in the member, output offset
+  std::vector<uint32_t> crc;        // per point: CRC-32 of its interval
+  std::vector<uint8_t> win;         // per point: 1 = window point
+  std::vector<uint64_t> win_at;     // per point: offset of its window in `windows` (window points with out > 0)
+  std::vector<uint8_t> windows;
+};
+
+namespace {
+
+void index_edges(const uint8_t *src, uint64_t len, uint8_t *head, uint8_t *tail) {
+  const size_t k = (size_t)std::min<uint64_t>(len, 32);
+  memset(head, 0, 32);
+  memset(tail, 0, 32);
+  if (k) {
+    memcpy(head, src, k);
+    memcpy(tail, src + len - k, k);
+  }
+}
+
+// gather byte ranges (src offset, dst offset, length) of a device buffer into dst, in pieces of ZB_GATHER_BYTES
+int index_gather(zb200_ctx *ctx, const uint8_t *d_src, const std::vector<uint64_t> &ranges, bool wide, void *d_dst) {
+  std::vector<ZbGather> g;
+  for (size_t i = 0; i + 3 <= ranges.size(); i += 3)
+    for (uint64_t r = 0; r < ranges[i + 2]; r += ZB_GATHER_BYTES) {
+      ZbGather e;
+      e.src = ranges[i] + r;
+      e.dst = ranges[i + 1] + r;
+      e.n = (uint32_t)std::min<uint64_t>(ZB_GATHER_BYTES, ranges[i + 2] - r);
+      e.wide = wide ? 1u : 0u;
+      g.push_back(e);
+    }
+  if (g.empty()) return ZB200_OK;
+  ENSURE(ctx->idx_desc, g.size() * sizeof(ZbGather));
+  CK(cudaMemcpyAsync(ctx->idx_desc.p, g.data(), g.size() * sizeof(ZbGather), cudaMemcpyHostToDevice, ctx->stream));
+  CK(zb_launch_gather(d_src, (const ZbGather *)ctx->idx_desc.p, (uint32_t)g.size(), d_dst, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));   // `g` goes out of scope
+  ctx->timing.kernel_launches += 1;
+  ctx->timing.h2d_bytes += g.size() * sizeof(ZbGather);
+  return ZB200_OK;
+}
+
+// One counting pass over the segments bits[i] .. bits[i + 1] (the last one to end_bit) of the member staged in
+// in_stage; with `base` the recorder stores access points into rec [2 * nrec].
+int index_count(zb200_ctx *ctx, const std::vector<uint64_t> &bits, uint64_t end_bit, uint64_t len, const uint64_t *base,
+                uint64_t *d_rec, uint32_t nrec, std::vector<uint64_t> &sl, std::vector<int> &sst, std::vector<uint32_t> &sk) {
+  cudaStream_t s = ctx->stream;
+  const size_t S = bits.size();
+  std::vector<uint64_t> sb(2 * S);
+  for (size_t i = 0; i < S; i++) {
+    sb[2 * i] = bits[i];
+    sb[2 * i + 1] = i + 1 < S ? bits[i + 1] : end_bit;
+  }
+  ENSURE(ctx->seg_bits, 2 * S * 8);
+  ENSURE(ctx->seg_dst, (S + 1) * 8);
+  ENSURE(ctx->seg_len, S * 8);
+  ENSURE(ctx->seg_status, S * 4);
+  ENSURE(ctx->seg_kind, S * 4);
+  ENSURE(ctx->seg_expect, S * 4);
+  ENSURE(ctx->counter, 128);
+  CK(cudaMemcpyAsync(ctx->seg_bits.p, sb.data(), 2 * S * 8, cudaMemcpyHostToDevice, s));
+  if (base) CK(cudaMemcpyAsync(ctx->seg_dst.p, base, (S + 1) * 8, cudaMemcpyHostToDevice, s));
+  ZbInflateWork w;
+  memset(&w, 0, sizeof(w));
+  w.src = (const uint8_t *)ctx->in_stage.p;
+  w.seg_bits = (const uint64_t *)ctx->seg_bits.p;
+  w.seg_limit = len;
+  w.dst_off = (const uint64_t *)ctx->seg_dst.p;
+  w.out_len = (uint64_t *)ctx->seg_len.p;
+  w.status = (int *)ctx->seg_status.p;
+  w.expect = (uint32_t *)ctx->seg_expect.p;
+  w.kind = (uint32_t *)ctx->seg_kind.p;
+  w.counter = (uint32_t *)ctx->counter.p + 4;
+  w.tabs = ctx->d_tabs;
+  w.n = (uint32_t)S;
+  w.data_format = ZB200_DF_DEFLATE;
+  w.seg_mode = 1;
+  w.count_only = 1;
+  if (base) {
+    w.rec = d_rec;
+    w.rec_base = (const uint64_t *)ctx->seg_dst.p;
+    w.nrec = nrec;
+  }
+  CK(zb_launch_inflate(w, s));
+  sl.resize(S);
+  sst.resize(S);
+  sk.resize(S);
+  CK(cudaMemcpyAsync(sl.data(), ctx->seg_len.p, S * 8, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(sst.data(), ctx->seg_status.p, S * 4, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(sk.data(), ctx->seg_kind.p, S * 4, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  ctx->timing.kernel_launches += 1;
+  return ZB200_OK;
+}
+
+int index_build_locked(zb200_ctx *ctx, const uint8_t *src, size_t len, int data_format, uint64_t span, zb200_index **out) {
+  cudaStream_t s = ctx->stream;
+  uint64_t size = 0;
+  {
+    size_t n = 0;
+    const int st = decode_begin_locked(ctx, src, len, data_format, 0, &n);
+    ctx->pending = false;
+    if (st) return st;
+    size = n;
+  }
+  uint64_t payload = 0;
+  uint32_t kind = 0, expect = 0, isize = 0;
+  if (zb_parse_wrapper(src, len, data_format, 0, payload, kind, expect, isize) != ZB200_OK) return ZB200_ERR_UNCOMPRESS;
+  const uint64_t trailer = kind == ZB200_DF_GZIP ? 8 : kind == ZB200_DF_ZLIB ? 4 : 0;
+  // 1. block starts: closed segments at the boundaries the decompress streams use, else one serial segment
+  std::vector<uint64_t> bits;
+  const char *path = "serial";
+  int rc = find_segment_bits(ctx, (const uint8_t *)ctx->in_stage.p, payload * 8ull, len - trailer, bits, path);
+  if (rc) return rc;
+  const uint32_t nrec = (uint32_t)(size / 32768ull + 1ull);
+  ENSURE(ctx->idx_out, (size_t)nrec * 16);
+  uint64_t *d_rec = (uint64_t *)ctx->idx_out.p;
+  std::vector<uint64_t> sl, base;
+  std::vector<int> sst;
+  std::vector<uint32_t> sk;
+  auto regular = [&]() {
+    uint64_t t = 0;
+    for (size_t i = 0; i < bits.size(); i++) {
+      // (several segments: each one's output must fit the marker decode's 32-bit positions; one serial segment
+      // has the limit uncompress has)
+      if (sst[i] != ZB200_OK || (sk[i] != 0) != (i + 1 == bits.size()) || (bits.size() > 1 && sl[i] > 0xf0000000ull))
+        return false;
+      t += sl[i];
+    }
+    return t == size;
+  };
+  for (;;) {
+    const size_t S = bits.size();
+    base.assign(S + 1, 0);
+    if (S > 1) {   // the sizes first: every segment's output offset
+      rc = index_count(ctx, bits, len * 8ull, len, nullptr, nullptr, 0, sl, sst, sk);
+      if (rc) return rc;
+      if (!regular()) {
+        bits.resize(1);
+        continue;
+      }
+      for (size_t i = 0; i < S; i++) base[i + 1] = base[i] + sl[i];
+    } else {
+      base[1] = size;
+    }
+    CK(cudaMemsetAsync(d_rec, 0xff, (size_t)nrec * 16, s));
+    rc = index_count(ctx, bits, len * 8ull, len, base.data(), d_rec, nrec, sl, sst, sk);
+    if (rc) return rc;
+    if (regular()) break;
+    if (S == 1) return ZB200_ERR_UNCOMPRESS;   // a member uncompress accepts counts the same
+    bits.resize(1);
+  }
+  std::vector<uint64_t> rec((size_t)nrec * 2);
+  CK(cudaMemcpyAsync(rec.data(), d_rec, (size_t)nrec * 16, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  std::unique_ptr<zb200_index> idx(new zb200_index());
+  for (uint32_t k = 0; k < nrec; k++) {
+    uint64_t b = rec[2 * k], o = rec[2 * k + 1];
+    if (b == ~0ull) {   // no block start of its segment reaches the multiple: the next segment's start
+      size_t j = 1;
+      while (j < bits.size() && base[j] < (uint64_t)k * 32768ull) j++;
+      if (j >= bits.size()) continue;
+      b = bits[j];
+      o = base[j];
+    }
+    if (!idx->bit.empty() && idx->bit.back() == b) continue;
+    if (!idx->bit.empty() && (b < idx->bit.back() || o <= idx->out.back())) return ZB200_ERR_UNCOMPRESS;
+    idx->bit.push_back(b);
+    idx->out.push_back(o);
+  }
+  const size_t np = idx->bit.size();
+  if (np == 0 || idx->out[0] != 0) return ZB200_ERR_UNCOMPRESS;
+  // 2. window flags, windows and interval CRCs, from the decoded output in out_stage
+  idx->win.assign(np, 0);
+  idx->win_at.assign(np, ~0ull);
+  std::vector<uint64_t> ranges;
+  uint64_t next = 0, wbytes = 0;
+  for (size_t p = 0; p < np; p++) {
+    if (idx->out[p] < next) continue;
+    idx->win[p] = 1;
+    next = (idx->out[p] / span + 1) * span;
+    if (idx->out[p] > 0) {
+      idx->win_at[p] = wbytes;
+      ranges.push_back(idx->out[p] - 32768ull);
+      ranges.push_back(wbytes);
+      ranges.push_back(32768ull);
+      wbytes += 32768ull;
+    }
+  }
+  idx->crc.assign(np, 0);
+  std::vector<uint64_t> offs(idx->out);
+  offs.push_back(size);
+  rc = checksum_device_locked(ctx, (const uint8_t *)ctx->out_stage.p, offs.data(), np, 0, idx->crc.data());
+  if (rc) return rc;
+  idx->windows.resize(wbytes);
+  if (wbytes) {
+    ENSURE(ctx->idx_out, wbytes);
+    rc = index_gather(ctx, (const uint8_t *)ctx->out_stage.p, ranges, false, ctx->idx_out.p);
+    if (rc) return rc;
+    CK(cudaMemcpyAsync(idx->windows.data(), ctx->idx_out.p, wbytes, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    ctx->timing.d2h_bytes += wbytes;
+  }
+  idx->fmt = (int)kind;
+  idx->payload = payload;
+  idx->len = len;
+  idx->size = size;
+  idx->span = span;
+  index_edges(src, len, idx->head, idx->tail);
+  *out = idx.release();
+  return ZB200_OK;
+}
+
+// A chain decodes the segment intervals [p0, p1) of an index, starting at window point p0 (its window in front).
+struct IndexChain {
+  size_t p0, p1;
+};
+
+// One launch group of an extraction: the chains [c0, c1), then the pieces that they serve.  `piece` holds, per
+// piece: chain, output offset, length, destination (host pointer).  chain_st receives each chain's status.
+int index_extract_group(zb200_ctx *ctx, const zb200_index *idx, const uint8_t *src, const std::vector<IndexChain> &ch,
+                        size_t c0, size_t c1, std::vector<int> &chain_st) {
+  cudaStream_t s = ctx->stream;
+  const size_t np = idx->bit.size();
+  const uint64_t end_bit = idx->len * 8ull;
+  // 1. the host staging: every chain's window, then its compressed slice
+  std::vector<uint8_t> stage;
+  std::vector<uint64_t> sb, dof, wranges;
+  std::vector<ZbMarkSegHost> segs;
+  std::vector<size_t> seg_chain, seg_point;   // per inflate segment: its chain and point
+  std::vector<size_t> rseg_of_point;          // per inflate segment: its index in `segs`
+  uint64_t se = 0, de = 0;
+  uint32_t max_n = 0;
+  for (size_t c = c0; c < c1; c++) {
+    const IndexChain &k = ch[c];
+    if (k.p0 > 0) {
+      const uint64_t at = stage.size();
+      stage.insert(stage.end(), idx->windows.begin() + (ptrdiff_t)idx->win_at[k.p0],
+                   idx->windows.begin() + (ptrdiff_t)idx->win_at[k.p0] + 32768);
+      se += 32768ull;
+      ZbMarkSegHost m = {se, de, 32768u, 0u};
+      segs.push_back(m);
+      wranges.push_back(at);
+      wranges.push_back(se);
+      wranges.push_back(32768ull);
+      se += 32768ull;
+      de += 32768ull;
+      max_n = std::max<uint32_t>(max_n, 32768u);
+    }
+    const uint64_t b0 = idx->bit[k.p0] / 8ull;
+    const uint64_t b1 = k.p1 < np ? (idx->bit[k.p1] + 7ull) / 8ull : idx->len;
+    const uint64_t at = stage.size();
+    stage.insert(stage.end(), src + b0, src + b1);
+    for (size_t p = k.p0; p < k.p1; p++) {
+      const uint64_t n = (p + 1 < np ? idx->out[p + 1] : idx->size) - idx->out[p];
+      const uint64_t eb = p + 1 < np ? idx->bit[p + 1] : end_bit;
+      // the segment, then an empty one that starts where it must end: it owns the gap up to the next segment, so
+      // every segment's capacity is exactly its interval and a corrupt one cannot write into its neighbours
+      sb.push_back(at * 8ull + idx->bit[p] - b0 * 8ull);
+      sb.push_back(at * 8ull + eb - b0 * 8ull);
+      sb.push_back(at * 8ull + eb - b0 * 8ull);
+      sb.push_back(at * 8ull + eb - b0 * 8ull);
+      se += 32768ull;
+      dof.push_back(se);
+      dof.push_back(se + n);
+      rseg_of_point.push_back(segs.size());
+      ZbMarkSegHost m = {se, de, (uint32_t)n, 0u};
+      segs.push_back(m);
+      seg_chain.push_back(c);
+      seg_point.push_back(p);
+      se += n;
+      de += n;
+      max_n = std::max<uint32_t>(max_n, (uint32_t)n);
+    }
+  }
+  dof.push_back(se);
+  const size_t T = seg_chain.size(), R = segs.size();
+  ENSURE(ctx->in_stage, stage.size() + 64);
+  int rc = h2d_copy(ctx, (uint8_t *)ctx->in_stage.p, stage.data(), stage.size(), s, true);
+  if (rc) return rc;
+  ctx->timing.h2d_bytes += stage.size();
+  ENSURE(ctx->mark_scratch, (size_t)se * 2 + 64);
+  ENSURE(ctx->mark_segs, R * sizeof(ZbMarkSegHost) + 16);
+  const size_t T2 = 2 * T;   // every segment is followed by its empty gap segment
+  ENSURE(ctx->seg_bits, T2 * 16);
+  ENSURE(ctx->seg_dst, (T2 + 1) * 8);
+  ENSURE(ctx->seg_len, T2 * 8);
+  ENSURE(ctx->seg_status, T2 * 4);
+  ENSURE(ctx->seg_kind, T2 * 4);
+  ENSURE(ctx->seg_expect, T2 * 4);
+  ENSURE(ctx->counter, 128);
+  ENSURE(ctx->out_stage, (size_t)de + 64);
+  CK(cudaMemcpyAsync(ctx->mark_segs.p, segs.data(), R * sizeof(ZbMarkSegHost), cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(ctx->seg_bits.p, sb.data(), T2 * 16, cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(ctx->seg_dst.p, dof.data(), (T2 + 1) * 8, cudaMemcpyHostToDevice, s));
+  ctx->timing.h2d_bytes += R * sizeof(ZbMarkSegHost) + T2 * 24 + 8;
+  // 2. markers, then the windows as byte symbols, then one marker decode of every segment of every chain
+  CK(zb_launch_mark_prefill((uint16_t *)ctx->mark_scratch.p, ctx->mark_segs.p, (uint32_t)R, s));
+  ctx->timing.kernel_launches += 1;
+  rc = index_gather(ctx, (const uint8_t *)ctx->in_stage.p, wranges, true, ctx->mark_scratch.p);
+  if (rc) return rc;
+  ZbInflateWork w;
+  memset(&w, 0, sizeof(w));
+  w.src = (const uint8_t *)ctx->in_stage.p;
+  w.seg_bits = (const uint64_t *)ctx->seg_bits.p;
+  w.seg_limit = stage.size();
+  w.seg_win0 = ch[c0].p0 > 0;   // a chain from point 0 has no window: a distance before the member start is an error
+  w.dst = (uint8_t *)ctx->mark_scratch.p;
+  w.dst_off = (const uint64_t *)ctx->seg_dst.p;
+  w.out_len = (uint64_t *)ctx->seg_len.p;
+  w.status = (int *)ctx->seg_status.p;
+  w.expect = (uint32_t *)ctx->seg_expect.p;
+  w.kind = (uint32_t *)ctx->seg_kind.p;
+  w.counter = (uint32_t *)ctx->counter.p + 4;
+  w.tabs = ctx->d_tabs;
+  w.n = (uint32_t)T2;
+  w.data_format = ZB200_DF_DEFLATE;
+  w.seg_mode = 1;
+  w.mark = 1;
+  CK(zb_launch_inflate(w, s));
+  ctx->timing.kernel_launches += 1;
+  std::vector<uint64_t> sl(T2);
+  std::vector<int> sst(T2);
+  std::vector<uint32_t> sk(T2);
+  CK(cudaMemcpyAsync(sl.data(), ctx->seg_len.p, T2 * 8, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(sst.data(), ctx->seg_status.p, T2 * 4, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(sk.data(), ctx->seg_kind.p, T2 * 4, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  for (size_t c = c0; c < c1; c++) chain_st[c] = ZB200_OK;
+  bool any_failed = false;
+  for (size_t t = 0; t < T; t++) {
+    const size_t c = seg_chain[t], p = seg_point[t];
+    const bool last = p + 1 == np;
+    if (sst[2 * t] != ZB200_OK || sl[2 * t] != segs[rseg_of_point[t]].n || (sk[2 * t] != 0) != last) {
+      // a failed segment's symbols are not all written: resolve none of them (its chain has failed, and the next
+      // chain starts from its own window, so nothing else reads them)
+      chain_st[c] = ZB200_ERR_UNCOMPRESS;
+      segs[rseg_of_point[t]].n = 0;
+      any_failed = true;
+    }
+  }
+  if (any_failed)
+    CK(cudaMemcpyAsync(ctx->mark_segs.p, segs.data(), R * sizeof(ZbMarkSegHost), cudaMemcpyHostToDevice, s));
+  // 3. one resolve over [window, chain segments, window, chain segments, ...]: the windows hold no markers, so
+  // every chain resolves against its own window.  Only the first chain of a group can reach before the member
+  // start, and only the chain from point 0 starts a group without a window; it decodes without one, so a marker
+  // before the start (`bad`) cannot be produced by a segment that decoded.
+  int *d_bad = (int *)((uint32_t *)ctx->counter.p + 12);
+  CK(cudaMemsetAsync(d_bad, 0, 4, s));
+  const uint32_t gsz = std::max<uint32_t>(1u, (uint32_t)std::ceil(std::sqrt((double)R)));
+  const size_t ngroups = (R + gsz - 1) / gsz;
+  ENSURE(ctx->mark_win, ngroups * 32768ull * 3);
+  CK(zb_launch_resolve_groups((uint16_t *)ctx->mark_scratch.p, ctx->mark_segs.p, (uint32_t)R, max_n, gsz, 0, 0,
+                              (uint16_t *)ctx->mark_win.p, (uint8_t *)ctx->mark_win.p + ngroups * 65536ull,
+                              (uint8_t *)ctx->out_stage.p, d_bad, s));
+  ctx->timing.kernel_launches += 4;
+  int bad = 0;
+  CK(cudaMemcpyAsync(&bad, d_bad, 4, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  // 4. every decoded interval against its CRC-32
+  std::vector<uint64_t> coff(R + 1);
+  for (size_t r = 0; r < R; r++) coff[r] = segs[r].dst;
+  coff[R] = de;
+  std::vector<uint32_t> crc(R);
+  rc = checksum_device_locked(ctx, (const uint8_t *)ctx->out_stage.p, coff.data(), R, 0, crc.data());
+  if (rc) return rc;
+  if (bad) chain_st[c0] = ZB200_ERR_UNCOMPRESS;
+  for (size_t t = 0; t < T; t++) {
+    const size_t c = seg_chain[t], p = seg_point[t];
+    if (chain_st[c] == ZB200_OK && crc[rseg_of_point[t]] != idx->crc[p]) chain_st[c] = ZB200_ERR_CHECKSUM;
+  }
+  if (ctx->index_log)
+    fprintf(stderr, "zb200 index: group of %zu chains, %zu segments, %zu bytes uploaded\n", c1 - c0, T, stage.size());
+  return ZB200_OK;
+}
+
+int index_extract_locked(zb200_ctx *ctx, const zb200_index *idx, const uint8_t *src, size_t len, const uint64_t *offsets,
+                         const uint64_t *lens, size_t n, uint8_t *dst, const uint64_t *dst_offsets, int *statuses) {
+  cudaStream_t s = ctx->stream;
+  uint8_t head[32], tail[32];
+  index_edges(src, len, head, tail);
+  if (len != idx->len || memcmp(head, idx->head, 32) || memcmp(tail, idx->tail, 32)) return ZB200_ERR_ARG;
+  for (size_t i = 0; i < n; i++) {
+    if (offsets[i] > idx->size || lens[i] > idx->size - offsets[i]) return ZB200_ERR_ARG;
+    if (dst_offsets[i + 1] < dst_offsets[i] || dst_offsets[i + 1] - dst_offsets[i] < lens[i]) return ZB200_ERR_ARG;
+  }
+  const size_t np = idx->bit.size();
+  std::vector<size_t> wpts;   // window point indices
+  for (size_t p = 0; p < np; p++)
+    if (idx->win[p]) wpts.push_back(p);
+  // every range cut at window points: piece (range, window point slot, start, end)
+  struct Piece {
+    size_t range, slot;
+    uint64_t a, b;
+  };
+  std::vector<Piece> pieces;
+  std::vector<size_t> reach(wpts.size(), 0);   // per window point: the chain's end point (exclusive), 0 = unused
+  for (size_t i = 0; i < n; i++) {
+    statuses[i] = ZB200_OK;
+    uint64_t a = offsets[i];
+    const uint64_t e = offsets[i] + lens[i];
+    while (a < e) {
+      // the last window point at or before a
+      size_t j = (size_t)(std::upper_bound(wpts.begin(), wpts.end(), a, [&](uint64_t v, size_t p) { return v < idx->out[p]; }) -
+                          wpts.begin()) - 1;
+      const uint64_t b = j + 1 < wpts.size() ? std::min<uint64_t>(e, idx->out[wpts[j + 1]]) : e;
+      // the first segment point at or past b, or the member's end
+      const size_t p1 = (size_t)(std::lower_bound(idx->out.begin(), idx->out.end(), b) - idx->out.begin());
+      reach[j] = std::max(reach[j], std::max(p1, wpts[j] + 1));
+      pieces.push_back(Piece{i, j, a, b});
+      a = b;
+    }
+  }
+  std::vector<IndexChain> ch;
+  std::vector<size_t> chain_of(wpts.size(), 0);
+  for (size_t j = 0; j < wpts.size(); j++)
+    if (reach[j]) {
+      chain_of[j] = ch.size();
+      ch.push_back(IndexChain{wpts[j], std::min(reach[j], np)});
+    }
+  std::vector<int> chain_st(ch.size(), ZB200_OK);
+  std::vector<uint64_t> chain_dst(ch.size(), 0);   // output offset in out_stage of the chain's first interval
+  // launch groups of chains under the output budget; a chain larger than it has a group of its own
+  std::vector<uint8_t> host;
+  for (size_t c0 = 0; c0 < ch.size();) {
+    size_t c1 = c0;
+    uint64_t bytes = 0;
+    while (c1 < ch.size()) {
+      const uint64_t o0 = idx->out[ch[c1].p0], o1 = ch[c1].p1 < np ? idx->out[ch[c1].p1] : idx->size;
+      const uint64_t cb = (o1 - o0) + (ch[c1].p0 > 0 ? 32768ull : 0ull);
+      if (c1 > c0 && bytes + cb > ctx->index_group_bytes) break;
+      bytes += cb;
+      chain_dst[c1] = bytes - (o1 - o0);
+      c1++;
+    }
+    int rc = index_extract_group(ctx, idx, src, ch, c0, c1, chain_st);
+    if (rc) return rc;
+    // 5. the pieces this group serves, gathered into one packed buffer, one copy out
+    std::vector<uint64_t> ranges;
+    std::vector<size_t> which;
+    uint64_t packed = 0;
+    for (size_t k = 0; k < pieces.size(); k++) {
+      const size_t c = chain_of[pieces[k].slot];
+      if (c < c0 || c >= c1 || chain_st[c] != ZB200_OK) continue;
+      ranges.push_back(chain_dst[c] + (pieces[k].a - idx->out[ch[c].p0]));
+      ranges.push_back(packed);
+      ranges.push_back(pieces[k].b - pieces[k].a);
+      which.push_back(k);
+      packed += pieces[k].b - pieces[k].a;
+    }
+    if (packed) {
+      ENSURE(ctx->idx_out, packed);
+      rc = index_gather(ctx, (const uint8_t *)ctx->out_stage.p, ranges, false, ctx->idx_out.p);
+      if (rc) return rc;
+      host.resize(packed);
+      CK(cudaMemcpyAsync(host.data(), ctx->idx_out.p, packed, cudaMemcpyDeviceToHost, s));
+      CK(cudaStreamSynchronize(s));
+      ctx->timing.d2h_bytes += packed;
+      uint64_t at = 0;
+      for (size_t k : which) {
+        const Piece &pc = pieces[k];
+        memcpy(dst + dst_offsets[pc.range] + (pc.a - offsets[pc.range]), host.data() + at, pc.b - pc.a);
+        at += pc.b - pc.a;
+      }
+    }
+    c0 = c1;
+  }
+  // per range: the worst of its chains (a decode failure before a CRC mismatch)
+  for (const Piece &pc : pieces) {
+    const int cs = chain_st[chain_of[pc.slot]];
+    int &st = statuses[pc.range];
+    if (cs == ZB200_ERR_UNCOMPRESS || (cs != ZB200_OK && st == ZB200_OK)) st = cs;
+  }
+  return ZB200_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int zb200_index_build(zb200_ctx *ctx, const uint8_t *src, size_t len, int data_format, uint64_t span, zb200_index **out) {
+  return guarded(ctx, [&]() -> int {
+    if (!ctx || !out || (len && !src)) return ZB200_ERR_ARG;
+    *out = nullptr;
+    if (data_format < ZB200_DF_DETECT || data_format > ZB200_DF_DEFLATE) return ZB200_ERR_INVALID_FORMAT;
+    if (span < 32768 || span % 32768) return ZB200_ERR_ARG;
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    DeviceGuard g(ctx->device);
+    memset(&ctx->timing, 0, sizeof(ctx->timing));
+    uint8_t dummy = 0;
+    return index_build_locked(ctx, src ? src : &dummy, len, data_format, span, out);
+  });
+}
+
+int zb200_index_extract_batch(zb200_ctx *ctx, const zb200_index *idx, const uint8_t *src, size_t len,
+                              const uint64_t *offsets, const uint64_t *lens, size_t n, uint8_t *dst,
+                              const uint64_t *dst_offsets, int *statuses) {
+  return guarded(ctx, [&]() -> int {
+    if (!ctx || !idx || (len && !src) || (n && (!offsets || !lens || !dst_offsets || !statuses))) return ZB200_ERR_ARG;
+    if (n && dst_offsets[n] > dst_offsets[0] && !dst) return ZB200_ERR_ARG;
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    DeviceGuard g(ctx->device);
+    memset(&ctx->timing, 0, sizeof(ctx->timing));
+    uint8_t dummy = 0;
+    return index_extract_locked(ctx, idx, src ? src : &dummy, len, offsets, lens, n, dst, dst_offsets, statuses);
+  });
+}
+
+void zb200_index_free(zb200_index *idx) { delete idx; }
+
+uint64_t zb200_index_size(const zb200_index *idx) { return idx ? idx->size : 0; }
+
+size_t zb200_index_points(const zb200_index *idx, uint64_t *bits, uint64_t *outs, uint32_t *crcs, uint8_t *window,
+                          size_t cap) {
+  if (!idx) return 0;
+  const size_t np = idx->bit.size();
+  for (size_t p = 0; p < np && p < cap; p++) {
+    if (bits) bits[p] = idx->bit[p];
+    if (outs) outs[p] = idx->out[p];
+    if (crcs) crcs[p] = idx->crc[p];
+    if (window) window[p] = idx->win[p];
+  }
+  return np;
+}
+
+// ---- index serialisation (format: include/zippy_b200.h) ----
+static const uint8_t kIndexMagic[8] = {'Z', 'B', '2', '0', '0', 'I', 'D', 'X'};
+static constexpr uint32_t kIndexVersion = 1;
+static constexpr size_t kIndexHeader = 8 + 4 + 4 + 8 * 5 + 32 + 32 + 8 + 8;   // through the two counts
+static constexpr size_t kIndexPoint = 8 + 8 + 4 + 4;
+
+static uint32_t host_crc32(const uint8_t *p, size_t n) {
+  static uint32_t tab[256];
+  static std::once_flag once;
+  std::call_once(once, [] {
+    for (uint32_t i = 0; i < 256; i++) {
+      uint32_t c = i;
+      for (int k = 0; k < 8; k++) c = (c >> 1) ^ ((0u - (c & 1u)) & 0xedb88320u);
+      tab[i] = c;
+    }
+  });
+  uint32_t c = 0xffffffffu;
+  for (size_t i = 0; i < n; i++) c = tab[(c ^ p[i]) & 255u] ^ (c >> 8);
+  return ~c;
+}
+static void put_le(std::vector<uint8_t> &b, uint64_t v, int n) {
+  for (int i = 0; i < n; i++) b.push_back((uint8_t)(v >> (8 * i)));
+}
+static uint64_t get_le(const uint8_t *p, int n) {
+  uint64_t v = 0;
+  for (int i = 0; i < n; i++) v |= (uint64_t)p[i] << (8 * i);
+  return v;
+}
+
+int zb200_index_export(zb200_ctx *ctx, const zb200_index *idx, uint8_t *dst, size_t cap, size_t *len) {
+  if (!ctx || !idx || !len) return ZB200_ERR_ARG;
+  const size_t np = idx->bit.size(), nw = idx->windows.size() / 32768;
+  // the windows as raw DEFLATE at level 1, one compress_batch
+  std::vector<uint64_t> so(nw + 1), doff(nw + 1, 0);
+  for (size_t i = 0; i <= nw; i++) so[i] = 32768ull * i;
+  std::vector<uint8_t> comp(nw * (zb200_compress_bound(32768, ZB200_DF_DEFLATE) + 64) + 64);
+  std::vector<int> cst(nw + 1, 0);
+  if (nw) {
+    const int rc = zb200_compress_batch(ctx, idx->windows.data(), so.data(), nw, 1, ZB200_DF_DEFLATE, nullptr, comp.data(),
+                                        comp.size(), doff.data(), cst.data());
+    if (rc) return rc;
+    for (size_t i = 0; i < nw; i++)
+      if (cst[i]) return cst[i];
+  }
+  return guarded(ctx, [&]() -> int {
+    std::vector<uint8_t> b;
+    b.insert(b.end(), kIndexMagic, kIndexMagic + 8);
+    put_le(b, kIndexVersion, 4);
+    put_le(b, (uint64_t)idx->fmt, 4);
+    put_le(b, idx->payload, 8);
+    put_le(b, idx->len, 8);
+    put_le(b, idx->size, 8);
+    put_le(b, idx->span, 8);
+    put_le(b, 0, 8);
+    b.insert(b.end(), idx->head, idx->head + 32);
+    b.insert(b.end(), idx->tail, idx->tail + 32);
+    put_le(b, np, 8);
+    put_le(b, nw, 8);
+    for (size_t p = 0; p < np; p++) {
+      put_le(b, idx->bit[p], 8);
+      put_le(b, idx->out[p], 8);
+      put_le(b, idx->crc[p], 4);
+      put_le(b, idx->win[p], 4);
+    }
+    for (size_t i = 0; i < nw; i++) put_le(b, doff[i + 1] - doff[i], 8);
+    b.insert(b.end(), comp.begin(), comp.begin() + (ptrdiff_t)doff[nw]);
+    put_le(b, host_crc32(b.data(), b.size()), 4);
+    *len = b.size();
+    if (!dst) return ZB200_OK;
+    if (cap < b.size()) return ZB200_ERR_DST_TOO_SMALL;
+    memcpy(dst, b.data(), b.size());
+    return ZB200_OK;
+  });
+}
+
+static int index_import(zb200_ctx *ctx, const uint8_t *src, size_t len, zb200_index **out) {
+  std::unique_ptr<zb200_index> idx(new zb200_index());
+  std::vector<uint64_t> clen;
+  size_t pos = 0;
+  // everything but the windows' contents, checked on the host
+  {
+    if (len < kIndexHeader + 4 || memcmp(src, kIndexMagic, 8) || get_le(src + 8, 4) != kIndexVersion) return ZB200_ERR_ARG;
+    if (host_crc32(src, len - 4) != (uint32_t)get_le(src + len - 4, 4)) return ZB200_ERR_ARG;
+    const uint8_t *h = src + 12;
+    const uint64_t fmt = get_le(h, 4);
+    idx->payload = get_le(h + 4, 8);
+    idx->len = get_le(h + 12, 8);
+    idx->size = get_le(h + 20, 8);
+    idx->span = get_le(h + 28, 8);
+    const uint64_t reserved = get_le(h + 36, 8);
+    memcpy(idx->head, h + 44, 32);
+    memcpy(idx->tail, h + 76, 32);
+    const uint64_t np = get_le(h + 108, 8), nw = get_le(h + 116, 8);
+    if (fmt < ZB200_DF_ZLIB || fmt > ZB200_DF_DEFLATE || reserved || idx->span < 32768 || idx->span % 32768 ||
+        idx->payload > idx->len || idx->len > (1ull << 62) || idx->size > (1ull << 62))
+      return ZB200_ERR_ARG;
+    idx->fmt = (int)fmt;
+    const uint64_t body = len - 4 - kIndexHeader;
+    if (np == 0 || np > idx->size / 32768 + 1 || np > body / kIndexPoint || nw > np || nw > (body - np * kIndexPoint) / 8)
+      return ZB200_ERR_ARG;
+    pos = kIndexHeader;
+    idx->bit.resize(np);
+    idx->out.resize(np);
+    idx->crc.resize(np);
+    idx->win.resize(np);
+    idx->win_at.assign(np, ~0ull);
+    uint64_t next = 0, w = 0;
+    for (size_t p = 0; p < np; p++, pos += kIndexPoint) {
+      idx->bit[p] = get_le(src + pos, 8);
+      idx->out[p] = get_le(src + pos + 8, 8);
+      idx->crc[p] = (uint32_t)get_le(src + pos + 16, 4);
+      const uint64_t flag = get_le(src + pos + 20, 4);
+      if (p == 0 ? idx->out[0] != 0 || idx->bit[0] != idx->payload * 8ull
+                 : idx->bit[p] <= idx->bit[p - 1] || idx->out[p] <= idx->out[p - 1])
+        return ZB200_ERR_ARG;
+      if (idx->bit[p] >= idx->len * 8ull || idx->out[p] > idx->size) return ZB200_ERR_ARG;
+      const bool is_win = idx->out[p] >= next;
+      if (flag != (is_win ? 1u : 0u)) return ZB200_ERR_ARG;
+      idx->win[p] = (uint8_t)flag;
+      if (is_win) {
+        next = (idx->out[p] / idx->span + 1) * idx->span;
+        if (idx->out[p] > 0) idx->win_at[p] = 32768ull * w++;
+      }
+    }
+    if (w != nw) return ZB200_ERR_ARG;
+    clen.resize(nw);
+    uint64_t total = 0;
+    for (size_t i = 0; i < nw; i++, pos += 8) {
+      clen[i] = get_le(src + pos, 8);
+      if (clen[i] == 0 || clen[i] > len) return ZB200_ERR_ARG;
+      total += clen[i];
+    }
+    if (total != len - 4 - pos) return ZB200_ERR_ARG;
+  }
+  // the windows: one uncompress_batch, each exactly 32768 bytes (every window point past 0 is at >= span >= 32768)
+  const size_t nw = clen.size();
+  idx->windows.resize(nw * 32768);
+  if (nw) {
+    std::vector<uint64_t> so(nw + 1), doff(nw + 1), dl(nw);
+    std::vector<int> st(nw);
+    so[0] = pos;
+    for (size_t i = 0; i < nw; i++) {
+      so[i + 1] = so[i] + clen[i];
+      doff[i] = 32768ull * i;
+    }
+    doff[nw] = 32768ull * nw;
+    const int rc = zb200_uncompress_batch(ctx, src, so.data(), nw, ZB200_DF_DEFLATE, idx->windows.data(), doff.data(),
+                                          dl.data(), st.data());
+    if (rc) return rc;
+    for (size_t i = 0; i < nw; i++)
+      if (st[i] != ZB200_OK || dl[i] != 32768) return ZB200_ERR_ARG;
+  }
+  *out = idx.release();
+  return ZB200_OK;
+}
+
+int zb200_index_import(zb200_ctx *ctx, const uint8_t *src, size_t len, zb200_index **out) {
+  if (!ctx || !out || (len && !src)) return ZB200_ERR_ARG;
+  *out = nullptr;
+  try {
+    return index_import(ctx, src, len, out);
+  } catch (const std::bad_alloc &) {
+    return ZB200_ERR_NOMEM;
+  }
 }
 
 int zb200_last_timing(zb200_ctx *ctx, zb200_timing *out) {

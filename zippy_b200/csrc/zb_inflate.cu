@@ -734,6 +734,7 @@ __global__ void __launch_bounds__(INF_THREADS, INF_MIN_CTAS)
   g.b.overrun = false;
   g.op = g.cap = 0;
   g.out = nullptr;
+  uint32_t rec_k = 0;   // the recorder's next multiple of 32768 (counting instantiation only)
   for (;;) {
     int done = 1;  // status to report when `fin` is set
     bool fin = false;
@@ -790,6 +791,7 @@ __global__ void __launch_bounds__(INF_THREADS, INF_MIN_CTAS)
         g.b.overrun = false;
         br_seek(g.b, g.shift0, 0);
         br_skip<false>(g.b, (uint32_t)(sb & 7ull));
+        if (COUNT_ONLY && w.rec) rec_k = i == 0 ? 0u : (uint32_t)(w.rec_base[i] / 32768ull + 1ull);
         g.st = ST_BLOCK;
       } else {
         const uint64_t s0 = w.src_off[i], s1 = w.src_off[i + 1];
@@ -837,6 +839,18 @@ __global__ void __launch_bounds__(INF_THREADS, INF_MIN_CTAS)
         // The marker pass decodes that segment again as a closed one, up to the block boundary found here.)
         w.resume[0] = (uint64_t)(reinterpret_cast<const uint8_t *>(g.b.gbase) - w.src) * 8ull + br_consumed_abs(g.b);
         w.resume[1] = g.op;
+      }
+      if (COUNT_ONLY && w.rec && lane == 0) {
+        // an access point for every multiple of 32768 this block start is the first one at or past
+        const uint64_t o = w.rec_base[g.idx] + g.op;
+        if (rec_k < w.nrec && (uint64_t)rec_k * 32768ull <= o) {
+          const uint64_t bit = (uint64_t)(reinterpret_cast<const uint8_t *>(g.b.gbase) - w.src) * 8ull + br_consumed_abs(g.b);
+          do {
+            w.rec[2 * rec_k] = bit;
+            w.rec[2 * rec_k + 1] = o;
+            rec_k++;
+          } while (rec_k < w.nrec && (uint64_t)rec_k * 32768ull <= o);
+        }
       }
       int r = begin_block<COUNT_ONLY, OutT>(g, gs);
       if (r >= 0) {
@@ -1697,6 +1711,23 @@ cudaError_t zb_launch_resolve_groups(uint16_t *scr, const void *segs, uint32_t n
   k_resolve_tails_par<<<tgrid, 256, 0, s>>>(scr, sg, nseg, gsz, gin, dst);
   const uint32_t slabs = (max_n + 2047u) / 2048u;
   if (slabs) k_resolve_rest<<<resolve_rest_grid(nseg, slabs), 256, 0, s>>>(scr, sg, nseg, slabs, base, dst, bad);
+  return cudaGetLastError();
+}
+
+__global__ void __launch_bounds__(256) k_gather(const uint8_t *src, const ZbGather *gs, void *dst) {
+  const ZbGather g = gs[blockIdx.x];
+  const uint8_t *s = src + g.src;
+  if (g.wide) {
+    uint16_t *d = reinterpret_cast<uint16_t *>(dst) + g.dst;
+    for (uint32_t k = threadIdx.x; k < g.n; k += 256u) d[k] = s[k];
+  } else {
+    uint8_t *d = reinterpret_cast<uint8_t *>(dst) + g.dst;
+    for (uint32_t k = threadIdx.x; k < g.n; k += 256u) d[k] = s[k];
+  }
+}
+cudaError_t zb_launch_gather(const uint8_t *src, const ZbGather *g, uint32_t n, void *dst, cudaStream_t s) {
+  if (!n) return cudaSuccess;
+  k_gather<<<n, 256, 0, s>>>(src, g, dst);
   return cudaGetLastError();
 }
 

@@ -120,6 +120,14 @@ struct ZbInflateWork {
   // ZB_ERR_END_OF_BUFFER (the input ran out) or ZB_ERR_DST_TOO_SMALL (the count ran out), its output up to [1] is
   // complete and the stream resumes decoding at bit [0].
   uint64_t *resume;
+  // With seg_bits and count_only: null, or the access-point recorder of zb200_index_build.  rec_base [n + 1] (device)
+  // holds every segment's output offset in the member.  Segment 0 owns the multiples k * 32768 in [0, rec_base[1]],
+  // segment i > 0 those in (rec_base[i], rec_base[i + 1]]; for each owned k < nrec, rec[2k] / rec[2k + 1] receive the
+  // bit position in src and the member output offset of the segment's first block start at or past the multiple.
+  // A multiple that no block start of its segment reaches is left as it was (it belongs to the next segment's start).
+  uint64_t *rec;
+  const uint64_t *rec_base;
+  uint32_t nrec;
 };
 cudaError_t zb_launch_inflate(const ZbInflateWork &w, cudaStream_t s);
 // positions just past every byte sequence 00 00 ff ff (the empty stored block that byte-aligns a
@@ -148,6 +156,17 @@ cudaError_t zb_launch_resolve(const uint16_t *scr, const void *segs, uint32_t ns
 // gmap [ceil(nseg / gsz) x 32768] uint16, gin the same count of bytes.  Rewrites the tails in scr.
 cudaError_t zb_launch_resolve_groups(uint16_t *scr, const void *segs, uint32_t nseg, uint32_t max_n, uint32_t gsz, uint64_t base,
                                      uint64_t w0, uint16_t *gmap, uint8_t *gin, uint8_t *dst, int *bad, cudaStream_t s);
+
+// byte ranges copied from src to dst, at most ZB_GATHER_BYTES each; wide: dst is uint16 symbols (a window placed
+// in the marker scratch, each byte its own literal symbol) and dst counts elements
+#define ZB_GATHER_BYTES 65536u
+struct ZbGather {
+  uint64_t src;
+  uint64_t dst;
+  uint32_t n;
+  uint32_t wide;
+};
+cudaError_t zb_launch_gather(const uint8_t *src, const ZbGather *g, uint32_t n, void *dst, cudaStream_t s);
 
 // ---- checksums over a batch of buffers (standalone crc32/adler32, and the trailer
 // verification after inflate) ----
