@@ -56,7 +56,8 @@ enum {
   ZB200_ERR_DST_TOO_SMALL = 19,
   ZB200_ERR_CUDA = 20,
   ZB200_ERR_NOMEM = 21,
-  ZB200_ERR_ARG = 22
+  ZB200_ERR_ARG = 22,
+  ZB200_ERR_DICTIONARY = 23      /* a zlib member's DICTID is not the Adler-32 of the dictionary given */
 };
 
 /* CompressedDataFormat (src/zippy/common.nim:4-5), same ordinals */
@@ -141,6 +142,38 @@ int zb200_uncompress_batch(zb200_ctx *ctx, const uint8_t *src_base, const uint64
 int zb200_inflate_batch_crc32(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n,
                               uint8_t *dst_base, const uint64_t *dst_offsets, uint64_t *dst_lens, uint32_t *crcs,
                               int *statuses);
+/* ---- preset dictionaries (zlib's deflateSetDictionary / inflateSetDictionary, Python zlib's zdict) ----
+ * D = dict[0 .. dict_len), any length; the window W is its last min(32768, dict_len) bytes and DICTID is the
+ * Adler-32 of all of D.  dict_len == 0 is exactly the call without a dictionary (outputs and statuses).
+ * Dictionaries apply to zlib and raw DEFLATE; D is uploaded once per call and shared by every member.
+ *  - compress: a zlib member starts 78 20 DICTID (big-endian), so it is 4 bytes longer than without a dictionary
+ *    (bound: zb200_compress_bound(len, fmt) + 4); its trailer is the Adler-32 of the input alone.  At levels -1 and
+ *    2..9 the member's first chunk sees W as its history: the blocks are byte for byte what a compress stream of the
+ *    same level emits for the input after W was written and sync-flushed.  Levels 0, 1 and -2 keep no history:
+ *    their blocks are those without a dictionary.  gzip with a non-empty dictionary: ZB200_ERR_INVALID_FORMAT.
+ *  - decode: a raw stream S decodes (output and status) as uncompress(stored(W) || S, DEFLATE) without its first
+ *    |W| output bytes, stored(W) being the one non-final stored block 00 LEN ~LEN W: a distance may reach |W| bytes
+ *    in front of the output.  A zlib member with FDICT: ZB200_ERR_FDICT without a dictionary (dict_len 0, or the
+ *    calls without _dict), ZB200_ERR_UNCOMPRESS below 10 bytes, ZB200_ERR_DICTIONARY if its DICTID is not D's,
+ *    else its payload from byte 6 decodes as a raw stream above and the trailer is checked against the Adler-32 of
+ *    the output.  gzip members and zlib members without FDICT ignore the dictionary; DETECT works as without one.
+ *  - uncompress_batch_dict decodes every member whole, one 8-lane group per member (~10 MB/s each): members of
+ *    512 KiB and more are not cut into parallel segments.  decode_begin_dict (finished by zb200_decode_finish; raw
+ *    members start at byte 0) decodes stored(W) || payload through zb200_decode_begin's paths, so large members
+ *    decode in parallel wherever they do without a dictionary.
+ *  - compress_stream_begin_dict: a compress stream (below) whose history starts as W (LZ levels) and whose zlib
+ *    header carries DICTID; a full flush drops W with the rest of the history.  No FNAME: gzip is refused. */
+int zb200_compress_batch_dict(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n,
+                              int level, int data_format, const uint8_t *dict, size_t dict_len,
+                              uint8_t *dst_base, size_t dst_cap, uint64_t *dst_offsets, int *statuses);
+int zb200_uncompress_sizes_dict(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n,
+                                int data_format, const uint8_t *dict, size_t dict_len, uint64_t *sizes, int *statuses);
+int zb200_uncompress_batch_dict(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n,
+                                int data_format, const uint8_t *dict, size_t dict_len, uint8_t *dst_base,
+                                const uint64_t *dst_offsets, uint64_t *dst_lens, int *statuses);
+int zb200_decode_begin_dict(zb200_ctx *ctx, const uint8_t *src, size_t len, int data_format, const uint8_t *dict,
+                            size_t dict_len, size_t *out_len);
+
 /* crc32 (kind 0) or adler32 (kind 1) of every input */
 int zb200_checksum_batch(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n,
                          int kind, uint32_t *out);
@@ -184,6 +217,8 @@ int zb200_checksum_batch(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t
 enum { ZB200_SYNC_FLUSH = 2, ZB200_FULL_FLUSH = 3 };
 typedef struct zb200_compress_stream zb200_compress_stream;
 int zb200_compress_stream_begin(zb200_ctx *ctx, int level, int data_format, int fname_len, zb200_compress_stream **out);
+int zb200_compress_stream_begin_dict(zb200_ctx *ctx, int level, int data_format, const uint8_t *dict, size_t dict_len,
+                                     zb200_compress_stream **out);
 size_t zb200_compress_stream_bound(const zb200_compress_stream *st, size_t len);
 int zb200_compress_stream_write(zb200_compress_stream *st, const uint8_t *src, size_t len,
                                 uint8_t *dst, size_t dst_cap, size_t *dst_len);
@@ -229,6 +264,12 @@ void zb200_compress_stream_free(zb200_compress_stream *st);
  *  - free: at any time, finished or not. */
 typedef struct zb200_decompress_stream zb200_decompress_stream;
 int zb200_decompress_stream_begin(zb200_ctx *ctx, int data_format, zb200_decompress_stream **out);
+/* a decompress stream against a preset dictionary (see "preset dictionaries" above): what it returns, and its status,
+ * are zb200_decode_begin_dict's for the whole input.  A raw stream, or a zlib member whose FDICT carries D's DICTID,
+ * holds stored(W) in front of its payload once the header is decided; the window's bytes are never returned or
+ * checksummed.  gzip members and zlib members without FDICT ignore the dictionary. */
+int zb200_decompress_stream_begin_dict(zb200_ctx *ctx, int data_format, const uint8_t *dict, size_t dict_len,
+                                       zb200_decompress_stream **out);
 int zb200_decompress_stream_write(zb200_decompress_stream *st, const uint8_t *src, size_t len, size_t *avail);
 int zb200_decompress_stream_drain(zb200_decompress_stream *st, size_t *avail);
 int zb200_decompress_stream_finish(zb200_decompress_stream *st, size_t *avail);

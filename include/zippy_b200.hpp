@@ -55,6 +55,33 @@ inline void inflate(std::string &dst, const uint8_t *src, size_t len, size_t pos
 inline uint32_t read32le(const uint8_t *p) {
   return (uint32_t)p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16) | ((uint32_t)p[3] << 24);
 }
+inline uint32_t read32be(const uint8_t *p) {
+  return ((uint32_t)p[0] << 24) | ((uint32_t)p[1] << 16) | ((uint32_t)p[2] << 8) | p[3];
+}
+inline void put32be(std::string &dst, uint32_t v) {
+  for (int s = 24; s >= 0; s -= 8) dst.push_back((char)((v >> s) & 255));
+}
+// the raw stream of src against a preset dictionary (appended to dst): zb200_compress_batch_dict on one input
+inline void deflateDict(std::string &dst, const uint8_t *src, size_t len, int level, const std::string &dict) {
+  const uint64_t offs[2] = {0, len};
+  uint64_t out_offs[2] = {0, 0};
+  int st = 0;
+  size_t start = dst.size();
+  dst.resize(start + zb200_deflate_bound(len) + 64);
+  uint8_t dummy = 0;
+  check(zb200_compress_batch_dict(ctx(), len ? src : &dummy, offs, 1, level, ZB200_DF_DEFLATE, u8(dict), dict.size(),
+                                  reinterpret_cast<uint8_t *>(&dst[start]), dst.size() - start, out_offs, &st));
+  dst.resize(start + out_offs[1]);
+}
+// a raw stream decoded against a preset dictionary: zb200_decode_begin_dict + zb200_decode_finish
+inline void inflateDict(std::string &dst, const uint8_t *src, size_t len, const std::string &dict) {
+  size_t n = 0;
+  uint8_t dummy = 0;
+  check(zb200_decode_begin_dict(ctx(), len ? src : &dummy, len, ZB200_DF_DEFLATE, u8(dict), dict.size(), &n));
+  dst.resize(n);
+  check(zb200_decode_finish(ctx(), n ? reinterpret_cast<uint8_t *>(&dst[0]) : &dummy, n, &n));
+  dst.resize(n);
+}
 }  // namespace detail
 
 inline uint32_t crc32(const void *src, size_t len) {  // crc.nim:53
@@ -105,6 +132,28 @@ inline std::string compress(const void *srcp, size_t len, int level = DefaultCom
 inline std::string compress(const std::string &src, int level = DefaultCompression,
                             CompressedDataFormat dataFormat = dfGzip) {
   return compress(src.data(), src.size(), level, dataFormat);
+}
+// With a preset dictionary (zlib's zdict; include/zippy_b200.h "preset dictionaries"): zlib members start 78 20 and
+// the DICTID (the Adler-32 of the whole dictionary), raw members carry nothing, gzip is refused.  An empty dictionary
+// is the call without one.
+inline std::string compress(const void *srcp, size_t len, int level, CompressedDataFormat dataFormat,
+                            const std::string &dictionary) {
+  if (dictionary.empty()) return compress(srcp, len, level, dataFormat);
+  if (level < -2 || level > 9) throw ZippyError(ZB200_ERR_INVALID_LEVEL, "Invalid compression level");
+  if (dataFormat != dfZlib && dataFormat != dfDeflate) throw ZippyError(ZB200_ERR_INVALID_FORMAT, "Invalid data format");
+  const uint8_t *src = static_cast<const uint8_t *>(srcp);
+  std::string result;
+  if (dataFormat == dfZlib) {
+    result.assign({0x78, 0x20});
+    detail::put32be(result, adler32(dictionary));
+  }
+  detail::deflateDict(result, src, len, level, dictionary);
+  if (dataFormat == dfZlib) detail::put32be(result, adler32(src, len));
+  return result;
+}
+inline std::string compress(const std::string &src, int level, CompressedDataFormat dataFormat,
+                            const std::string &dictionary) {
+  return compress(src.data(), src.size(), level, dataFormat, dictionary);
 }
 
 // gzip.nim:3-88
@@ -170,6 +219,46 @@ inline std::string uncompress(const void *srcp, size_t len, CompressedDataFormat
 inline std::string uncompress(const std::string &src, CompressedDataFormat dataFormat = dfDetect) {
   return uncompress(src.data(), src.size(), dataFormat);
 }
+// With a preset dictionary: raw members, and zlib members with FDICT, decode against it (a DICTID that is not the
+// dictionary's: ZB200_ERR_DICTIONARY); gzip members and zlib members without FDICT ignore it.  An empty dictionary
+// is the call without one.
+inline std::string uncompress(const void *srcp, size_t len, CompressedDataFormat dataFormat,
+                              const std::string &dictionary) {
+  if (dictionary.empty()) return uncompress(srcp, len, dataFormat);
+  const uint8_t *src = static_cast<const uint8_t *>(srcp);
+  std::string result;
+  switch (dataFormat) {
+    case dfDetect:
+      if (len > 18 && src[0] == 31 && src[1] == 139 && src[2] == 8 && (src[3] & 0xe0) == 0)
+        return uncompress(src, len, dfGzip);
+      if (len > 6 && (src[0] & 0x0f) == 8 && (src[0] >> 4) <= 7 && (((uint32_t)src[0] * 256u) + src[1]) % 31u == 0)
+        return uncompress(src, len, dfZlib, dictionary);
+      throw ZippyError(ZB200_ERR_DETECT, "Unable to detect compressed data format");
+    case dfGzip:
+      return uncompress(src, len, dfGzip);
+    case dfZlib: {
+      if (len < 6 || !(src[1] & 0x20)) return uncompress(src, len, dfZlib);
+      uint8_t cmf = src[0], flg = src[1];
+      if ((cmf & 0x0f) != 8) throw ZippyError(ZB200_ERR_METHOD, "Unsupported compression method");
+      if ((cmf >> 4) > 7) throw ZippyError(ZB200_ERR_CINFO, "Invalid compression info");
+      if ((((uint32_t)cmf * 256u) + flg) % 31u != 0) throw ZippyError(ZB200_ERR_HEADER, "Invalid header");
+      if (len < 10) throw ZippyError(ZB200_ERR_UNCOMPRESS, "Invalid buffer, unable to uncompress");
+      if (detail::read32be(src + 2) != adler32(dictionary))
+        throw ZippyError(ZB200_ERR_DICTIONARY, zb200_strerror(ZB200_ERR_DICTIONARY));
+      detail::inflateDict(result, src + 6, len - 6, dictionary);
+      if (detail::read32be(src + len - 4) != adler32(result))
+        throw ZippyError(ZB200_ERR_CHECKSUM, "Checksum verification failed");
+      return result;
+    }
+    case dfDeflate:
+      detail::inflateDict(result, src, len, dictionary);
+      return result;
+  }
+  throw ZippyError(ZB200_ERR_INVALID_FORMAT, "Invalid data format");
+}
+inline std::string uncompress(const std::string &src, CompressedDataFormat dataFormat, const std::string &dictionary) {
+  return uncompress(src.data(), src.size(), dataFormat, dictionary);
+}
 
 // One GPU launch sequence for many inputs (no reference counterpart; cf. the loop over entries
 // in ziparchives.nim:505-540).
@@ -204,6 +293,11 @@ class CompressStream {
                           zb200_ctx *ctx = nullptr) {
     if (fnameLen < 0) fnameLen = dataFormat == dfGzip ? (int)(std::random_device()() % 26) : 0;
     detail::check(zb200_compress_stream_begin(ctx ? ctx : detail::ctx(), level, dataFormat, fnameLen, &st_));
+  }
+  // with a preset dictionary (zlib / raw; no FNAME): zb200_compress_stream_begin_dict
+  CompressStream(int level, CompressedDataFormat dataFormat, const std::string &dictionary, zb200_ctx *ctx = nullptr) {
+    detail::check(zb200_compress_stream_begin_dict(ctx ? ctx : detail::ctx(), level, dataFormat, detail::u8(dictionary),
+                                                   dictionary.size(), &st_));
   }
   ~CompressStream() { zb200_compress_stream_free(st_); }
   CompressStream(const CompressStream &) = delete;
@@ -247,6 +341,11 @@ class DecompressStream {
  public:
   explicit DecompressStream(CompressedDataFormat dataFormat = dfDetect, zb200_ctx *ctx = nullptr) {
     detail::check(zb200_decompress_stream_begin(ctx ? ctx : detail::ctx(), dataFormat, &st_));
+  }
+  // with a preset dictionary: zb200_decompress_stream_begin_dict
+  DecompressStream(CompressedDataFormat dataFormat, const std::string &dictionary, zb200_ctx *ctx = nullptr) {
+    detail::check(zb200_decompress_stream_begin_dict(ctx ? ctx : detail::ctx(), dataFormat, detail::u8(dictionary),
+                                                     dictionary.size(), &st_));
   }
   ~DecompressStream() { zb200_decompress_stream_free(st_); }
   DecompressStream(const DecompressStream &) = delete;

@@ -187,6 +187,90 @@ proc uncompress*(src: string, dataFormat = dfDetect): string {.inline, raises: [
 proc uncompress*(src: seq[uint8], dataFormat = dfDetect): seq[uint8] {.inline, raises: [ZippyError].} =
   cast[seq[uint8]](uncompress(cast[string](src), dataFormat))   # zippy.nim:173-177
 
+# ---- preset dictionaries (zlib's zdict; include/zippy_b200.h "preset dictionaries"): zlib members start 78 20 and
+# the DICTID (the Adler-32 of the whole dictionary), raw members carry nothing, gzip is refused; an empty
+# dictionary is the call without one ----
+proc zb200_compress_batch_dict(ctx: Zb200Ctx, srcBase: pointer, srcOffsets: ptr uint64, n: csize_t,
+                               level, dataFormat: cint, dict: pointer, dictLen: csize_t, dstBase: pointer,
+                               dstCap: csize_t, dstOffsets: ptr uint64, statuses: ptr cint): cint {.importc, cdecl, dynlib: lib.}
+proc zb200_decode_begin_dict(ctx: Zb200Ctx, src: pointer, len: csize_t, dataFormat: cint, dict: pointer,
+                             dictLen: csize_t, outLen: ptr csize_t): cint {.importc, cdecl, dynlib: lib.}
+
+proc deflateDict(dst: var string, src: pointer, len, level: int, dictionary: string) =
+  ## appends the raw stream of src against the dictionary (zb200_compress_batch_dict on one input)
+  var offs = [0'u64, len.uint64]
+  var outOffs = [0'u64, 0'u64]
+  var st: cint
+  var dummy: char
+  let start = dst.len
+  dst.setLen(start + zb200_deflate_bound(len.csize_t).int + 64)
+  check zb200_compress_batch_dict(getCtx(), (if len > 0: src else: dummy.addr), offs[0].addr, 1, level.cint,
+                                  dfDeflate.cint, dictionary.cstring, dictionary.len.csize_t, dst[start].addr,
+                                  (dst.len - start).csize_t, outOffs[0].addr, st.addr)
+  dst.setLen(start + outOffs[1].int)
+
+proc inflateDict(dst: var string, src: pointer, len: int, dictionary: string) =
+  ## a raw stream decoded against the dictionary (zb200_decode_begin_dict, then zb200_decode_finish)
+  var n: csize_t
+  var dummy: char
+  check zb200_decode_begin_dict(getCtx(), (if len > 0: src else: dummy.addr), len.csize_t, dfDeflate.cint,
+                                dictionary.cstring, dictionary.len.csize_t, n.addr)
+  dst.setLen(n.int)
+  check zb200_decode_finish(getCtx(), (if n > 0: dst[0].addr else: dummy.addr), n, n.addr)
+
+proc compress*(src: pointer, len: int, level: int, dataFormat: CompressedDataFormat,
+               dictionary: string): string {.raises: [ZippyError].} =
+  if dictionary.len == 0: return compress(src, len, level, dataFormat)
+  if level < -2 or level > 9: raise newException(ZippyError, "Invalid compression level")
+  if dataFormat notin {dfZlib, dfDeflate}: raise newException(ZippyError, "Invalid data format")
+  if dataFormat == dfZlib:
+    result.setLen(2)
+    result[0] = 0x78.char; result[1] = 0x20.char
+    let id = adler32(dictionary)
+    for s in [24, 16, 8, 0]: result.add(((id shr s) and 255).char)
+  deflateDict(result, src, len, level, dictionary)
+  if dataFormat == dfZlib:
+    let checksum = adler32(src, len)
+    for s in [24, 16, 8, 0]: result.add(((checksum shr s) and 255).char)
+
+proc compress*(src: string, level: int, dataFormat: CompressedDataFormat, dictionary: string): string =
+  compress(src.cstring, src.len, level, dataFormat, dictionary)
+
+proc uncompress*(src: pointer, len: int, dataFormat: CompressedDataFormat,
+                 dictionary: string): string {.raises: [ZippyError].} =
+  ## raw members, and zlib members with FDICT, decode against the dictionary; gzip members and zlib members
+  ## without FDICT ignore it
+  if dictionary.len == 0: return uncompress(src, len, dataFormat)
+  let s = cast[ptr UncheckedArray[uint8]](src)
+  case dataFormat
+  of dfDetect:
+    if len > 18 and s[0] == 31 and s[1] == 139 and s[2] == 8 and (s[3] and 0b11100000) == 0:
+      return uncompress(src, len, dfGzip)
+    if len > 6 and (s[0] and 0b00001111) == 8 and (s[0] shr 4) <= 7 and
+        ((s[0].uint16 * 256) + s[1].uint16) mod 31 == 0:
+      return uncompress(src, len, dfZlib, dictionary)
+    raise newException(ZippyError, "Unable to detect compressed data format")
+  of dfGzip:
+    return uncompress(src, len, dfGzip)
+  of dfZlib:
+    if len < 6 or (s[1] and 0b00100000) == 0: return uncompress(src, len, dfZlib)
+    let cmf = s[0]; let flg = s[1]
+    if (cmf and 0b00001111) != 8: raise newException(ZippyError, "Unsupported compression method")
+    if (cmf shr 4) > 7.uint8: raise newException(ZippyError, "Invalid compression info")
+    if ((cmf.uint16 * 256) + flg.uint16) mod 31 != 0: raise newException(ZippyError, "Invalid header")
+    if len < 10: failUncompress()
+    let id = (s[2].uint32 shl 24) or (s[3].uint32 shl 16) or (s[4].uint32 shl 8) or s[5].uint32
+    if id != adler32(dictionary): raise newException(ZippyError, $zb200_strerror(23))
+    inflateDict(result, s[6].addr, len - 6, dictionary)
+    let checksum = (s[len - 4].uint32 shl 24) or (s[len - 3].uint32 shl 16) or
+                   (s[len - 2].uint32 shl 8) or s[len - 1].uint32
+    if checksum != adler32(result): raise newException(ZippyError, "Checksum verification failed")
+  of dfDeflate:
+    inflateDict(result, src, len, dictionary)
+
+proc uncompress*(src: string, dataFormat: CompressedDataFormat, dictionary: string): string {.raises: [ZippyError].} =
+  uncompress(src.cstring, src.len, dataFormat, dictionary)
+
 # ---- batch (no counterpart in zippy.nim; what ziparchives.nim:505-540 should call instead of a
 # per-entry loop of crc32 + compress): N independent inputs, one GPU launch sequence ----
 proc zb200_compress_bound(len: csize_t, dataFormat: cint): csize_t {.importc, cdecl, dynlib: lib.}
@@ -275,6 +359,15 @@ proc newCompressStream*(level = DefaultCompression, dataFormat = dfGzip,
       k = (urand[0] mod 26).int
   check zb200_compress_stream_begin(getCtx(), level.cint, dataFormat.cint, k.cint, result.st.addr)
 
+proc zb200_compress_stream_begin_dict(ctx: Zb200Ctx, level, dataFormat: cint, dict: pointer, dictLen: csize_t,
+                                      st: ptr Zb200CompressStream): cint {.importc, cdecl, dynlib: lib.}
+
+proc newCompressStream*(level: int, dataFormat: CompressedDataFormat,
+                        dictionary: string): CompressStream {.raises: [ZippyError].} =
+  ## with a preset dictionary (zlib / raw; no FNAME): zb200_compress_stream_begin_dict
+  check zb200_compress_stream_begin_dict(getCtx(), level.cint, dataFormat.cint, dictionary.cstring,
+                                         dictionary.len.csize_t, result.st.addr)
+
 proc write*(s: var CompressStream, data: string): string {.raises: [ZippyError].} =
   ## small writes are gathered on the host and return ""
   result = newString(zb200_compress_stream_bound(s.st, data.len.csize_t).int + 1)
@@ -319,6 +412,14 @@ type DecompressStream* = object
 
 proc newDecompressStream*(dataFormat = dfDetect): DecompressStream {.raises: [ZippyError].} =
   check zb200_decompress_stream_begin(getCtx(), dataFormat.cint, result.st.addr)
+
+proc zb200_decompress_stream_begin_dict(ctx: Zb200Ctx, dataFormat: cint, dict: pointer, dictLen: csize_t,
+                                        st: ptr Zb200DecompressStream): cint {.importc, cdecl, dynlib: lib.}
+
+proc newDecompressStream*(dataFormat: CompressedDataFormat, dictionary: string): DecompressStream {.raises: [ZippyError].} =
+  ## with a preset dictionary: zb200_decompress_stream_begin_dict
+  check zb200_decompress_stream_begin_dict(getCtx(), dataFormat.cint, dictionary.cstring, dictionary.len.csize_t,
+                                           result.st.addr)
 
 proc take(s: var DecompressStream, avail: csize_t): string {.raises: [ZippyError].} =
   result = newString(avail.int + 1)

@@ -58,6 +58,13 @@ def _as_u8(buf):
     return np.frombuffer(bytes(buf) if not isinstance(buf, (bytes, bytearray, memoryview)) else buf, dtype=np.uint8)
 
 
+def _dict(dictionary):
+    """A preset dictionary (zlib's zdict) as a uint8 array; None and an empty dictionary give None: the calls
+    without a dictionary, as zlib writes no FDICT for an empty zdict."""
+    d = None if dictionary is None else _as_u8(dictionary)
+    return d if d is not None and d.size else None
+
+
 def _pack(items):
     """list of bytes-like -> (base uint8 array, offsets uint64[n+1])"""
     lens = np.fromiter((len(x) for x in items), dtype=np.uint64, count=len(items))
@@ -99,17 +106,25 @@ class Context:
             pass
 
     # ---- batches over host buffers -------------------------------------------------
-    def compress_batch(self, base, offsets, level=DefaultCompression, dataFormat=dfGzip, fname_lens=None):
-        """-> (out uint8 array, out_offsets uint64[n+1]).  fname_lens: per-input gzip FNAME letters (0..25)."""
+    def compress_batch(self, base, offsets, level=DefaultCompression, dataFormat=dfGzip, fname_lens=None,
+                       dictionary=None):
+        """-> (out uint8 array, out_offsets uint64[n+1]).  fname_lens: per-input gzip FNAME letters (0..25).
+        dictionary: a preset dictionary shared by every input (zlib / raw only; zb200_compress_batch_dict)."""
         L = _native.lib()
         base = _as_u8(base)
         offsets = np.ascontiguousarray(offsets, dtype=np.uint64)
         n = len(offsets) - 1
         bound = sum(L.zb200_compress_bound(int(offsets[i + 1] - offsets[i]), dataFormat) for i in range(n)) \
             if n <= 4096 else int(L.zb200_compress_bound(int(offsets[-1] - offsets[0]), dataFormat)) + 64 * n
-        out = np.empty(int(bound) + 64, dtype=np.uint8)
+        out = np.empty(int(bound) + (4 * n if _dict(dictionary) is not None else 0) + 64, dtype=np.uint8)
         out_offs = np.zeros(n + 1, dtype=np.uint64)
         st = np.zeros(max(n, 1), dtype=np.int32)
+        d = _dict(dictionary)
+        if d is not None:
+            _check(self._h, L.zb200_compress_batch_dict(self._h, base.ctypes.data, offsets.ctypes.data, n, level,
+                                                         dataFormat, d.ctypes.data, d.size, out.ctypes.data, out.size,
+                                                         out_offs.ctypes.data, st.ctypes.data))
+            return out[:int(out_offs[n])], out_offs
         fl = None
         if fname_lens is not None:
             fl = np.ascontiguousarray(fname_lens, dtype=np.uint8)
@@ -119,26 +134,33 @@ class Context:
         _check(self._h, rc)
         return out[:int(out_offs[n])], out_offs
 
-    def uncompressed_sizes(self, base, offsets, dataFormat=dfDetect):
+    def uncompressed_sizes(self, base, offsets, dataFormat=dfDetect, dictionary=None):
         L = _native.lib()
         base = _as_u8(base)
         offsets = np.ascontiguousarray(offsets, dtype=np.uint64)
         n = len(offsets) - 1
         sizes = np.zeros(max(n, 1), dtype=np.uint64)
         st = np.zeros(max(n, 1), dtype=np.int32)
+        d = _dict(dictionary)
+        if d is not None:
+            _check(self._h, L.zb200_uncompress_sizes_dict(self._h, base.ctypes.data, offsets.ctypes.data, n, dataFormat,
+                                                           d.ctypes.data, d.size, sizes.ctypes.data, st.ctypes.data))
+            return sizes[:n], st[:n]
         _check(self._h, L.zb200_uncompress_sizes(self._h, base.ctypes.data, offsets.ctypes.data, n, dataFormat,
                                                   sizes.ctypes.data, st.ctypes.data))
         return sizes[:n], st[:n]
 
-    def uncompress_batch(self, base, offsets, dataFormat=dfDetect, max_total=None, sizes=None):
+    def uncompress_batch(self, base, offsets, dataFormat=dfDetect, max_total=None, sizes=None, dictionary=None):
         """-> (out uint8 array, out_offsets uint64[n+1], out_lens uint64[n], statuses int32[n]).
-        `sizes`: uncompressed sizes known to the caller (a container's directory); skips the sizing pass."""
+        `sizes`: uncompressed sizes known to the caller (a container's directory); skips the sizing pass.
+        `dictionary`: a preset dictionary for every raw member and every zlib member with FDICT."""
         L = _native.lib()
         base = _as_u8(base)
         offsets = np.ascontiguousarray(offsets, dtype=np.uint64)
         n = len(offsets) - 1
+        d = _dict(dictionary)
         if sizes is None:
-            sizes, st0 = self.uncompressed_sizes(base, offsets, dataFormat)
+            sizes, st0 = self.uncompressed_sizes(base, offsets, dataFormat, dictionary=d)
         else:
             sizes, st0 = np.ascontiguousarray(sizes, dtype=np.uint64), np.zeros(n, dtype=np.int32)
         sizes = np.where(st0 == 0, sizes, 0).astype(np.uint64)
@@ -153,14 +175,20 @@ class Context:
         out = np.empty(int(dst_offs[n]) + 64, dtype=np.uint8)
         lens = np.zeros(max(n, 1), dtype=np.uint64)
         st = np.zeros(max(n, 1), dtype=np.int32)
-        _check(self._h, L.zb200_uncompress_batch(self._h, base.ctypes.data, offsets.ctypes.data, n, dataFormat,
-                                                  out.ctypes.data, dst_offs.ctypes.data, lens.ctypes.data,
-                                                  st.ctypes.data))
+        if d is None:
+            _check(self._h, L.zb200_uncompress_batch(self._h, base.ctypes.data, offsets.ctypes.data, n, dataFormat,
+                                                      out.ctypes.data, dst_offs.ctypes.data, lens.ctypes.data,
+                                                      st.ctypes.data))
+        else:
+            _check(self._h, L.zb200_uncompress_batch_dict(self._h, base.ctypes.data, offsets.ctypes.data, n, dataFormat,
+                                                           d.ctypes.data, d.size, out.ctypes.data, dst_offs.ctypes.data,
+                                                           lens.ctypes.data, st.ctypes.data))
         st = np.where(st0 != 0, st0, st[:n]).astype(np.int32)
-        out, dst_offs = self._redo_too_small(base, offsets, dataFormat, out[:int(dst_offs[n])], dst_offs, lens[:n], st)
+        out, dst_offs = self._redo_too_small(base, offsets, dataFormat, out[:int(dst_offs[n])], dst_offs, lens[:n], st,
+                                             dictionary=d)
         return out, dst_offs, lens[:n], st
 
-    def _redo_too_small(self, base, offsets, dataFormat, out, dst_offs, lens, st, crcs=None):
+    def _redo_too_small(self, base, offsets, dataFormat, out, dst_offs, lens, st, crcs=None, dictionary=None):
         """A size claim (gzip ISIZE, a container's directory) understated the content (status 19): the reference
         inflates anyway and lets its checksum / size checks decide (gzip.nim:80-88) -- redo those members one by
         one.  lens / st / crcs are updated in place; -> (out, dst_offs) with the redone outputs appended."""
@@ -172,7 +200,7 @@ class Context:
         dst_offs = dst_offs.copy()
         for i in small:
             try:
-                b = self.decode_one(base[int(offsets[i]):int(offsets[i + 1])], dataFormat)
+                b = self.decode_one(base[int(offsets[i]):int(offsets[i + 1])], dataFormat, dictionary=dictionary)
                 st[i] = 0
                 dst_offs[i] = end          # appended behind the slots; callers use out[off : off + len]
                 lens[i] = len(b)
@@ -295,13 +323,21 @@ class Context:
                                         ctypes.byref(n)))
         return out[:n.value].tobytes()
 
-    def decode_one(self, src, dataFormat=dfDetect, pos=0):
+    def decode_one(self, src, dataFormat=dfDetect, pos=0, dictionary=None):
         """One input of unknown size, decoded once: zb200_decode_begin (inflate + trailer check into device
-        memory, size reported) then zb200_decode_finish (copy out)."""
+        memory, size reported) then zb200_decode_finish (copy out).  With a dictionary: zb200_decode_begin_dict
+        (raw members start at byte 0, so pos must be 0)."""
         L = _native.lib()
         src = _as_u8(src)
         n = ctypes.c_size_t(0)
-        _check(self._h, L.zb200_decode_begin(self._h, src.ctypes.data, src.size, dataFormat, pos, ctypes.byref(n)))
+        d = _dict(dictionary)
+        if d is None:
+            _check(self._h, L.zb200_decode_begin(self._h, src.ctypes.data, src.size, dataFormat, pos, ctypes.byref(n)))
+        elif pos:
+            raise ZippyError(22, "a dictionary decode starts at byte 0")
+        else:
+            _check(self._h, L.zb200_decode_begin_dict(self._h, src.ctypes.data, src.size, dataFormat, d.ctypes.data,
+                                                       d.size, ctypes.byref(n)))
         out = np.empty(n.value + 8, dtype=np.uint8)
         m = ctypes.c_size_t(0)
         _check(self._h, L.zb200_decode_finish(self._h, out.ctypes.data, n.value, ctypes.byref(m)))
@@ -329,11 +365,17 @@ class CompressStream:
     gathered until a batch is pending, so most small writes return b"".  With gzip and fname_len=None the FNAME
     length is drawn at random, as compress() does (zippy.nim:28-42)."""
 
-    def __init__(self, level=DefaultCompression, dataFormat=dfGzip, fname_len=None, ctx=None):
-        if fname_len is None:
-            fname_len = os.urandom(1)[0] % 26 if dataFormat == dfGzip else 0
+    def __init__(self, level=DefaultCompression, dataFormat=dfGzip, fname_len=None, ctx=None, dictionary=None):
         self._ctx = ctx if ctx is not None else default_context()
         self._h = ctypes.c_void_p()
+        d = _dict(dictionary)
+        if d is not None:   # zb200_compress_stream_begin_dict: zlib / raw only, no FNAME
+            _check(self._ctx._h, _native.lib().zb200_compress_stream_begin_dict(self._ctx._h, level, dataFormat,
+                                                                                d.ctypes.data, d.size,
+                                                                                ctypes.byref(self._h)))
+            return
+        if fname_len is None:
+            fname_len = os.urandom(1)[0] % 26 if dataFormat == dfGzip else 0
         _check(self._ctx._h, _native.lib().zb200_compress_stream_begin(self._ctx._h, level, dataFormat, fname_len,
                                                                        ctypes.byref(self._h)))
 
@@ -389,9 +431,16 @@ class DecompressStream:
     input raises the ZippyError uncompress raises (at the latest from finish()).  Input is gathered until a batch is
     pending, so most small writes return b""."""
 
-    def __init__(self, dataFormat=dfDetect, ctx=None):
+    def __init__(self, dataFormat=dfDetect, ctx=None, dictionary=None):
+        """dictionary: a preset dictionary for a raw stream or a zlib member with FDICT
+        (zb200_decompress_stream_begin_dict)."""
         self._ctx = ctx if ctx is not None else default_context()
         self._h = ctypes.c_void_p()
+        d = _dict(dictionary)
+        if d is not None:
+            _check(self._ctx._h, _native.lib().zb200_decompress_stream_begin_dict(self._ctx._h, dataFormat, d.ctypes.data,
+                                                                                  d.size, ctypes.byref(self._h)))
+            return
         _check(self._ctx._h, _native.lib().zb200_decompress_stream_begin(self._ctx._h, dataFormat, ctypes.byref(self._h)))
 
     def _handle(self):
@@ -623,25 +672,25 @@ def default_context():
 
 
 # ---- the reference's public procs ------------------------------------------------------
-def compress(src, level=DefaultCompression, dataFormat=dfGzip):
-    """zippy.compress (zippy.nim:11-98)."""
+def compress(src, level=DefaultCompression, dataFormat=dfGzip, dictionary=None):
+    """zippy.compress (zippy.nim:11-98).  dictionary: a preset dictionary (zlib / raw only; zlib's zdict)."""
     if level < -2 or level > 9:
         raise ZippyError(1, "Invalid compression level %d" % level)          # deflate.nim:208-209
     if dataFormat not in (dfGzip, dfZlib, dfDeflate):
         raise ZippyError(2, "Invalid data format dfDetect")                  # zippy.nim:83-84
     fl = None
-    if dataFormat == dfGzip:
+    if dataFormat == dfGzip and _dict(dictionary) is None:
         fl = [os.urandom(1)[0] % 26]                                         # zippy.nim:28-42
     base, offs = _pack([src])
-    out, _ = default_context().compress_batch(base, offs, level, dataFormat, fl)
+    out, _ = default_context().compress_batch(base, offs, level, dataFormat, fl, dictionary=dictionary)
     return out.tobytes()
 
 
-def uncompress(src, dataFormat=dfDetect):
-    """zippy.uncompress (zippy.nim:100-177)."""
+def uncompress(src, dataFormat=dfDetect, dictionary=None):
+    """zippy.uncompress (zippy.nim:100-177).  dictionary: for raw members and zlib members with FDICT."""
     if dataFormat not in (dfDetect, dfZlib, dfGzip, dfDeflate):
         raise ZippyError(2)
-    return default_context().decode_one(src, dataFormat)
+    return default_context().decode_one(src, dataFormat, dictionary=dictionary)
 
 
 def crc32(src):
@@ -660,26 +709,26 @@ def inflate(src, pos=0):
     return default_context().inflate(src, pos)
 
 
-def compress_batch(items, level=DefaultCompression, dataFormat=dfGzip, fname_lens=None):
+def compress_batch(items, level=DefaultCompression, dataFormat=dfGzip, fname_lens=None, dictionary=None):
     """list of bytes -> list of bytes (one zippy.compress per item, one GPU launch sequence)."""
     base, offs = _pack(items)
-    out, oo = default_context().compress_batch(base, offs, level, dataFormat, fname_lens)
+    out, oo = default_context().compress_batch(base, offs, level, dataFormat, fname_lens, dictionary=dictionary)
     return [out[int(oo[i]):int(oo[i + 1])].tobytes() for i in range(len(items))]
 
 
-def uncompress_batch(items, dataFormat=dfDetect):
+def uncompress_batch(items, dataFormat=dfDetect, dictionary=None):
     """list of bytes -> list of (bytes | ZippyError)."""
     base, offs = _pack(items)
-    out, do, lens, st = default_context().uncompress_batch(base, offs, dataFormat)
+    out, do, lens, st = default_context().uncompress_batch(base, offs, dataFormat, dictionary=dictionary)
     res = []
     for i in range(len(items)):
         res.append(ZippyError(int(st[i])) if st[i] != 0 else out[int(do[i]):int(do[i]) + int(lens[i])].tobytes())
     return res
 
 
-def uncompressed_sizes(items, dataFormat=dfDetect):
+def uncompressed_sizes(items, dataFormat=dfDetect, dictionary=None):
     base, offs = _pack(items)
-    return default_context().uncompressed_sizes(base, offs, dataFormat)
+    return default_context().uncompressed_sizes(base, offs, dataFormat, dictionary=dictionary)
 
 
 def checksum_batch(items, kind="crc32"):

@@ -50,6 +50,14 @@ SYMBOLS = {
     "zb200_inflate_batch_crc32": (c_int, [ctypes.c_void_p, c_u8p, c_u64p, c_size_t, c_u8p, c_u64p, c_u64p,
                                           ctypes.c_void_p, c_intp]),
     "zb200_checksum_batch": (c_int, [ctypes.c_void_p, c_u8p, c_u64p, c_size_t, c_int, ctypes.c_void_p]),
+    "zb200_compress_batch_dict": (c_int, [ctypes.c_void_p, c_u8p, c_u64p, c_size_t, c_int, c_int, c_u8p, c_size_t, c_u8p,
+                                          c_size_t, c_u64p, c_intp]),
+    "zb200_uncompress_sizes_dict": (c_int, [ctypes.c_void_p, c_u8p, c_u64p, c_size_t, c_int, c_u8p, c_size_t, c_u64p,
+                                            c_intp]),
+    "zb200_uncompress_batch_dict": (c_int, [ctypes.c_void_p, c_u8p, c_u64p, c_size_t, c_int, c_u8p, c_size_t, c_u8p,
+                                            c_u64p, c_u64p, c_intp]),
+    "zb200_decode_begin_dict": (c_int, [ctypes.c_void_p, c_u8p, c_size_t, c_int, c_u8p, c_size_t,
+                                        ctypes.POINTER(c_size_t)]),
     "zb200_compress_batch_device": (c_int, [ctypes.c_void_p, c_u8p, c_u64p, c_size_t, c_int, c_int, c_u8p, c_u8p,
                                             c_size_t, c_u64p, c_intp]),
     "zb200_uncompress_batch_device": (c_int, [ctypes.c_void_p, c_u8p, c_u64p, c_size_t, c_int, c_u8p, c_u64p, c_u64p,
@@ -57,12 +65,16 @@ SYMBOLS = {
     "zb200_uncompress_sizes_device": (c_int, [ctypes.c_void_p, c_u8p, c_u64p, c_size_t, c_int, c_u64p, c_intp]),
     "zb200_checksum_batch_device": (c_int, [ctypes.c_void_p, c_u8p, c_u64p, c_size_t, c_int, ctypes.c_void_p]),
     "zb200_compress_stream_begin": (c_int, [ctypes.c_void_p, c_int, c_int, c_int, ctypes.POINTER(ctypes.c_void_p)]),
+    "zb200_compress_stream_begin_dict": (c_int, [ctypes.c_void_p, c_int, c_int, c_u8p, c_size_t,
+                                                 ctypes.POINTER(ctypes.c_void_p)]),
     "zb200_compress_stream_bound": (c_size_t, [ctypes.c_void_p, c_size_t]),
     "zb200_compress_stream_write": (c_int, [ctypes.c_void_p, c_u8p, c_size_t, c_u8p, c_size_t, ctypes.POINTER(c_size_t)]),
     "zb200_compress_stream_flush": (c_int, [ctypes.c_void_p, c_int, c_u8p, c_size_t, ctypes.POINTER(c_size_t)]),
     "zb200_compress_stream_finish": (c_int, [ctypes.c_void_p, c_u8p, c_size_t, ctypes.POINTER(c_size_t)]),
     "zb200_compress_stream_free": (None, [ctypes.c_void_p]),
     "zb200_decompress_stream_begin": (c_int, [ctypes.c_void_p, c_int, ctypes.POINTER(ctypes.c_void_p)]),
+    "zb200_decompress_stream_begin_dict": (c_int, [ctypes.c_void_p, c_int, c_u8p, c_size_t,
+                                                   ctypes.POINTER(ctypes.c_void_p)]),
     "zb200_decompress_stream_write": (c_int, [ctypes.c_void_p, c_u8p, c_size_t, ctypes.POINTER(c_size_t)]),
     "zb200_decompress_stream_drain": (c_int, [ctypes.c_void_p, ctypes.POINTER(c_size_t)]),
     "zb200_decompress_stream_finish": (c_int, [ctypes.c_void_p, ctypes.POINTER(c_size_t)]),

@@ -192,6 +192,13 @@ struct zb200_ctx {
   DevBuf idx_desc, idx_out;          // index build / extraction: gather descriptors, gathered bytes
   uint64_t index_group_bytes = kDstreamMaxOut;  // output budget of one extraction launch group (env ZB200_INDEX_GROUP_BYTES)
   bool index_log = false;            // env ZB200_INDEX_LOG: one stderr line per extraction launch group
+  // the preset dictionary of the *_dict call in progress (DictScope): its window W on the device, once as is
+  // (k_inflate) and once as the 16 alignment copies k_lz2 stages from (ZbCompressWork::win16); dict_on is false
+  // outside such a call, so every other call runs exactly as without dictionaries
+  DevBuf dict_win, dict_win16;
+  uint32_t dict_len = 0, dict_id = 0;
+  bool dict_on = false;
+  uint64_t pending_skip = 0;         // zb200_decode_begin_dict: output bytes in front of the result (the window)
   cudaEvent_t ev[10] = {};
   cudaStream_t h2d_stream = nullptr, d2h_stream = nullptr;
   std::vector<cudaEvent_t> gev;   // per-group events (H2D done, compute done, offsets ready)
@@ -216,6 +223,8 @@ struct zb200_compress_stream {
   size_t hist = 0;             // bytes of history (the LZ levels: the last <= 32 KiB compressed since the member
                                // start or the last full flush)
   ZbMemberCarry carry{0u, 1u, 0ull};  // the input compressed so far: raw CRC-32, Adler-32, bytes
+  bool has_dict = false;       // zlib: the header carries FDICT and dict_id
+  uint32_t dict_id = 0;
   bool head_done = false, finished = false;
   int err = ZB200_OK;          // a CUDA failure: the stream is unusable
 };
@@ -243,6 +252,11 @@ struct zb200_decompress_stream {
   bool finished = false;
   bool log = false;            // env ZB200_DSTREAM_LOG: one line per launch on stderr (which decode path ran)
   int err = ZB200_OK;          // once a write or finish failed, every later call reports it
+  // a preset dictionary (zb200_decompress_stream_begin_dict): its window W and DICTID; once the header is decided a raw
+  // stream, or a zlib member whose FDICT carries dict_id, holds stored(W) in front of its payload (dstream_header)
+  std::vector<uint8_t> dict_win;
+  uint32_t dict_id = 0;
+  bool has_dict = false;
 };
 
 namespace {
@@ -434,6 +448,58 @@ struct StreamPart {
   uint32_t hist;
   bool head, last;
   ZbMemberCarry carry_in, carry_out;
+  bool has_dict;       // a zlib header with FDICT and dict_id
+  uint32_t dict_id;
+};
+
+// Adler-32 on the host: the DICTID of a dictionary (zlib: the Adler-32 of all of it)
+uint32_t host_adler32(const uint8_t *p, size_t n) {
+  uint64_t a = 1, b = 0;
+  while (n) {
+    const size_t k = std::min<size_t>(n, 5552);
+    for (size_t i = 0; i < k; i++) {
+      a += p[i];
+      b += a;
+    }
+    a %= 65521;
+    b %= 65521;
+    p += k;
+    n -= k;
+  }
+  return (uint32_t)(b << 16 | a);
+}
+
+// A *_dict call's dictionary D: the window W (the last min(32768, |D|) bytes) is uploaded once for the call -- as
+// is for the decode calls, as the 16 copies of ZbCompressWork::win16 for an LZ-level compress, not at all for
+// compress at levels 0 / 1 / -2 (only the header carries D) -- and its DICTID is the Adler-32 of all of D.  An empty D leaves
+// the ctx as it is (the call is the one without a dictionary).  The destructor turns the dictionary off again.
+struct DictScope {
+  zb200_ctx *ctx;
+  explicit DictScope(zb200_ctx *c) : ctx(c) {}
+  // lz_compress: the call runs k_lz2 (the 16 copies); decode calls need W as is, compress at levels 0 / 1 / -2 neither
+  int set(const uint8_t *dict, size_t dict_len, bool lz_compress = false) {
+    if (!dict_len) return ZB200_OK;
+    zb200_ctx *ctx = this->ctx;   // (CK / ENSURE)
+    const uint32_t wl = (uint32_t)std::min<size_t>(dict_len, 32768);
+    const uint8_t *w = dict + (dict_len - wl);
+    if (lz_compress) {
+      const uint32_t stride = zb_win16_stride(wl);
+      std::vector<uint8_t> h16((size_t)16 * stride, 0);
+      for (uint32_t c = 0; c < 16; c++) memcpy(h16.data() + (size_t)c * stride + ZB_WIN16_SLACK + ((c - wl) & 15u), w, wl);
+      ENSURE(ctx->dict_win16, h16.size() + 64);
+      CK(cudaMemcpyAsync(ctx->dict_win16.p, h16.data(), h16.size(), cudaMemcpyHostToDevice, ctx->stream));
+      CK(cudaStreamSynchronize(ctx->stream));  // the host copies go out of scope
+    } else {
+      ENSURE(ctx->dict_win, wl + 64);
+      CK(cudaMemcpyAsync(ctx->dict_win.p, w, wl, cudaMemcpyHostToDevice, ctx->stream));
+      CK(cudaStreamSynchronize(ctx->stream));
+    }
+    ctx->dict_len = wl;
+    ctx->dict_id = host_adler32(dict, dict_len);
+    ctx->dict_on = true;
+    return ZB200_OK;
+  }
+  ~DictScope() { ctx->dict_on = false; }
 };
 
 // ---- compress: device-resident (h_src == h_dst == nullptr) or pipelined host buffers ----
@@ -463,6 +529,12 @@ int compress_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint8_t *h_src, 
   if (n == 0) return ZB200_OK;
   const uint64_t hist = sp ? sp->hist : 0;
   const bool head = !sp || sp->head, last = !sp || sp->last;
+  const bool lz = level == -1 || level >= 2;
+  // a batch's dictionary: every member's first chunk sees the window as its history (LZ levels), and zlib headers
+  // carry FDICT; a stream's dictionary is history in its own buffer, so only its header is the stream's business
+  const bool dict_hist = !sp && ctx->dict_on && lz;
+  const bool has_dict = data_format == ZB200_DF_ZLIB && (sp ? sp->has_dict : ctx->dict_on);
+  const uint32_t dict_id = sp ? sp->dict_id : ctx->dict_id;
   const uint64_t src_lo = src_offsets[0] - hist;  // d_src holds [src_lo, src_hi) rebased to 0 when staging from the host
   const bool src_pageable = h_src && is_pageable(h_src + src_lo), dst_pageable = h_dst && is_pageable(h_dst);
 
@@ -498,7 +570,11 @@ int compress_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint8_t *h_src, 
         d.len = (uint32_t)std::min<uint64_t>(ZB_CHUNK_BYTES, len - (uint64_t)k * ZB_CHUNK_BYTES);
         d.member = (uint32_t)(m1 - m0);
         d.flags = (k == 0 ? ZB_CHUNK_FIRST | (head ? ZB_CHUNK_HEAD : 0u) : 0u) | (k == nc - 1 && last ? ZB_CHUNK_LAST : 0u);
-        d.pad = (level == -1 || level >= 2) ? (uint32_t)std::min<uint64_t>(32768, hist + (uint64_t)k * ZB_CHUNK_BYTES) : 0u;
+        d.pad = lz ? (uint32_t)std::min<uint64_t>(32768, hist + (uint64_t)k * ZB_CHUNK_BYTES) : 0u;
+        if (dict_hist && k == 0) {
+          d.pad = ctx->dict_len;
+          d.flags |= ZB_CHUNK_DICT;
+        }
         desc.push_back(d);
       }
       g.bound += zb200_compress_bound((size_t)len, data_format) + 64;
@@ -530,7 +606,7 @@ int compress_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint8_t *h_src, 
   ENSURE(ctx->chunk_off, max_nc * sizeof(uint64_t));
   ENSURE(ctx->member_check, max_nm * sizeof(uint32_t));
   ENSURE(ctx->member_isize, max_nm * sizeof(uint32_t));
-  if (level == -1 || level >= 2) ENSURE(ctx->lz2_tables, zb_lz2_table_bytes(nullptr));
+  if (lz) ENSURE(ctx->lz2_tables, zb_lz2_table_bytes(nullptr));
   if (sp) ENSURE(ctx->carry, 2 * sizeof(ZbMemberCarry));
   {
     int rc = ensure_pinned(ctx, nfirst * sizeof(uint64_t) + sizeof(ZbMemberCarry) + 64);
@@ -585,6 +661,11 @@ int compress_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint8_t *h_src, 
     w.data_format = data_format;
     w.out_base = 0;
     w.out_base_ptr = (const uint64_t *)ctx->group_end.p + gi;
+    w.win16 = dict_hist ? (const uint8_t *)ctx->dict_win16.p : nullptr;
+    w.win_len = dict_hist ? ctx->dict_len : 0u;
+    w.win_stride = dict_hist ? zb_win16_stride(ctx->dict_len) : 0u;
+    w.dict_id = dict_id;
+    w.has_dict = has_dict ? 1 : 0;
     return w;
   };
 
@@ -692,6 +773,8 @@ int stream_run(zb200_compress_stream *st, size_t nbytes, bool last, uint8_t *dst
   sp.head = !st->head_done;
   sp.last = last;
   sp.carry_in = st->carry;
+  sp.has_dict = st->has_dict;
+  sp.dict_id = st->dict_id;
   int rc = compress_locked(ctx, (const uint8_t *)ctx->in_stage.p, st->buf.data(), offs, 1, st->level, st->data_format,
                            &st->fname_len, (uint8_t *)ctx->out_stage.p, ctx->out_stage.cap & ~(size_t)3, dst, dst_cap,
                            dst_offs, nullptr, ctx->host_group_chunks, &sp);
@@ -1383,7 +1466,7 @@ int dstream_header(zb200_decompress_stream *st, bool final) {
   uint32_t kind = 0, expect = 0, isize = 0;
   uint8_t dummy = 0;
   const int r = zb_parse_wrapper(st->in.empty() ? &dummy : st->in.data(), st->in.size(), st->data_format, 0, pos, kind,
-                                 expect, isize);
+                                 expect, isize, st->has_dict ? &st->dict_id : nullptr);
   if (r == ZB200_ERR_UNCOMPRESS && !final) return ZB200_OK;   // a gzip header longer than what is held so far
   if (r) return r;
   st->fmt = (int)kind;
@@ -1391,6 +1474,17 @@ int dstream_header(zb200_decompress_stream *st, bool final) {
   st->in.erase(st->in.begin(), st->in.begin() + (ptrdiff_t)pos);
   st->in_off = pos;
   st->bit0 = 0;
+  if (st->has_dict && (kind == ZB200_DF_DEFLATE || (kind == ZB200_DF_ZLIB && pos == 6))) {
+    // the payload decodes as stored(W) || payload (zb200_decode_begin_dict's definition): the stored block counts
+    // as held member bytes, and its |W| output bytes count as output already emitted, so dstream_run never emits
+    // them or folds them into the checksum -- yet they are the window the first blocks may reach into
+    const size_t wl = st->dict_win.size();
+    const uint8_t head[5] = {0, (uint8_t)wl, (uint8_t)(wl >> 8), (uint8_t)~wl, (uint8_t)(~wl >> 8)};
+    st->in.insert(st->in.begin(), st->dict_win.begin(), st->dict_win.end());
+    st->in.insert(st->in.begin(), head, head + 5);
+    st->total_in += 5 + wl;
+    st->out_total = wl;
+  }
   return ZB200_OK;
 }
 
@@ -1786,6 +1880,14 @@ bool longest_first_order(const uint64_t *src_offsets, size_t n, std::vector<uint
 // With d_crcs it is the plain crc32 configuration instead (no kinds, no expected values): d_crcs[i] gets the CRC-32 of
 // every output that inflated, raw deflate included, and nothing is compared -- a ZIP entry's CRC lives in the
 // archive's headers, not behind the stream.
+// the dictionary of the *_dict call in progress, if any, for a whole-member inflate launch
+void set_dict(const zb200_ctx *ctx, ZbInflateWork &w) {
+  if (!ctx->dict_on) return;
+  w.dict = (const uint8_t *)ctx->dict_win.p;
+  w.dict_len = ctx->dict_len;
+  w.dict_id = ctx->dict_id;
+}
+
 void set_check_pass(ZbChecksumWork &cw, const ZbInflateWork &w, uint32_t *d_crcs) {
   cw.src = w.dst;
   cw.off = w.dst_off;
@@ -1841,6 +1943,7 @@ int uncompress_device_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint64_
   w.skip = nullptr;
   w.seg_mode = 0;
   w.order = nullptr;
+  set_dict(ctx, w);
   {
     std::vector<uint32_t> order;
     if (longest_first_order(src_offsets, n, order)) {
@@ -1861,7 +1964,7 @@ int uncompress_device_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint64_
   // large member that did not work out) goes through the ordinary launch below
   std::vector<BigResult> big;
   std::vector<uint8_t> skip_host;
-  {
+  if (!ctx->dict_on) {  // with a dictionary every member is decoded whole, by k_inflate's dictionary instantiation
     int rc = inflate_big_members(ctx, d_src, src_offsets, n, data_format, raw_pos, d_dst, dst_offsets, count_only, big);
     if (rc) return rc;
     if (!big.empty()) {
@@ -2037,6 +2140,7 @@ int uncompress_host_pipelined(zb200_ctx *ctx, const uint8_t *h_src, const std::v
     w.gate_done = d_gate + 1;
     w.gate_first = d_gate + 1 + ng;
     w.n_gates = (uint32_t)ng;
+    set_dict(ctx, w);
     CK(zb_launch_inflate(w, s));
     // from here on the kernel may be waiting for copies: if this function leaves early (a failed copy, a failed
     // enqueue), open every gate so that the kernel drains instead of waiting out its timeout
@@ -2135,6 +2239,7 @@ int uncompress_host_pipelined(zb200_ctx *ctx, const uint8_t *h_src, const std::v
     w.n = (uint32_t)nm;
     w.data_format = data_format;
     w.order = has_order[gi] ? (const uint32_t *)ctx->order.p + m0 : nullptr;
+    set_dict(ctx, w);
     CK(zb_launch_inflate(w, s));
     // the checksum pass of every member that inflated
     ZbChecksumWork cw;
@@ -2368,7 +2473,7 @@ void zb200_shutdown(zb200_ctx *ctx) {
                     &ctx->src_off, &ctx->dst_off, &ctx->out_len, &ctx->status, &ctx->expect, &ctx->kind,
                     &ctx->counter, &ctx->ck_out, &ctx->ck_pieces, &ctx->ck_first, &ctx->ck_piece_out, &ctx->ck_partials, &ctx->in_stage, &ctx->out_stage, &ctx->lz2_tables, &ctx->carry,
                     &ctx->seg_src, &ctx->seg_dst, &ctx->seg_len, &ctx->seg_status, &ctx->seg_kind, &ctx->seg_expect, &ctx->seg_cand, &ctx->skip_mask, &ctx->order, &ctx->mark_scratch, &ctx->mark_segs, &ctx->seg_bits, &ctx->mark_win, &ctx->gate,
-                    &ctx->idx_desc, &ctx->idx_out};
+                    &ctx->idx_desc, &ctx->idx_out, &ctx->dict_win, &ctx->dict_win16};
   for (DevBuf *b : bufs)
     if (b->p) cudaFree(b->p);
   if (ctx->d_tabs) cudaFree(ctx->d_tabs);
@@ -2424,6 +2529,7 @@ const char *zb200_strerror(int s) {
     case ZB200_ERR_CUDA: return "CUDA error (no CPU fallback)";
     case ZB200_ERR_NOMEM: return "Out of device memory";
     case ZB200_ERR_ARG: return "Invalid argument";
+    case ZB200_ERR_DICTIONARY: return "Dictionary does not match the member's DICTID";
     default: return "unknown status";
   }
 }
@@ -2452,14 +2558,21 @@ int zb200_compress_batch_device(zb200_ctx *ctx, const uint8_t *d_src, const uint
   });
 }
 
-int zb200_compress_batch(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n, int level,
-                         int data_format, const uint8_t *fname_lens, uint8_t *dst_base, size_t dst_cap,
-                         uint64_t *dst_offsets, int *statuses) {
+// zb200_compress_batch, and with a non-empty dictionary zb200_compress_batch_dict
+static int compress_batch_host(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n, int level,
+                               int data_format, const uint8_t *dict, size_t dict_len, const uint8_t *fname_lens,
+                               uint8_t *dst_base, size_t dst_cap, uint64_t *dst_offsets, int *statuses) {
   return guarded(ctx, [&]() -> int {
-  if (!ctx || !src_offsets || !dst_offsets || (n && (!src_base || !dst_base))) return ZB200_ERR_ARG;
+  if (!ctx || !src_offsets || !dst_offsets || (n && (!src_base || !dst_base)) || (dict_len && !dict)) return ZB200_ERR_ARG;
+  if (dict_len) {  // zlib's deflateSetDictionary refuses gzip too: the format has no field for it
+    if (level < -2 || level > 9) return ZB200_ERR_INVALID_LEVEL;
+    if (data_format != ZB200_DF_ZLIB && data_format != ZB200_DF_DEFLATE) return ZB200_ERR_INVALID_FORMAT;
+  }
   std::lock_guard<std::mutex> lk(ctx->mu);
   DeviceGuard g(ctx->device);
   memset(&ctx->timing, 0, sizeof(ctx->timing));
+  DictScope ds(ctx);
+  if (int rc = ds.set(dict, dict_len, level == -1 || level >= 2)) return rc;
   if (n == 0) {
     dst_offsets[0] = 0;
     return ZB200_OK;
@@ -2482,6 +2595,20 @@ int zb200_compress_batch(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t
   ctx->timing.d2h_bytes = dst_offsets[n];
   return ZB200_OK;
   });
+}
+
+int zb200_compress_batch(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n, int level,
+                         int data_format, const uint8_t *fname_lens, uint8_t *dst_base, size_t dst_cap,
+                         uint64_t *dst_offsets, int *statuses) {
+  return compress_batch_host(ctx, src_base, src_offsets, n, level, data_format, nullptr, 0, fname_lens, dst_base, dst_cap,
+                             dst_offsets, statuses);
+}
+
+int zb200_compress_batch_dict(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n, int level,
+                              int data_format, const uint8_t *dict, size_t dict_len, uint8_t *dst_base, size_t dst_cap,
+                              uint64_t *dst_offsets, int *statuses) {
+  return compress_batch_host(ctx, src_base, src_offsets, n, level, data_format, dict, dict_len, nullptr, dst_base, dst_cap,
+                             dst_offsets, statuses);
 }
 
 // host inputs (pipelined H2D over launch groups) -> members left in device memory: the sharded
@@ -2513,13 +2640,17 @@ int zb200_compress_batch_h2d(zb200_ctx *ctx, const uint8_t *src_base, const uint
 }
 
 // ---- compress streams ----
-int zb200_compress_stream_begin(zb200_ctx *ctx, int level, int data_format, int fname_len, zb200_compress_stream **out) {
+// zb200_compress_stream_begin, and with a non-empty dictionary zb200_compress_stream_begin_dict: the window is the
+// history in front of the first chunk (LZ levels), exactly as after a sync flush of it, and zlib's header carries it
+static int compress_stream_begin(zb200_ctx *ctx, int level, int data_format, int fname_len, const uint8_t *dict,
+                                 size_t dict_len, zb200_compress_stream **out) {
   return guarded(ctx, [&]() -> int {
-    if (!ctx || !out) return ZB200_ERR_ARG;
+    if (!ctx || !out || (dict_len && !dict)) return ZB200_ERR_ARG;
     *out = nullptr;
     if (level < -2 || level > 9) return ZB200_ERR_INVALID_LEVEL;
     if (data_format != ZB200_DF_GZIP && data_format != ZB200_DF_ZLIB && data_format != ZB200_DF_DEFLATE)
       return ZB200_ERR_INVALID_FORMAT;
+    if (dict_len && data_format == ZB200_DF_GZIP) return ZB200_ERR_INVALID_FORMAT;
     if (fname_len < 0 || fname_len > 25) return ZB200_ERR_ARG;
     zb200_compress_stream *st = new zb200_compress_stream();
     st->ctx = ctx;
@@ -2531,13 +2662,30 @@ int zb200_compress_stream_begin(zb200_ctx *ctx, int level, int data_format, int 
       st->batch_bytes = ctx->stream_batch_bytes;
     }
     st->buf.reserve(65536);  // a non-null source even for an empty member
+    if (dict_len) {
+      st->has_dict = true;
+      st->dict_id = host_adler32(dict, dict_len);
+      if (level == -1 || level >= 2) {
+        st->hist = std::min<size_t>(dict_len, 32768);
+        st->buf.assign(dict + (dict_len - st->hist), dict + dict_len);
+      }
+    }
     *out = st;
     return ZB200_OK;
   });
 }
 
+int zb200_compress_stream_begin(zb200_ctx *ctx, int level, int data_format, int fname_len, zb200_compress_stream **out) {
+  return compress_stream_begin(ctx, level, data_format, fname_len, nullptr, 0, out);
+}
+
+int zb200_compress_stream_begin_dict(zb200_ctx *ctx, int level, int data_format, const uint8_t *dict, size_t dict_len,
+                                     zb200_compress_stream **out) {
+  return compress_stream_begin(ctx, level, data_format, 0, dict, dict_len, out);
+}
+
 size_t zb200_compress_stream_bound(const zb200_compress_stream *st, size_t len) {
-  return st ? zb200_compress_bound(st->buf.size() - st->hist + len, st->data_format) : 0;
+  return st ? zb200_compress_bound(st->buf.size() - st->hist + len, st->data_format) + (st->has_dict ? 4 : 0) : 0;
 }
 
 int zb200_compress_stream_write(zb200_compress_stream *st, const uint8_t *src, size_t len, uint8_t *dst, size_t dst_cap,
@@ -2610,14 +2758,21 @@ int zb200_compress_stream_finish(zb200_compress_stream *st, uint8_t *dst, size_t
 void zb200_compress_stream_free(zb200_compress_stream *st) { delete st; }
 
 // ---- decompress streams ----
-int zb200_decompress_stream_begin(zb200_ctx *ctx, int data_format, zb200_decompress_stream **out) {
+static int decompress_stream_begin(zb200_ctx *ctx, int data_format, const uint8_t *dict, size_t dict_len,
+                                   zb200_decompress_stream **out) {
   return guarded(ctx, [&]() -> int {
-    if (!ctx || !out) return ZB200_ERR_ARG;
+    if (!ctx || !out || (dict_len && !dict)) return ZB200_ERR_ARG;
     *out = nullptr;
     if (data_format < ZB200_DF_DETECT || data_format > ZB200_DF_DEFLATE) return ZB200_ERR_INVALID_FORMAT;
     zb200_decompress_stream *st = new zb200_decompress_stream();
     st->ctx = ctx;
     st->data_format = data_format;
+    if (dict_len) {
+      st->has_dict = true;
+      st->dict_id = host_adler32(dict, dict_len);
+      const size_t wl = std::min<size_t>(dict_len, 32768);
+      st->dict_win.assign(dict + (dict_len - wl), dict + dict_len);
+    }
     {
       std::lock_guard<std::mutex> lk(ctx->mu);
       st->batch_bytes = ctx->dstream_batch_bytes;
@@ -2627,6 +2782,15 @@ int zb200_decompress_stream_begin(zb200_ctx *ctx, int data_format, zb200_decompr
     *out = st;
     return ZB200_OK;
   });
+}
+
+int zb200_decompress_stream_begin(zb200_ctx *ctx, int data_format, zb200_decompress_stream **out) {
+  return decompress_stream_begin(ctx, data_format, nullptr, 0, out);
+}
+
+int zb200_decompress_stream_begin_dict(zb200_ctx *ctx, int data_format, const uint8_t *dict, size_t dict_len,
+                                       zb200_decompress_stream **out) {
+  return decompress_stream_begin(ctx, data_format, dict, dict_len, out);
 }
 
 static size_t dstream_avail(const zb200_decompress_stream *st) { return st->q.size() - st->q_head; }
@@ -2819,14 +2983,17 @@ int zb200_uncompress_sizes_device(zb200_ctx *ctx, const uint8_t *d_src, const ui
   });
 }
 
-int zb200_uncompress_sizes(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n,
-                           int data_format, uint64_t *sizes, int *statuses) {
+// zb200_uncompress_sizes, and with a non-empty dictionary zb200_uncompress_sizes_dict
+static int uncompress_sizes_host(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n,
+                                 int data_format, const uint8_t *dict, size_t dict_len, uint64_t *sizes, int *statuses) {
   return guarded(ctx, [&]() -> int {
-  if (!ctx || !src_offsets || !sizes || (n && !src_base)) return ZB200_ERR_ARG;
+  if (!ctx || !src_offsets || !sizes || (n && !src_base) || (dict_len && !dict)) return ZB200_ERR_ARG;
   if (data_format < ZB200_DF_DETECT || data_format > ZB200_DF_DEFLATE) return ZB200_ERR_INVALID_FORMAT;
   std::lock_guard<std::mutex> lk(ctx->mu);
   DeviceGuard g(ctx->device);
   memset(&ctx->timing, 0, sizeof(ctx->timing));
+  DictScope ds(ctx);
+  if (int rc = ds.set(dict, dict_len)) return rc;
   for (size_t i = 0; i < n; i++)
     if (src_offsets[i + 1] < src_offsets[i]) return ZB200_ERR_ARG;
   // gzip members answer from their trailer (gzip.nim:66) after the same wrapper checks the device decoder
@@ -2837,7 +3004,7 @@ int zb200_uncompress_sizes(zb200_ctx *ctx, const uint8_t *src_base, const uint64
     uint64_t payload = 0;
     uint32_t kind = 0, expect = 0, isize = 0;
     const int st = zb_parse_wrapper(src_base + src_offsets[i], src_offsets[i + 1] - src_offsets[i], data_format, 0, payload,
-                                    kind, expect, isize);
+                                    kind, expect, isize, ctx->dict_on ? &ctx->dict_id : nullptr);
     if (st == ZB200_OK && kind != ZB200_DF_GZIP) need_device = true;
     sizes[i] = st == ZB200_OK ? isize : 0;
     if (statuses) statuses[i] = st;
@@ -2851,15 +3018,28 @@ int zb200_uncompress_sizes(zb200_ctx *ctx, const uint8_t *src_base, const uint64
   });
 }
 
-// zb200_uncompress_batch, and with crcs (host, may be null) zb200_inflate_batch_crc32
+int zb200_uncompress_sizes(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n,
+                           int data_format, uint64_t *sizes, int *statuses) {
+  return uncompress_sizes_host(ctx, src_base, src_offsets, n, data_format, nullptr, 0, sizes, statuses);
+}
+
+int zb200_uncompress_sizes_dict(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n,
+                                int data_format, const uint8_t *dict, size_t dict_len, uint64_t *sizes, int *statuses) {
+  return uncompress_sizes_host(ctx, src_base, src_offsets, n, data_format, dict, dict_len, sizes, statuses);
+}
+
+// zb200_uncompress_batch, with crcs (host, may be null) zb200_inflate_batch_crc32, with a non-empty dictionary
+// zb200_uncompress_batch_dict
 static int uncompress_batch_host(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n,
                                  int data_format, uint8_t *dst_base, const uint64_t *dst_offsets, uint64_t *dst_lens,
-                                 int *statuses, uint32_t *crcs) {
+                                 int *statuses, uint32_t *crcs, const uint8_t *dict = nullptr, size_t dict_len = 0) {
   return guarded(ctx, [&]() -> int {
-  if (!ctx || !src_offsets || !dst_offsets || !dst_lens || (n && !src_base)) return ZB200_ERR_ARG;
+  if (!ctx || !src_offsets || !dst_offsets || !dst_lens || (n && !src_base) || (dict_len && !dict)) return ZB200_ERR_ARG;
   std::lock_guard<std::mutex> lk(ctx->mu);
   DeviceGuard g(ctx->device);
   memset(&ctx->timing, 0, sizeof(ctx->timing));
+  DictScope ds(ctx);
+  if (int rc = ds.set(dict, dict_len)) return rc;
   if (n == 0) return ZB200_OK;
   for (size_t i = 0; i < n; i++)
     if (src_offsets[i + 1] < src_offsets[i] || dst_offsets[i + 1] < dst_offsets[i]) return ZB200_ERR_ARG;
@@ -2909,7 +3089,7 @@ static int uncompress_batch_host(zb200_ctx *ctx, const uint8_t *src_base, const 
       for (size_t i = 0; i < n; i++) count += reb[i + 1] - reb[i] >= big_thr;
       if (count > 256) big_thr = std::max<uint64_t>(big_thr, 64ull << 20);
     }
-    for (size_t i = 0; i < n && !any_big; i++) any_big = reb[i + 1] - reb[i] >= big_thr;
+    for (size_t i = 0; i < n && !any_big && !ctx->dict_on; i++) any_big = reb[i + 1] - reb[i] >= big_thr;
     if (!any_big) {
       int rc = uncompress_host_pipelined(ctx, src_base + slo, reb, n, data_format, dst_base ? dst_base + lo : nullptr, dreb,
                                          dst_lens, statuses, gb, crcs);
@@ -2982,6 +3162,13 @@ int zb200_uncompress_batch(zb200_ctx *ctx, const uint8_t *src_base, const uint64
                                nullptr);
 }
 
+int zb200_uncompress_batch_dict(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n,
+                                int data_format, const uint8_t *dict, size_t dict_len, uint8_t *dst_base,
+                                const uint64_t *dst_offsets, uint64_t *dst_lens, int *statuses) {
+  return uncompress_batch_host(ctx, src_base, src_offsets, n, data_format, dst_base, dst_offsets, dst_lens, statuses,
+                               nullptr, dict, dict_len);
+}
+
 int zb200_inflate_batch_crc32(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n,
                               uint8_t *dst_base, const uint64_t *dst_offsets, uint64_t *dst_lens, uint32_t *crcs,
                               int *statuses) {
@@ -3023,8 +3210,11 @@ int zb200_checksum_batch(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t
 // reference's answer for a gzip member whose ISIZE understates its content: the data is produced, the CRC
 // is checked, then the size check fails (gzip.nim:80-88), instead of "destination too small".
 // decode_begin with the ctx locked: the member staged in in_stage, its output in out_stage (ctx->pending)
-static int decode_begin_locked(zb200_ctx *ctx, const uint8_t *src, size_t len, int data_format, size_t pos, size_t *out_len) {
+// pre (pre_len bytes, raw members only): the member decoded is pre || src, staged in place (zb200_decode_begin_dict)
+static int decode_begin_locked(zb200_ctx *ctx, const uint8_t *src, size_t len, int data_format, size_t pos, size_t *out_len,
+                               const uint8_t *pre = nullptr, size_t pre_len = 0) {
     ctx->pending = false;
+    ctx->pending_skip = 0;
     uint8_t dummy = 0;
     const uint8_t *sp = src ? src : &dummy;
     uint64_t payload = 0;
@@ -3033,10 +3223,22 @@ static int decode_begin_locked(zb200_ctx *ctx, const uint8_t *src, size_t len, i
     if (st != ZB200_OK) return st;
     uint64_t cap = kind == ZB200_DF_GZIP ? std::min<uint64_t>(isize, (uint64_t)len * 1032ull + 1024ull)
                                          : std::min<uint64_t>(std::max<uint64_t>((uint64_t)len * 8ull, 256ull << 10), 1ull << 30);
-    uint64_t so[2] = {0, len};
     std::vector<uint64_t> reb;
-    int rc = stage_in(ctx, sp, so, 1, reb);
-    if (rc) return rc;
+    int rc;
+    if (pre_len) {
+      len += pre_len;
+      cap = std::min<uint64_t>(cap + pre_len, (1ull << 30) + pre_len);
+      ENSURE(ctx->in_stage, len + 64);
+      CK(cudaMemcpyAsync(ctx->in_stage.p, pre, pre_len, cudaMemcpyHostToDevice, ctx->stream));
+      if (len > pre_len)
+        CK(cudaMemcpyAsync((uint8_t *)ctx->in_stage.p + pre_len, sp, len - pre_len, cudaMemcpyHostToDevice, ctx->stream));
+      ctx->timing.h2d_bytes = len;
+      reb = {0, (uint64_t)len};
+    } else {
+      uint64_t so[2] = {0, len};
+      rc = stage_in(ctx, sp, so, 1, reb);
+      if (rc) return rc;
+    }
     for (int attempt = 0; attempt < 2; attempt++) {
       ENSURE(ctx->out_stage, (size_t)cap + 64);
       uint64_t dof[2] = {0, cap}, dl = 0;
@@ -3073,6 +3275,63 @@ int zb200_decode_begin(zb200_ctx *ctx, const uint8_t *src, size_t len, int data_
   });
 }
 
+// decode_begin against a dictionary D (ctx locked).  A raw member S, or the payload of a zlib member whose FDICT
+// carries D's DICTID, is decoded as the raw member stored(W) || S through decode_begin_locked -- so every
+// single-member path (joints, speculative segments, serial) and its verdicts apply -- and the first |W| output bytes
+// are skipped.  A zlib member's trailer is then checked against the Adler-32 of the rest.  gzip members and zlib
+// members without FDICT ignore the dictionary.
+static int decode_begin_dict_locked(zb200_ctx *ctx, const uint8_t *src, size_t len, int data_format, const uint8_t *dict,
+                                    size_t dict_len, size_t *out_len) {
+  if (!dict_len) return decode_begin_locked(ctx, src, len, data_format, 0, out_len);
+  ctx->pending = false;
+  uint8_t dummy = 0;
+  const uint8_t *sp = src ? src : &dummy;
+  const uint32_t id = host_adler32(dict, dict_len);
+  uint64_t payload = 0;
+  uint32_t kind = 0, expect = 0, isize = 0;
+  int st = zb_parse_wrapper(sp, len, data_format, 0, payload, kind, expect, isize, &id);
+  if (st != ZB200_OK) return st;
+  if (kind == ZB200_DF_GZIP || (kind == ZB200_DF_ZLIB && payload == 2))
+    return decode_begin_locked(ctx, src, len, data_format, 0, out_len);
+  const size_t wl = std::min<size_t>(dict_len, 32768);
+  std::vector<uint8_t> pre(5 + wl);   // stored(W): one non-final stored block, staged in front of the payload
+  pre[0] = 0;
+  pre[1] = (uint8_t)wl;
+  pre[2] = (uint8_t)(wl >> 8);
+  pre[3] = (uint8_t)~wl;
+  pre[4] = (uint8_t)(~wl >> 8);
+  memcpy(pre.data() + 5, dict + (dict_len - wl), wl);
+  size_t n = 0;
+  st = decode_begin_locked(ctx, sp + payload, len - payload, ZB200_DF_DEFLATE, 0, &n, pre.data(), pre.size());
+  if (st != ZB200_OK) return st;
+  ctx->pending_skip = wl;
+  ctx->pending_len = n - wl;
+  if (kind == ZB200_DF_ZLIB) {
+    const uint64_t offs[2] = {0, ctx->pending_len};
+    uint32_t v = 0;
+    int rc = checksum_device_locked(ctx, (const uint8_t *)ctx->out_stage.p + wl, offs, 1, 1, &v);
+    if (rc) return rc;
+    if (v != expect) {
+      ctx->pending = false;
+      return ZB200_ERR_CHECKSUM;
+    }
+  }
+  *out_len = (size_t)ctx->pending_len;
+  return ZB200_OK;
+}
+
+int zb200_decode_begin_dict(zb200_ctx *ctx, const uint8_t *src, size_t len, int data_format, const uint8_t *dict,
+                            size_t dict_len, size_t *out_len) {
+  return guarded(ctx, [&]() -> int {
+    if (!ctx || !out_len || (len && !src) || (dict_len && !dict)) return ZB200_ERR_ARG;
+    if (data_format < ZB200_DF_DETECT || data_format > ZB200_DF_DEFLATE) return ZB200_ERR_INVALID_FORMAT;
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    DeviceGuard g(ctx->device);
+    memset(&ctx->timing, 0, sizeof(ctx->timing));
+    return decode_begin_dict_locked(ctx, src, len, data_format, dict, dict_len, out_len);
+  });
+}
+
 int zb200_decode_finish(zb200_ctx *ctx, uint8_t *dst, size_t dst_cap, size_t *dst_len) {
   return guarded(ctx, [&]() -> int {
     if (!ctx || !dst_len) return ZB200_ERR_ARG;
@@ -3082,7 +3341,8 @@ int zb200_decode_finish(zb200_ctx *ctx, uint8_t *dst, size_t dst_cap, size_t *ds
     if (ctx->pending_len > dst_cap) return ZB200_ERR_DST_TOO_SMALL;
     if (ctx->pending_len && !dst) return ZB200_ERR_ARG;
     if (ctx->pending_len) {
-      CK(cudaMemcpyAsync(dst, ctx->out_stage.p, (size_t)ctx->pending_len, cudaMemcpyDeviceToHost, ctx->stream));
+      CK(cudaMemcpyAsync(dst, (const uint8_t *)ctx->out_stage.p + ctx->pending_skip, (size_t)ctx->pending_len,
+                         cudaMemcpyDeviceToHost, ctx->stream));
       CK(cudaStreamSynchronize(ctx->stream));
     }
     *dst_len = (size_t)ctx->pending_len;

@@ -58,7 +58,8 @@ enum {
   ZB_ERR_DST_TOO_SMALL = 19,
   ZB_ERR_CUDA = 20,
   ZB_ERR_NOMEM = 21,
-  ZB_ERR_ARG = 22
+  ZB_ERR_ARG = 22,
+  ZB_ERR_DICTIONARY = 23
 };
 
 enum { ZB_DF_DETECT = 0, ZB_DF_ZLIB = 1, ZB_DF_GZIP = 2, ZB_DF_DEFLATE = 3 };

@@ -629,10 +629,46 @@ __device__ __forceinline__ void lz2_extend(const Lz2Pos &P, const uint8_t *data,
   if (m >= good && budget > 1) budget = 1;
 }
 
+// Stage a ZB_CHUNK_DICT chunk: its hb bytes of history are the end of the dictionary window W, the chunk itself
+// comes from src.  The region keeps the layout of zb_stage_chunk(rsrc, hb + len): region position q at
+// data[mis + q] with mis = (chunk start - hb) & 15, so the chunk's 16-byte granules start at the aligned offset
+// a0 = hb + mis - cmis.  win16's copy number cmis ends W at an address that is cmis modulo 16, so W's tail lines up
+// with the same granules: one bulk copy fills data[0, a0) from W, one fills data[a0, ..) from src (with the cmis
+// bytes of src in front of the chunk), and after the wait the <= 15 history bytes at q >= hb - cmis are stored
+// from W by plain stores.  Called by thread 0 (the copies) and then by every thread (fix_dict_head).
+__device__ __forceinline__ void stage_dict_chunk(uint8_t *data, const uint8_t *chunk, uint32_t len, uint32_t hb,
+                                                 const uint8_t *wend, uint64_t *bar) {
+  const uint32_t cmis = (uint32_t)((uintptr_t)chunk & 15u);
+  const uint32_t mis = (cmis - hb) & 15u, a0 = hb + mis - cmis;
+  const uint32_t cbytes = (cmis + len + 15u) & ~15u;
+  zb_mbar_expect_tx(bar, a0 + cbytes);
+  for (uint32_t done = 0; done < a0;) {
+    const uint32_t n = min(a0 - done, 32768u);
+    zb_tma_load_1d(data + done, wend - hb - mis + done, n, bar);
+    done += n;
+  }
+  for (uint32_t done = 0; done < cbytes;) {
+    const uint32_t n = min(cbytes - done, 32768u);
+    zb_tma_load_1d(data + a0 + done, chunk - cmis + done, n, bar);
+    done += n;
+  }
+}
+__device__ __forceinline__ void fix_dict_head(uint8_t *data, const uint8_t *chunk, uint32_t hb, const uint8_t *wend) {
+  const uint32_t cmis = (uint32_t)((uintptr_t)chunk & 15u);
+  const uint32_t mis = (cmis - hb) & 15u;
+  const uint32_t q = hb - min(hb, cmis) + threadIdx.x;
+  if (q < hb) {
+    data[mis + q] = wend[(int)q - (int)hb];
+    zb_fence_proxy_async();  // before the next chunk's bulk copies overwrite this byte
+  }
+}
+
+template <bool DICT>
 __global__ void __launch_bounds__(LZ_THREADS, 2)
     k_lz2(const uint8_t *__restrict__ src, const ZbChunkDesc *__restrict__ desc, uint2 *__restrict__ masks,
           uint32_t *__restrict__ recs, uint16_t *__restrict__ hist, ZbChunkCheck *__restrict__ chk,
-          const ZbCrcTables *__restrict__ tabs, uint2 *__restrict__ tables, uint32_t n_chunks, ZbLz2Params prm) {
+          const ZbCrcTables *__restrict__ tabs, uint2 *__restrict__ tables, uint32_t n_chunks, ZbLz2Params prm,
+          const uint8_t *__restrict__ win16, uint32_t win_len, uint32_t win_stride) {
   extern __shared__ __align__(128) uint8_t smem[];
   uint8_t *data = smem;
   uint32_t *hist_all = reinterpret_cast<uint32_t *>(smem + LZ2_SM_HIST);
@@ -671,7 +707,16 @@ __global__ void __launch_bounds__(LZ_THREADS, 2)
     const uint32_t mis = (uint32_t)((uintptr_t)rsrc & 15u);
     const uint32_t off0 = mis + hb;           // chunk position x lives at data[off0 + x]
     const uint32_t rlen = hb + len;           // staged bytes; region position q = hb + chunk position
-    if (tid == 0 && rlen) zb_stage_chunk(data, rsrc, rlen, bar);
+    const uint8_t *wend = nullptr;            // DICT: the end of W in the copy that matches the chunk's alignment
+    if (DICT && (d.flags & ZB_CHUNK_DICT)) {
+      const uint32_t c = (uint32_t)((uintptr_t)(src + d.src_off) & 15u);
+      wend = win16 + (size_t)c * win_stride + ZB_WIN16_SLACK + ((c - win_len) & 15u) + win_len;
+    }
+    if (DICT && wend) {
+      if (tid == 0) stage_dict_chunk(data, src + d.src_off, len, hb, wend, bar);
+    } else if (tid == 0 && rlen) {
+      zb_stage_chunk(data, rsrc, rlen, bar);
+    }
     for (int i = tid; i < ZB_WARPS_PER_CHUNK * ZB_HIST_WORDS; i += LZ_THREADS) hist_all[i] = 0;
     // every table starts empty for every chunk: what a member compresses to does not depend on which
     // chunks this CTA saw before (identical inputs give identical output wherever they sit in a batch)
@@ -680,6 +725,10 @@ __global__ void __launch_bounds__(LZ_THREADS, 2)
     if (rlen) {
       zb_mbar_wait(bar, phase);
       phase ^= 1u;
+    }
+    if (DICT && wend) {
+      fix_dict_head(data, src + d.src_off, hb, wend);
+      __syncthreads();
     }
 
     const uint32_t b0 = (uint32_t)warp * ZB_SUB_BYTES;
@@ -851,9 +900,9 @@ extern "C" int zb200_huff_stage_clocks(unsigned long long *out) {
 #endif
 
 // ------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t frame_head_bytes(int fmt, const uint8_t *fname_len, uint32_t m) {
+__device__ __forceinline__ uint32_t frame_head_bytes(int fmt, const uint8_t *fname_len, uint32_t m, int has_dict) {
   if (fmt == ZB_DF_GZIP) return 10u + (fname_len ? (uint32_t)fname_len[m] : 0u) + 1u;
-  if (fmt == ZB_DF_ZLIB) return 2u;
+  if (fmt == ZB_DF_ZLIB) return has_dict ? 6u : 2u;  // FDICT: DICTID follows CMF / FLG
   return 0u;
 }
 __device__ __forceinline__ uint32_t frame_tail_bytes(int fmt) {
@@ -878,7 +927,7 @@ __global__ void __launch_bounds__(SCAN_THREADS)
       member = d.member;
       sz = w.cb[c].total_bytes;
       if (flags & ZB_CHUNK_HEAD) {
-        head = frame_head_bytes(w.data_format, w.fname_len, member);
+        head = frame_head_bytes(w.data_format, w.fname_len, member, w.has_dict);
         sz += head;
       }
       if (flags & ZB_CHUNK_LAST) sz += frame_tail_bytes(w.data_format);
@@ -1102,6 +1151,11 @@ __global__ void __launch_bounds__(LZ_THREADS, 6)  // 6 CTAs (48 warps) per SM: <
       h[10 + k] = 0;
     } else if (w.data_format == ZB_DF_ZLIB) {
       h[0] = 0x78; h[1] = 0x01;
+      if (w.has_dict) {  // 0x7820 = 31 x 992: FDICT, FLEVEL 0, then the DICTID big-endian
+        const uint32_t id = w.dict_id;
+        h[1] = 0x20;
+        h[2] = (uint8_t)(id >> 24); h[3] = (uint8_t)(id >> 16); h[4] = (uint8_t)(id >> 8); h[5] = (uint8_t)id;
+      }
     }
   }
   if (tid == 64 && (d.flags & ZB_CHUNK_LAST)) {
@@ -1326,7 +1380,8 @@ cudaError_t zb_setup_deflate_attrs() {
       // three CTAs of 75 KiB: ask for the largest shared-memory carve-out
       if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
     }
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(k_lz2, cudaFuncAttributeMaxDynamicSharedMemorySize, LZ2_SM_TOTAL);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(k_lz2<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, LZ2_SM_TOTAL);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(k_lz2<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, LZ2_SM_TOTAL);
   // load the remaining kernels now rather than at their first launch (see zb_setup_inflate_attrs)
   cudaFuncAttributes fa;
   if (e == cudaSuccess) e = cudaFuncGetAttributes(&fa, k_huff);
@@ -1341,8 +1396,12 @@ cudaError_t zb_launch_lz(const ZbCompressWork &w, cudaStream_t s) {
     int grid = 0;
     (void)zb_lz2_table_bytes(&grid);
     if ((uint32_t)grid > w.n_chunks) grid = (int)w.n_chunks;
-    k_lz2<<<grid, LZ_THREADS, LZ2_SM_TOTAL, s>>>(w.src, w.desc, w.masks, w.recs, w.hist, w.chk, w.tabs, w.lz2_tables,
-                                                 w.n_chunks, zb_lz2_params(w.level));
+    if (w.win16)
+      k_lz2<true><<<grid, LZ_THREADS, LZ2_SM_TOTAL, s>>>(w.src, w.desc, w.masks, w.recs, w.hist, w.chk, w.tabs, w.lz2_tables,
+                                                         w.n_chunks, zb_lz2_params(w.level), w.win16, w.win_len, w.win_stride);
+    else
+      k_lz2<false><<<grid, LZ_THREADS, LZ2_SM_TOTAL, s>>>(w.src, w.desc, w.masks, w.recs, w.hist, w.chk, w.tabs, w.lz2_tables,
+                                                          w.n_chunks, zb_lz2_params(w.level), nullptr, 0u, 0u);
   } else {
     const ZbLzKernel k = zb_lz_kernel((w.level == -2 || w.level == 0) ? 0 : 1, w.data_format);
     k<<<w.n_chunks, LZ_THREADS, LZ_SM_TOTAL, s>>>(w.src, w.desc, w.masks, w.recs, w.hist, w.chk, w.tabs);

@@ -313,11 +313,19 @@ __device__ __forceinline__ uint32_t decode_clc(BitReader &b, const GroupSmem *gs
 // (zb_api.cu: speculative segments): the 32768 elements in front of `out` then hold marker symbols
 // 0x8000 | k standing for "byte k of the unknown window", copies move markers like literals, and `win`
 // (0 or 32768) is how far before its own start the segment may reach.
-template <bool COUNT_ONLY, typename OutT>
+// DICT (byte output only): a member decoded against a preset dictionary.  `win` is then the window length and wend
+// points just past the window W: output position p < 0 (relative to `out`) is the byte wend[p].  Every copy reads
+// through copy_src, so a match may lie in W, in the output, or straddle the two.
+template <bool DICT, typename OutT>
+__device__ __forceinline__ OutT copy_src(const OutT *out, const uint8_t *wend, int64_t p) {
+  if (DICT && p < 0) return (OutT)wend[p];
+  return out[p];
+}
+template <bool COUNT_ONLY, typename OutT, bool DICT = false>
 __device__ __forceinline__ int flush_tokens(OutT *out, uint32_t &op, uint32_t cap, uint32_t win,
                                             const uint32_t (&ta)[INF_ROUNDS], const uint32_t (&tb)[INF_ROUNDS],
                                             uint32_t ntok, uint32_t len_addr, uint32_t dist_addr, uint32_t &bad_k,
-                                            uint32_t &bad_back) {
+                                            uint32_t &bad_back, const uint8_t *wend = nullptr) {
   const int lane = g_lane();
   const uint32_t gsel = INF_G == 32 ? 0xffffffffu : ((1u << INF_G) - 1u);
   const uint32_t batch_op = op;
@@ -397,8 +405,14 @@ __device__ __forceinline__ int flush_tokens(OutT *out, uint32_t &op, uint32_t ca
     for (int r = 0; r < INF_ROUNDS; r++) {
       const OutT *from = bout + rel[r] - dist[r];
       const bool go = is_m[r] && !dep[r];
+      if (DICT) {
+        const int64_t p0 = (int64_t)batch_op + rel[r] - dist[r];
 #pragma unroll
-      for (int k = 0; k < 4; k++) v[r][k] = (go && (uint32_t)k < len[r]) ? from[k] : (OutT)0;
+        for (int k = 0; k < 4; k++) v[r][k] = (go && (uint32_t)k < len[r]) ? copy_src<DICT>(out, wend, p0 + k) : (OutT)0;
+      } else {
+#pragma unroll
+        for (int k = 0; k < 4; k++) v[r][k] = (go && (uint32_t)k < len[r]) ? from[k] : (OutT)0;
+      }
     }
 #pragma unroll
     for (int r = 0; r < INF_ROUNDS; r++) {
@@ -414,13 +428,18 @@ __device__ __forceinline__ int flush_tokens(OutT *out, uint32_t &op, uint32_t ca
       if (more & (1u << r)) {
         OutT *to = bout + rel[r];
         const OutT *from = to - dist[r];
-        for (uint32_t k = 4; k < len[r]; k += 4) {
-          OutT c0 = from[k], c1 = k + 1 < len[r] ? from[k + 1] : (OutT)0, c2 = k + 2 < len[r] ? from[k + 2] : (OutT)0,
-               c3 = k + 3 < len[r] ? from[k + 3] : (OutT)0;
-          to[k] = c0;
-          if (k + 1 < len[r]) to[k + 1] = c1;
-          if (k + 2 < len[r]) to[k + 2] = c2;
-          if (k + 3 < len[r]) to[k + 3] = c3;
+        if (DICT) {
+          const int64_t p0 = (int64_t)batch_op + rel[r] - dist[r];
+          for (uint32_t k = 4; k < len[r]; k++) to[k] = copy_src<DICT>(out, wend, p0 + k);
+        } else {
+          for (uint32_t k = 4; k < len[r]; k += 4) {
+            OutT c0 = from[k], c1 = k + 1 < len[r] ? from[k + 1] : (OutT)0, c2 = k + 2 < len[r] ? from[k + 2] : (OutT)0,
+                 c3 = k + 3 < len[r] ? from[k + 3] : (OutT)0;
+            to[k] = c0;
+            if (k + 1 < len[r]) to[k + 1] = c1;
+            if (k + 2 < len[r]) to[k + 2] = c2;
+            if (k + 3 < len[r]) to[k + 3] = c3;
+          }
         }
       }
     }
@@ -437,7 +456,10 @@ __device__ __forceinline__ int flush_tokens(OutT *out, uint32_t &op, uint32_t ca
       g_sync();
       OutT *tj = bout + rj;
       const OutT *fj = tj - dj;
-      if (dj >= lj) {
+      if (DICT) {
+        const int64_t p0 = (int64_t)batch_op + rj - dj;
+        for (uint32_t i = (uint32_t)lane; i < lj; i += INF_G) tj[i] = copy_src<DICT>(out, wend, p0 + (dj >= lj ? i : i % dj));
+      } else if (dj >= lj) {
         for (uint32_t i = (uint32_t)lane; i < lj; i += INF_G) tj[i] = fj[i];
       } else {
         for (uint32_t i = (uint32_t)lane; i < lj; i += INF_G) tj[i] = fj[i % dj];
@@ -594,8 +616,8 @@ __device__ __forceinline__ int begin_block(Grp<OutT> &g, GroupSmem *gs) {
 // slot k / INF_G) and then flushed; a group that reaches the end of its block idles until the
 // batch ends, the loop stops, and the caller resolves the event.
 // Returns 0 (another group stopped the loop), 1 (end of block) or 100 + ZB_ERR_*.
-template <bool COUNT_ONLY, typename OutT>
-__device__ __forceinline__ int symbol_loop(Grp<OutT> &g, const GroupSmem *gs, uint32_t tab_addr) {
+template <bool COUNT_ONLY, typename OutT, bool DICT = false>
+__device__ __forceinline__ int symbol_loop(Grp<OutT> &g, const GroupSmem *gs, uint32_t tab_addr, const uint8_t *wend = nullptr) {
   const int lane = g_lane();
   bool act = g.st == ST_SYMS;
   BitReader &b = g.b;
@@ -671,10 +693,11 @@ __device__ __forceinline__ int symbol_loop(Grp<OutT> &g, const GroupSmem *gs, ui
       }
     }
     uint32_t bad_k = 0, bad_back = 0;
-    // only the counting and the marker kernels ever see a segment with a window in front of it
-    const uint32_t win = (COUNT_ONLY || sizeof(OutT) == 2) ? g.win : 0u;
-    const int fev = flush_tokens<COUNT_ONLY, OutT>(g.out, op, g.cap, win, ta, tb, ntok, len_addr, dist_addr, bad_k,
-                                                    bad_back);
+    // only the counting and the marker kernels ever see a segment with a window in front of it (and the byte
+    // kernel's dictionary instantiation, a member with its dictionary window in front)
+    const uint32_t win = (COUNT_ONLY || sizeof(OutT) == 2 || DICT) ? g.win : 0u;
+    const int fev = flush_tokens<COUNT_ONLY, OutT, DICT>(g.out, op, g.cap, win, ta, tb, ntok, len_addr, dist_addr, bad_k,
+                                                          bad_back, wend);
     // a group that stopped: end of block (symbol 256), or a reader far past the end of its input
     ev = (act0 && !act) ? (b.overrun ? 100 + ZB_ERR_END_OF_BUFFER : 1) : 0;
     if (fev) {
@@ -702,7 +725,9 @@ __device__ __forceinline__ int symbol_loop(Grp<OutT> &g, const GroupSmem *gs, ui
 #ifndef INF_MIN_CTAS
 #define INF_MIN_CTAS 5   // register budget for 5 CTAs (20 warps) per SM, the shared-memory limit
 #endif
-template <bool COUNT_ONLY, bool MARK>
+// DICT: whole members decoded against w.dict (ZbInflateWork); <true, false, true> counts, <false, false, true>
+// writes bytes.  The instantiations without it compile as they did before the dictionary existed.
+template <bool COUNT_ONLY, bool MARK, bool DICT = false>
 __global__ void __launch_bounds__(INF_THREADS, INF_MIN_CTAS)
     k_inflate(ZbInflateWork w) {
   typedef typename std::conditional<MARK, uint16_t, uint8_t>::type OutT;
@@ -805,7 +830,14 @@ __global__ void __launch_bounds__(INF_THREADS, INF_MIN_CTAS)
         uint32_t isize = 0;
         g.kind = 0;
         g.expect = 0;
-        int st = zb_parse_wrapper(g.src, g.len, w.data_format, w.pos, pos, g.kind, g.expect, isize);
+        int st;
+        if (DICT) {
+          st = zb_parse_wrapper(g.src, g.len, w.data_format, w.pos, pos, g.kind, g.expect, isize, &w.dict_id);
+          // raw members, and zlib members whose FDICT was accepted (payload at 6), see the window
+          g.win = (g.kind == ZB_DF_DEFLATE || (g.kind == ZB_DF_ZLIB && pos == 6)) ? w.dict_len : 0u;
+        } else {
+          st = zb_parse_wrapper(g.src, g.len, w.data_format, w.pos, pos, g.kind, g.expect, isize);
+        }
         if (st == ZB_OK && COUNT_ONLY && g.kind == ZB_DF_GZIP) {
           g.op = isize;  // gzip.nim:66 (trustSize's source)
           fin = true;
@@ -878,7 +910,7 @@ __global__ void __launch_bounds__(INF_THREADS, INF_MIN_CTAS)
     // run the lockstep symbol loop only when no group of the warp is waiting for a header or a
     // new member: those are short, and would otherwise stall behind a whole block of symbols
     if (__any_sync(FULL_MASK, g.st == ST_FETCH || g.st == ST_BLOCK)) continue;
-    const int ev = symbol_loop<COUNT_ONLY, OutT>(g, gs, tab_addr);
+    const int ev = symbol_loop<COUNT_ONLY, OutT, DICT>(g, gs, tab_addr, DICT ? w.dict + w.dict_len : nullptr);
     if (g.st == ST_SYMS && ev) {
       int st = ZB_OK;
       if (ev == 1) {
@@ -1749,6 +1781,8 @@ cudaError_t zb_setup_inflate_attrs() {
   cudaError_t e = cudaFuncSetAttribute(k_inflate<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(k_inflate<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(k_inflate<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(k_inflate<true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(k_inflate<false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(k_resolve_tails, cudaFuncAttributeMaxDynamicSharedMemorySize, 32768);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(k_resolve_groups, cudaFuncAttributeMaxDynamicSharedMemorySize, ZB_RS_WIN * 2);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(k_piece_checksum<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, CK_SM_TOTAL);
@@ -1781,7 +1815,10 @@ cudaError_t zb_launch_inflate(const ZbInflateWork &w, cudaStream_t s) {
   if (blocks > need) blocks = need;
   cudaError_t e = cudaMemsetAsync(w.counter, 0, sizeof(uint32_t), s);
   if (e != cudaSuccess) return e;
-  if (w.count_only) k_inflate<true, false><<<blocks, INF_THREADS, smem, s>>>(w);
+  if (w.dict && !w.seg_bits) {
+    if (w.count_only) k_inflate<true, false, true><<<blocks, INF_THREADS, smem, s>>>(w);
+    else k_inflate<false, false, true><<<blocks, INF_THREADS, smem, s>>>(w);
+  } else if (w.count_only) k_inflate<true, false><<<blocks, INF_THREADS, smem, s>>>(w);
   else if (w.mark) k_inflate<false, true><<<blocks, INF_THREADS, smem, s>>>(w);
   else k_inflate<false, false><<<blocks, INF_THREADS, smem, s>>>(w);
   return cudaGetLastError();

@@ -19,6 +19,7 @@ struct ZbChunkDesc {
 #define ZB_CHUNK_LAST 2u   // last chunk of its member: BFINAL, then the trailer
 #define ZB_CHUNK_HEAD 4u   // the member's gzip / zlib header goes in front of this chunk (a stream's later
                            // launches continue a member whose header an earlier launch wrote: FIRST without HEAD)
+#define ZB_CHUNK_DICT 8u   // k_lz2: the chunk's `pad` bytes of history are the end of the dictionary window, not src
 
 // The part of a member compressed before this launch (a compress stream): raw CRC-32 and Adler-32 of its
 // bytes and their count.  The empty prefix is {0, 1, 0}.
@@ -59,7 +60,16 @@ struct ZbCompressWork {
   uint2 *lz2_tables;           // k_lz2 dictionaries: [grid][8 own tables of 2048 x 4 ways + 12 segment tables of 8192 entries], u16 positions (LZ levels only)
   uint32_t n_chunks, n_members;
   int level, data_format;
+  // A preset dictionary (zb200_compress_batch_dict): has_dict puts FDICT and dict_id in the zlib header.  win16 holds
+  // 16 copies of the window W (win_len bytes; win16 256-byte aligned), copy c at
+  // win16 + c * win_stride + ZB_WIN16_SLACK + ((c - win_len) & 15), so that W ends at an address that is c modulo 16;
+  // chunks flagged ZB_CHUNK_DICT stage their history from copy (chunk start & 15).
+  const uint8_t *win16;
+  uint32_t win_len, win_stride, dict_id;
+  int has_dict;
 };
+#define ZB_WIN16_SLACK 16u   // bytes in front of each copy in win16 (the bulk copies read whole 16-byte granules)
+static inline uint32_t zb_win16_stride(uint32_t win_len) { return ((win_len + 15u) & ~15u) + 3u * ZB_WIN16_SLACK; }
 
 // per-device kernel attributes (dynamic shared memory limits); call with the device current
 cudaError_t zb_setup_deflate_attrs();
@@ -128,6 +138,11 @@ struct ZbInflateWork {
   uint64_t *rec;
   const uint64_t *rec_base;
   uint32_t nrec;
+  // A preset dictionary (whole members only, not seg_bits): null, or the device copy of its window W (the last
+  // dict_len <= 32768 bytes of the dictionary).  Raw members, and zlib members whose FDICT carries dict_id, decode
+  // as if W were output in front of their first byte; gzip and zlib members without FDICT ignore it.
+  const uint8_t *dict;
+  uint32_t dict_len, dict_id;
 };
 cudaError_t zb_launch_inflate(const ZbInflateWork &w, cudaStream_t s);
 // positions just past every byte sequence 00 00 ff ff (the empty stored block that byte-aligns a

@@ -10,8 +10,11 @@ ZB_HD uint32_t zb_ld_le32(const uint8_t *p) {
 
 // zippy.nim:100-165 + gzip.nim:3-66: resolve the format, validate the wrapper, find the
 // payload start and the trailer checksum.  On the device all lanes of a group run this redundantly.
+// dict_id: null (no dictionary: FDICT is ZB_ERR_FDICT), or the DICTID (Adler-32) of the caller's non-empty
+// dictionary: a zlib member with FDICT then needs 10 bytes and that DICTID, and its payload starts at byte 6.
 ZB_HD int zb_parse_wrapper(const uint8_t *src, uint64_t len, int fmt, uint64_t raw_pos,
-                                             uint64_t &pos, uint32_t &kind, uint32_t &expect, uint32_t &isize) {
+                                             uint64_t &pos, uint32_t &kind, uint32_t &expect, uint32_t &isize,
+                                             const uint32_t *dict_id = nullptr) {
   expect = 0;
   isize = 0;
   if (fmt == ZB_DF_DETECT) {
@@ -52,9 +55,15 @@ ZB_HD int zb_parse_wrapper(const uint8_t *src, uint64_t len, int fmt, uint64_t r
     if ((cmf & 0x0f) != 8) return ZB_ERR_METHOD;
     if ((cmf >> 4) > 7) return ZB_ERR_CINFO;
     if ((cmf * 256u + flg) % 31u != 0) return ZB_ERR_HEADER;
-    if (flg & 0x20) return ZB_ERR_FDICT;
-    expect = ((uint32_t)src[len - 4] << 24) | ((uint32_t)src[len - 3] << 16) | ((uint32_t)src[len - 2] << 8) | src[len - 1];
     pos = 2;
+    if (flg & 0x20) {
+      if (!dict_id) return ZB_ERR_FDICT;
+      if (len < 10) return ZB_ERR_UNCOMPRESS;
+      const uint32_t id = ((uint32_t)src[2] << 24) | ((uint32_t)src[3] << 16) | ((uint32_t)src[4] << 8) | src[5];
+      if (id != *dict_id) return ZB_ERR_DICTIONARY;
+      pos = 6;
+    }
+    expect = ((uint32_t)src[len - 4] << 24) | ((uint32_t)src[len - 3] << 16) | ((uint32_t)src[len - 2] << 8) | src[len - 1];
     return ZB_OK;
   }
   if (fmt == ZB_DF_DEFLATE) {
