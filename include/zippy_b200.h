@@ -391,6 +391,7 @@ typedef struct {
   uint64_t h2d_bytes, d2h_bytes;
   uint32_t kernel_launches;
   uint32_t n_chunks;
+  float plan_ms;                               /* compress: host time from entry to the first kernel launch */
 } zb200_timing;
 int zb200_last_timing(zb200_ctx *ctx, zb200_timing *out);
 

@@ -18,7 +18,7 @@ class Timing(ctypes.Structure):
                 ("pack_ms", ctypes.c_float), ("inflate_ms", ctypes.c_float), ("verify_ms", ctypes.c_float),
                 ("checksum_ms", ctypes.c_float), ("h2d_ms", ctypes.c_float), ("d2h_ms", ctypes.c_float),
                 ("h2d_bytes", ctypes.c_uint64), ("d2h_bytes", ctypes.c_uint64),
-                ("kernel_launches", ctypes.c_uint32), ("n_chunks", ctypes.c_uint32)]
+                ("kernel_launches", ctypes.c_uint32), ("n_chunks", ctypes.c_uint32), ("plan_ms", ctypes.c_float)]
 
 
 # name -> (restype, argtypes); every symbol include/zippy_b200.h declares

@@ -12,6 +12,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <chrono>
 #include <cmath>
 #include <condition_variable>
 #include <deque>
@@ -435,7 +436,6 @@ struct Group {
   size_t c0, nc;        // chunks [c0, c0 + nc) in the batch-wide descriptor array
   size_t first0;        // start of this group's (nm + 1) entries in the member_first / member_off arrays
   uint64_t in_lo, in_hi;  // source byte range
-  uint64_t bound;       // output bound of the group
 };
 
 // One launch of a compress stream (zb200_compress_stream_*): a run of chunks of ONE member that continues
@@ -511,6 +511,7 @@ int compress_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint8_t *h_src, 
                     size_t n, int level, int data_format, const uint8_t *fname_lens, uint8_t *d_dst,
                     size_t dst_cap, uint8_t *h_dst, size_t h_dst_cap, uint64_t *dst_offsets, int *statuses,
                     size_t max_group_chunks, StreamPart *sp = nullptr) {
+  const auto t_entry = std::chrono::steady_clock::now();
   if (level < -2 || level > 9) return ZB200_ERR_INVALID_LEVEL;
   if (data_format != ZB200_DF_GZIP && data_format != ZB200_DF_ZLIB && data_format != ZB200_DF_DEFLATE)
     return ZB200_ERR_INVALID_FORMAT;
@@ -519,11 +520,8 @@ int compress_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint8_t *h_src, 
       if (fname_lens[i] > 25) return ZB200_ERR_ARG;
   if (((uintptr_t)d_dst & 3u) != 0) return ZB200_ERR_ARG;
   dst_cap &= ~(size_t)3;  // the packer writes whole 32-bit words: never touch a word that straddles the end
-  for (size_t i = 0; i < n; i++) {
-    if (src_offsets[i + 1] < src_offsets[i]) return ZB200_ERR_ARG;
-    if (statuses) statuses[i] = ZB200_OK;
-  }
-  ctx->timing.lz_ms = ctx->timing.huff_ms = ctx->timing.scan_ms = ctx->timing.pack_ms = 0.f;
+  if (src_offsets[n] < src_offsets[0]) return ZB200_ERR_ARG;  // each member's offsets are checked by the plan
+  ctx->timing.lz_ms = ctx->timing.huff_ms = ctx->timing.scan_ms = ctx->timing.pack_ms = ctx->timing.plan_ms = 0.f;
   ctx->timing.n_chunks = 0;
   dst_offsets[0] = 0;
   if (n == 0) return ZB200_OK;
@@ -539,15 +537,29 @@ int compress_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint8_t *h_src, 
   const bool src_pageable = h_src && is_pageable(h_src + src_lo), dst_pageable = h_dst && is_pageable(h_dst);
 
   // ---- plan: groups, descriptors ----
-  std::vector<Group> groups;
-  std::vector<ZbChunkDesc> desc;
-  std::vector<uint32_t> first;
-  size_t max_nc = 0, max_nm = 0;
-  size_t chunks_left = 0;
-  for (size_t i = 0; i < n; i++) {
-    uint64_t len = src_offsets[i + 1] - src_offsets[i];
-    chunks_left += len == 0 ? 1 : (size_t)((len + ZB_CHUNK_BYTES - 1) / ZB_CHUNK_BYTES);
+  // One pass over the members validates their offsets and writes the descriptors and member_first entries straight
+  // into pinned memory, so that their upload is a true asynchronous copy; the member offsets come back at its
+  // start.  With offsets that do not decrease a member of len bytes has at most len / 64 KiB + 1 chunks, so the
+  // batch at most nc_cap; member_first holds n entries plus one per group, and a group holds at least one member.
+  auto chunks_of = [](uint64_t len) { return len == 0 ? (size_t)1 : (size_t)((len + ZB_CHUNK_BYTES - 1) / ZB_CHUNK_BYTES); };
+  const size_t nc_cap = n + (size_t)((src_offsets[n] - src_offsets[0]) / ZB_CHUNK_BYTES), nfirst_cap = 2 * n;
+  {
+    int rc = ensure_pinned(ctx, nfirst_cap * (sizeof(uint64_t) + sizeof(uint32_t)) + sizeof(ZbMemberCarry) +
+                                    nc_cap * sizeof(ZbChunkDesc) + 64);
+    if (rc) return rc;
   }
+  uint64_t *pin_off = (uint64_t *)ctx->pin;
+  ZbMemberCarry *pin_carry = (ZbMemberCarry *)(pin_off + nfirst_cap);  // a stream's carry-out comes back behind the offsets
+  ZbChunkDesc *desc = (ZbChunkDesc *)(pin_carry + 1);
+  uint32_t *first = (uint32_t *)(desc + nc_cap);
+  std::vector<Group> groups;
+  size_t max_nc = 0, max_nm = 0;
+  size_t nd = 0, nfirst = 0;  // entries of desc / first written so far
+  // the host pipeline sizes its groups by the chunks still to come (a wrong count from decreasing offsets is never
+  // used: the plan stops at the first such member)
+  size_t chunks_left = 0;
+  if (h_src)
+    for (size_t i = 0; i < n; i++) chunks_left += chunks_of(src_offsets[i + 1] - src_offsets[i]);
   const size_t group_cap = max_group_chunks;
   for (size_t m0 = 0; m0 < n;) {
     // host pipeline: the work after the last H2D (kernels + D2H of the last group) is not overlapped
@@ -555,17 +567,19 @@ int compress_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint8_t *h_src, 
     if (h_src) max_group_chunks = std::min(group_cap, std::max<size_t>(512, chunks_left / 2));
     Group g;
     g.m0 = m0;
-    g.c0 = desc.size();
-    g.first0 = first.size();
-    g.bound = 0;
+    g.c0 = nd;
+    g.first0 = nfirst;
     size_t m1 = m0;
     while (m1 < n) {
+      if (src_offsets[m1 + 1] < src_offsets[m1]) return ZB200_ERR_ARG;
       uint64_t len = src_offsets[m1 + 1] - src_offsets[m1];
-      size_t nc = len == 0 ? 1 : (size_t)((len + ZB_CHUNK_BYTES - 1) / ZB_CHUNK_BYTES);
-      if (desc.size() > g.c0 && desc.size() - g.c0 + nc > max_group_chunks) break;
-      first.push_back((uint32_t)(desc.size() - g.c0));
+      size_t nc = chunks_of(len);
+      if (nd + nc > nc_cap) return ZB200_ERR_ARG;  // only offsets that decrease further on get here
+      if (nd > g.c0 && nd - g.c0 + nc > max_group_chunks) break;
+      if (statuses) statuses[m1] = ZB200_OK;
+      first[nfirst++] = (uint32_t)(nd - g.c0);
       for (size_t k = 0; k < nc; k++) {
-        ZbChunkDesc d;
+        ZbChunkDesc &d = desc[nd++];
         d.src_off = src_offsets[m1] - (h_src ? src_lo : 0) + (uint64_t)k * ZB_CHUNK_BYTES;
         d.len = (uint32_t)std::min<uint64_t>(ZB_CHUNK_BYTES, len - (uint64_t)k * ZB_CHUNK_BYTES);
         d.member = (uint32_t)(m1 - m0);
@@ -575,15 +589,13 @@ int compress_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint8_t *h_src, 
           d.pad = ctx->dict_len;
           d.flags |= ZB_CHUNK_DICT;
         }
-        desc.push_back(d);
       }
-      g.bound += zb200_compress_bound((size_t)len, data_format) + 64;
       m1++;
     }
     g.m1 = m1;
-    g.nc = desc.size() - g.c0;
+    g.nc = nd - g.c0;
     chunks_left -= std::min(chunks_left, g.nc);
-    first.push_back((uint32_t)g.nc);
+    first[nfirst++] = (uint32_t)g.nc;
     g.in_lo = m0 == 0 ? 0 : src_offsets[m0] - src_lo;  // the first group also copies a stream's history
     g.in_hi = src_offsets[m1] - src_lo;
     max_nc = std::max(max_nc, g.nc);
@@ -591,7 +603,7 @@ int compress_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint8_t *h_src, 
     groups.push_back(g);
     m0 = m1;
   }
-  const size_t ng = groups.size(), nc_all = desc.size(), nfirst = first.size();
+  const size_t ng = groups.size(), nc_all = nd;
 
   ENSURE(ctx->desc, nc_all * sizeof(ZbChunkDesc));
   ENSURE(ctx->member_first, nfirst * sizeof(uint32_t));
@@ -609,19 +621,21 @@ int compress_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint8_t *h_src, 
   if (lz) ENSURE(ctx->lz2_tables, zb_lz2_table_bytes(nullptr));
   if (sp) ENSURE(ctx->carry, 2 * sizeof(ZbMemberCarry));
   {
-    int rc = ensure_pinned(ctx, nfirst * sizeof(uint64_t) + sizeof(ZbMemberCarry) + 64);
-    if (rc) return rc;
-    rc = ensure_group_events(ctx, 3 * ng + 1);
+    int rc = ensure_group_events(ctx, 3 * ng + 1);
     if (rc) return rc;
   }
-  uint64_t *pin_off = (uint64_t *)ctx->pin;
-  ZbMemberCarry *pin_carry = (ZbMemberCarry *)(pin_off + nfirst);  // a stream's carry-out comes back behind the offsets
   ZbMemberCarry *d_carry = (ZbMemberCarry *)ctx->carry.p;          // [0] in, [1] out
 
   cudaStream_t s = ctx->stream;
   cudaStream_t sh = h_src ? ctx->h2d_stream : s, sd = h_dst ? ctx->d2h_stream : s;
-  CK(cudaMemcpyAsync(ctx->desc.p, desc.data(), nc_all * sizeof(ZbChunkDesc), cudaMemcpyHostToDevice, s));
-  CK(cudaMemcpyAsync(ctx->member_first.p, first.data(), nfirst * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
+  // the next call writes its plan into the same pinned memory: no return, an early one included, leaves a copy
+  // from or to it running on s
+  struct SyncOnReturn {
+    cudaStream_t s;
+    ~SyncOnReturn() { cudaStreamSynchronize(s); }
+  } sync_on_return{s};
+  CK(cudaMemcpyAsync(ctx->desc.p, desc, nc_all * sizeof(ZbChunkDesc), cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(ctx->member_first.p, first, nfirst * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
   if (fname_lens && data_format == ZB200_DF_GZIP)
     CK(cudaMemcpyAsync(ctx->fname.p, fname_lens, n, cudaMemcpyHostToDevice, s));
   if (sp) CK(cudaMemcpyAsync(d_carry, &sp->carry_in, sizeof(ZbMemberCarry), cudaMemcpyHostToDevice, s));
@@ -705,7 +719,10 @@ int compress_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint8_t *h_src, 
     }
     ZbCompressWork w = make_work(g, gi);
     const bool timed = (gi == 0);  // per-kernel events on the first group; totals are scaled by chunk count
-    if (timed) CK(cudaEventRecord(ctx->ev[0], s));
+    if (timed) {
+      ctx->timing.plan_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t_entry).count();
+      CK(cudaEventRecord(ctx->ev[0], s));
+    }
     CK(zb_launch_lz(w, s));
     if (timed) CK(cudaEventRecord(ctx->ev[1], s));
     CK(zb_launch_huff(w, s));

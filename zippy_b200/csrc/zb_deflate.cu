@@ -1254,16 +1254,25 @@ __global__ void __launch_bounds__(LZ_THREADS, 6)  // 6 CTAs (48 warps) per SM: <
           const uint32_t bbase = b0 + (wbase << 5);
           const uint32_t *pw = reinterpret_cast<const uint32_t *>(src + bbase - mis);
           const uint32_t nword = min(1024u, b1 - bbase) + mis;  // 4 * (words to load) covers this many bytes
-#pragma unroll 1
-          for (uint32_t k = (uint32_t)lane; 4u * k < nword; k += 32) {
-            const uint32_t v = __ldg(pw + k);
-            uint32_t *q = stg + PK_LIT_OFF + k + (k >> 3);  // word k % 8 of slot k / 8
-            if (k < 256u) *q = v;
-            if (k && (k & 7u) == 0u) q[-1] = v;            // and the ninth word of the slot before
+          // every load is issued before the first store, so the batch waits for global memory once, not 8 times
+          uint32_t v[8];
+#pragma unroll
+          for (uint32_t j = 0; j < 8; j++) {
+            const uint32_t k = (uint32_t)lane + 32u * j;
+            v[j] = 4u * k < nword ? __ldg(pw + k) : 0u;
           }
+#pragma unroll
+          for (uint32_t j = 0; j < 8; j++) {
+            const uint32_t k = (uint32_t)lane + 32u * j;
+            uint32_t *q = stg + PK_LIT_OFF + k + (k >> 3);  // word k % 8 of slot k / 8
+            if (4u * k < nword) *q = v[j];
+            if (4u * k < nword && k && (k & 7u) == 0u) q[-1] = v[j];  // and the ninth word of the slot before
+          }
+          // word 256 (a misaligned source): only the ninth word of the last slot
+          if (lane == 0 && 4u * 256u < nword) stg[PK_LIT_OFF + 256 + 32 - 1] = __ldg(pw + 256);
           const uint32_t *brec = grecs + rec_base;
-#pragma unroll 1
-          for (uint32_t k = (uint32_t)lane; k < rtot; k += 32) stg[PK_REC_OFF + k] = brec[k];
+#pragma unroll 4
+          for (uint32_t k = (uint32_t)lane; k < rtot; k += 32) stg[PK_REC_OFF + k] = __ldg(brec + k);
         }
         rec_base += rtot;
         __syncwarp();
