@@ -331,6 +331,28 @@ void zb200_index_free(zb200_index *idx);
 int zb200_index_export(zb200_ctx *ctx, const zb200_index *idx, uint8_t *dst, size_t cap, size_t *len);
 int zb200_index_import(zb200_ctx *ctx, const uint8_t *src, size_t len, zb200_index **out);
 
+/* ---- an index written while compressing (no decode pass) ----
+ * zb200_compress_batch_index / zb200_compress_batch_device_index take zb200_compress_batch's /
+ * zb200_compress_batch_device's arguments plus span and indexes (n entries), and write the same members as those
+ * calls.  indexes[i] receives a new index of member i (free it with zb200_index_free) that exports to exactly the
+ * bytes zb200_index_build(member i, data_format, span) + zb200_index_export give, or NULL where statuses[i] != 0
+ * (every entry is NULL when the call fails).  The points come from the block layout the compressor wrote, the
+ * interval CRC-32s from the chunk checksums, the windows from the input.
+ * zb200_compress_stream_begin_index begins a stream as zb200_compress_stream_begin does that also writes the index;
+ * zb200_compress_stream_index, valid only after zb200_compress_stream_finish on such a stream (anything else is
+ * ZB200_ERR_ARG), returns a new index of the whole member.  span: a multiple of 32768, at least 32768, else
+ * ZB200_ERR_ARG before any work; an invalid level or format is reported as by the calls without an index. */
+int zb200_compress_batch_index(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n, int level,
+                               int data_format, const uint8_t *fname_lens, uint8_t *dst_base, size_t dst_cap,
+                               uint64_t *dst_offsets, int *statuses, uint64_t span, zb200_index **indexes);
+int zb200_compress_batch_device_index(zb200_ctx *ctx, const uint8_t *d_src, const uint64_t *src_offsets, size_t n,
+                                      int level, int data_format, const uint8_t *fname_lens, uint8_t *d_dst,
+                                      size_t dst_cap, uint64_t *dst_offsets, int *statuses, uint64_t span,
+                                      zb200_index **indexes);
+int zb200_compress_stream_begin_index(zb200_ctx *ctx, int level, int data_format, int fname_len, uint64_t span,
+                                      zb200_compress_stream **out);
+int zb200_compress_stream_index(zb200_compress_stream *st, zb200_index **out);
+
 /* ---- device-resident variants (pointers prefixed d_ are device memory on ctx's device;
  * offsets / statuses / sizes stay host arrays).  Used when the data already lives in HBM
  * (bench.py's `value`) and by the multi-GPU sharded path.  The call returns after the

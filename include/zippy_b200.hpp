@@ -287,6 +287,7 @@ inline std::vector<std::string> compressBatch(const std::vector<std::string> &it
 // counterpart): what write() and finish() return, concatenated, is the member compressBatch writes for the whole
 // input with the same FNAME length.  Small writes are gathered and return "".  fnameLen < 0 with gzip draws the
 // FNAME length at random, as compress() does; ctx nullptr is this thread's default context.
+class Index;
 class CompressStream {
  public:
   explicit CompressStream(int level = DefaultCompression, CompressedDataFormat dataFormat = dfGzip, int fnameLen = -1,
@@ -298,6 +299,12 @@ class CompressStream {
   CompressStream(int level, CompressedDataFormat dataFormat, const std::string &dictionary, zb200_ctx *ctx = nullptr) {
     detail::check(zb200_compress_stream_begin_dict(ctx ? ctx : detail::ctx(), level, dataFormat, detail::u8(dictionary),
                                                    dictionary.size(), &st_));
+  }
+  // that also writes the member's index (zb200_compress_stream_begin_index): index() after finish()
+  CompressStream(int level, CompressedDataFormat dataFormat, int fnameLen, uint64_t indexSpan, zb200_ctx *ctx = nullptr)
+      : ctx_(ctx ? ctx : detail::ctx()) {
+    if (fnameLen < 0) fnameLen = dataFormat == dfGzip ? (int)(std::random_device()() % 26) : 0;
+    detail::check(zb200_compress_stream_begin_index(ctx_, level, dataFormat, fnameLen, indexSpan, &st_));
   }
   ~CompressStream() { zb200_compress_stream_free(st_); }
   CompressStream(const CompressStream &) = delete;
@@ -328,9 +335,11 @@ class CompressStream {
     out.resize(n);
     return out;
   }
+  Index index() const;  // after finish() on a stream begun with an index span
 
  private:
   zb200_compress_stream *st_ = nullptr;
+  zb200_ctx *ctx_ = nullptr;
 };
 
 // One member decoded from compressed input that arrives piece by piece (zb200_decompress_stream_*, no reference
@@ -459,9 +468,36 @@ class Index {
   }
 
  private:
+  friend class CompressStream;
+  friend std::pair<std::string, Index> compressWithIndex(const std::string &, int, CompressedDataFormat, uint64_t, int,
+                                                         zb200_ctx *);
   explicit Index(zb200_ctx *ctx) : ctx_(ctx ? ctx : detail::ctx()) {}
   zb200_ctx *ctx_ = nullptr;
   zb200_index *idx_ = nullptr;
 };
+
+inline Index CompressStream::index() const {
+  Index ix(ctx_);
+  detail::check(zb200_compress_stream_index(st_, &ix.idx_));
+  return ix;
+}
+
+// compress() that also returns the member's index, the one Index::build(member, dataFormat, span) gives, written
+// while compressing (zb200_compress_batch_index).  fnameLen < 0: a random gzip FNAME length, as compress() draws.
+inline std::pair<std::string, Index> compressWithIndex(const std::string &src, int level = DefaultCompression,
+                                                       CompressedDataFormat dataFormat = dfGzip, uint64_t span = 1u << 20,
+                                                       int fnameLen = -1, zb200_ctx *ctx = nullptr) {
+  Index ix(ctx);
+  if (fnameLen < 0) fnameLen = dataFormat == dfGzip ? (int)(std::random_device()() % 26) : 0;
+  const uint8_t fl = (uint8_t)fnameLen;
+  const uint64_t offs[2] = {0, src.size()};
+  uint64_t doffs[2] = {0, 0};
+  int st = 0;
+  std::string out(zb200_compress_bound(src.size(), dataFormat) + 64, '\0');
+  detail::check(zb200_compress_batch_index(ix.ctx_, detail::u8(src), offs, 1, level, dataFormat, &fl,
+                                           reinterpret_cast<uint8_t *>(&out[0]), out.size(), doffs, &st, span, &ix.idx_));
+  out.resize(doffs[1]);
+  return {std::move(out), std::move(ix)};
+}
 
 }  // namespace zippy

@@ -523,3 +523,42 @@ proc close*(ix: var Index) =
   if ix.idx != nil:
     zb200_index_free(ix.idx)
     ix.idx = nil
+
+# ---- an index written while compressing (zb200_compress_batch_index, zb200_compress_stream_begin_index): the
+# index buildIndex(member, dataFormat, span) gives, without a decode pass ----
+proc zb200_compress_batch_index(ctx: Zb200Ctx, srcBase: pointer, srcOffsets: ptr uint64, n: csize_t,
+                                level, dataFormat: cint, fnameLens: pointer, dstBase: pointer, dstCap: csize_t,
+                                dstOffsets: ptr uint64, statuses: ptr cint, span: uint64,
+                                indexes: ptr Zb200Index): cint {.importc, cdecl, dynlib: lib.}
+proc zb200_compress_stream_begin_index(ctx: Zb200Ctx, level, dataFormat, fnameLen: cint, span: uint64,
+                                       st: ptr Zb200CompressStream): cint {.importc, cdecl, dynlib: lib.}
+proc zb200_compress_stream_index(st: Zb200CompressStream, res: ptr Zb200Index): cint {.importc, cdecl, dynlib: lib.}
+
+proc randomFnameLen(dataFormat: CompressedDataFormat): int {.raises: [ZippyError].} =
+  if dataFormat != dfGzip: return 0
+  var urand: array[1, uint8]
+  if not urandom(urand):
+    raise newException(ZippyError, "Failed to generate random number")
+  (urand[0] mod 26).int
+
+proc compressWithIndex*(src: string, level = DefaultCompression, dataFormat = dfGzip,
+                        span = 1'u64 shl 20): (string, Index) {.raises: [ZippyError].} =
+  ## compress that also returns the member's index
+  let fl = [randomFnameLen(dataFormat).uint8]
+  var offs = [0'u64, src.len.uint64]
+  var dofs: array[2, uint64]
+  var st: cint
+  var dst = newString(zb200_compress_bound(src.len.csize_t, dataFormat.cint).int + 64)
+  check zb200_compress_batch_index(getCtx(), src.cstring, offs[0].addr, 1, level.cint, dataFormat.cint, fl[0].unsafeAddr,
+                                   dst[0].addr, dst.len.csize_t, dofs[0].addr, st.addr, span, result[1].idx.addr)
+  dst.setLen(dofs[1].int)
+  result[0] = dst
+
+proc newCompressStream*(level: int, dataFormat: CompressedDataFormat, fnameLen: int,
+                        span: uint64): CompressStream {.raises: [ZippyError].} =
+  ## a stream that also writes the member's index: index() after finish
+  let k = if fnameLen < 0: randomFnameLen(dataFormat) else: fnameLen
+  check zb200_compress_stream_begin_index(getCtx(), level.cint, dataFormat.cint, k.cint, span, result.st.addr)
+
+proc index*(s: CompressStream): Index {.raises: [ZippyError].} =
+  check zb200_compress_stream_index(s.st, result.idx.addr)

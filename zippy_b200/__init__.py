@@ -30,6 +30,7 @@ SyncFlush, FullFlush = 2, 3                                            # zlib's 
 
 __all__ = ["compress", "uncompress", "crc32", "adler32", "deflate", "inflate", "compress_batch", "uncompress_batch",
            "uncompressed_sizes", "checksum_batch", "ZippyError", "Context", "CompressStream", "DecompressStream",
+           "compress_with_index", "compress_batch_with_index",
            "MultiGpu", "Index", "dfDetect",
            "dfZlib", "dfGzip",
            "dfDeflate", "NoCompression", "BestSpeed", "BestCompression", "DefaultCompression", "HuffmanOnly",
@@ -107,9 +108,11 @@ class Context:
 
     # ---- batches over host buffers -------------------------------------------------
     def compress_batch(self, base, offsets, level=DefaultCompression, dataFormat=dfGzip, fname_lens=None,
-                       dictionary=None):
+                       dictionary=None, index_span=None):
         """-> (out uint8 array, out_offsets uint64[n+1]).  fname_lens: per-input gzip FNAME letters (0..25).
-        dictionary: a preset dictionary shared by every input (zlib / raw only; zb200_compress_batch_dict)."""
+        dictionary: a preset dictionary shared by every input (zlib / raw only; zb200_compress_batch_dict).
+        index_span: also write each member's Index with this span (zb200_compress_batch_index; no dictionary):
+        -> (out, out_offsets, list of Index)."""
         L = _native.lib()
         base = _as_u8(base)
         offsets = np.ascontiguousarray(offsets, dtype=np.uint64)
@@ -120,6 +123,16 @@ class Context:
         out_offs = np.zeros(n + 1, dtype=np.uint64)
         st = np.zeros(max(n, 1), dtype=np.int32)
         d = _dict(dictionary)
+        if index_span is not None:
+            if d is not None:
+                raise ZippyError(22, "a compress-time index is not written with a dictionary")
+            fl = np.ascontiguousarray(fname_lens, dtype=np.uint8) if fname_lens is not None else None
+            hs = (ctypes.c_void_p * max(n, 1))()
+            _check(self._h, L.zb200_compress_batch_index(self._h, base.ctypes.data, offsets.ctypes.data, n, level,
+                                                          dataFormat, fl.ctypes.data if fl is not None else None,
+                                                          out.ctypes.data, out.size, out_offs.ctypes.data,
+                                                          st.ctypes.data, index_span, hs))
+            return out[:int(out_offs[n])], out_offs, [Index(h, self) for h in hs[:n]]
         if d is not None:
             _check(self._h, L.zb200_compress_batch_dict(self._h, base.ctypes.data, offsets.ctypes.data, n, level,
                                                          dataFormat, d.ctypes.data, d.size, out.ctypes.data, out.size,
@@ -249,12 +262,22 @@ class Context:
         return out[:n]
 
     # ---- device-resident batches (raw device pointers; e.g. torch tensor .data_ptr()) ----
-    def compress_batch_device(self, d_src, offsets, level, dataFormat, d_dst, dst_cap, fname_lens=None):
+    def compress_batch_device(self, d_src, offsets, level, dataFormat, d_dst, dst_cap, fname_lens=None,
+                              index_span=None):
+        """-> out_offsets; with index_span also each member's Index (zb200_compress_batch_device_index):
+        -> (out_offsets, list of Index)."""
         L = _native.lib()
         offsets = np.ascontiguousarray(offsets, dtype=np.uint64)
         n = len(offsets) - 1
         out_offs = np.zeros(n + 1, dtype=np.uint64)
         fl = np.ascontiguousarray(fname_lens, dtype=np.uint8) if fname_lens is not None else None
+        if index_span is not None:
+            hs = (ctypes.c_void_p * max(n, 1))()
+            _check(self._h, L.zb200_compress_batch_device_index(self._h, d_src, offsets.ctypes.data, n, level,
+                                                                 dataFormat, fl.ctypes.data if fl is not None else None,
+                                                                 d_dst, dst_cap, out_offs.ctypes.data, None,
+                                                                 index_span, hs))
+            return out_offs, [Index(h, self) for h in hs[:n]]
         _check(self._h, L.zb200_compress_batch_device(self._h, d_src, offsets.ctypes.data, n, level, dataFormat,
                                                        fl.ctypes.data if fl is not None else None, d_dst, dst_cap,
                                                        out_offs.ctypes.data, None))
@@ -365,10 +388,21 @@ class CompressStream:
     gathered until a batch is pending, so most small writes return b"".  With gzip and fname_len=None the FNAME
     length is drawn at random, as compress() does (zippy.nim:28-42)."""
 
-    def __init__(self, level=DefaultCompression, dataFormat=dfGzip, fname_len=None, ctx=None, dictionary=None):
+    def __init__(self, level=DefaultCompression, dataFormat=dfGzip, fname_len=None, ctx=None, dictionary=None,
+                 index_span=None):
+        """index_span: also write the member's Index with this span (zb200_compress_stream_begin_index; no
+        dictionary), returned by index() after finish()."""
         self._ctx = ctx if ctx is not None else default_context()
         self._h = ctypes.c_void_p()
         d = _dict(dictionary)
+        if index_span is not None:
+            if d is not None:
+                raise ZippyError(22, "a compress-time index is not written with a dictionary")
+            if fname_len is None:
+                fname_len = os.urandom(1)[0] % 26 if dataFormat == dfGzip else 0
+            _check(self._ctx._h, _native.lib().zb200_compress_stream_begin_index(
+                self._ctx._h, level, dataFormat, fname_len, index_span, ctypes.byref(self._h)))
+            return
         if d is not None:   # zb200_compress_stream_begin_dict: zlib / raw only, no FNAME
             _check(self._ctx._h, _native.lib().zb200_compress_stream_begin_dict(self._ctx._h, level, dataFormat,
                                                                                 d.ctypes.data, d.size,
@@ -406,6 +440,14 @@ class CompressStream:
         _check(self._ctx._h, _native.lib().zb200_compress_stream_finish(self._h, out.ctypes.data, out.size,
                                                                         ctypes.byref(m)))
         return out[:m.value].tobytes()
+
+    def index(self):
+        """The member's Index, after finish() on a stream begun with index_span."""
+        if not self._h:
+            raise ZippyError(22, "the stream is closed")
+        h = ctypes.c_void_p()
+        _check(self._ctx._h, _native.lib().zb200_compress_stream_index(self._h, ctypes.byref(h)))
+        return Index(h, self._ctx)
 
     def close(self):
         if self._h:
@@ -684,6 +726,21 @@ def compress(src, level=DefaultCompression, dataFormat=dfGzip, dictionary=None):
     base, offs = _pack([src])
     out, _ = default_context().compress_batch(base, offs, level, dataFormat, fl, dictionary=dictionary)
     return out.tobytes()
+
+
+def compress_with_index(src, level=DefaultCompression, dataFormat=dfGzip, span=1 << 20):
+    """compress() that also returns the member's Index (the one Index.build(member, dataFormat, span) gives),
+    written while compressing: -> (bytes, Index)."""
+    return compress_batch_with_index([src], level, dataFormat, span=span)[0]
+
+
+def compress_batch_with_index(items, level=DefaultCompression, dataFormat=dfGzip, fname_lens=None, span=1 << 20):
+    """compress_batch() that also returns each member's Index: -> list of (bytes, Index)."""
+    if fname_lens is None and dataFormat == dfGzip:
+        fname_lens = [b % 26 for b in os.urandom(len(items))]                # zippy.nim:28-42
+    base, offs = _pack(items)
+    out, oo, idx = default_context().compress_batch(base, offs, level, dataFormat, fname_lens, index_span=span)
+    return [(out[int(oo[i]):int(oo[i + 1])].tobytes(), idx[i]) for i in range(len(items))]
 
 
 def uncompress(src, dataFormat=dfDetect, dictionary=None):

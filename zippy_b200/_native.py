@@ -89,6 +89,13 @@ SYMBOLS = {
     "zb200_index_free": (None, [ctypes.c_void_p]),
     "zb200_index_export": (c_int, [ctypes.c_void_p, ctypes.c_void_p, c_u8p, c_size_t, ctypes.POINTER(c_size_t)]),
     "zb200_index_import": (c_int, [ctypes.c_void_p, c_u8p, c_size_t, ctypes.POINTER(ctypes.c_void_p)]),
+    "zb200_compress_batch_index": (c_int, [ctypes.c_void_p, c_u8p, c_u64p, c_size_t, c_int, c_int, c_u8p, c_u8p,
+                                           c_size_t, c_u64p, c_intp, ctypes.c_uint64, ctypes.c_void_p]),
+    "zb200_compress_batch_device_index": (c_int, [ctypes.c_void_p, c_u8p, c_u64p, c_size_t, c_int, c_int, c_u8p, c_u8p,
+                                                  c_size_t, c_u64p, c_intp, ctypes.c_uint64, ctypes.c_void_p]),
+    "zb200_compress_stream_begin_index": (c_int, [ctypes.c_void_p, c_int, c_int, c_int, ctypes.c_uint64,
+                                                  ctypes.POINTER(ctypes.c_void_p)]),
+    "zb200_compress_stream_index": (c_int, [ctypes.c_void_p, ctypes.POINTER(ctypes.c_void_p)]),
     "zb200_mgpu_init": (c_int, [ctypes.c_void_p, c_int, ctypes.POINTER(ctypes.c_void_p)]),
     "zb200_mgpu_shutdown": (None, [ctypes.c_void_p]),
     "zb200_mgpu_device_count": (c_int, [ctypes.c_void_p]),

@@ -191,6 +191,7 @@ struct zb200_ctx {
   bool joint_markers = true;       // env ZB200_JOINT_MARKERS=0 turns the marker segments at sync joints off (A/B timing)
   uint32_t mark_window_segs = 8192;  // segments per window of the joint marker decode (env ZB200_MARK_WINDOW_SEGS)
   DevBuf idx_desc, idx_out;          // index build / extraction: gather descriptors, gathered bytes
+  DevBuf cix_rec, cix_crc, cix_first, cix_out;  // a compress-time index: ZbIndexWork's arrays
   uint64_t index_group_bytes = kDstreamMaxOut;  // output budget of one extraction launch group (env ZB200_INDEX_GROUP_BYTES)
   bool index_log = false;            // env ZB200_INDEX_LOG: one stderr line per extraction launch group
   // the preset dictionary of the *_dict call in progress (DictScope): its window W on the device, once as is
@@ -213,6 +214,21 @@ struct zb200_ctx {
   std::mutex mu;
 };
 
+// Segment points: for k = 0, 1, ..., the first block start whose output offset is >= k * 32768 (duplicates removed).
+// Window points: for j = 0, 1, ..., the first segment point whose output offset is >= j * span; each keeps the 32 KiB
+// of output in front of it.  Every segment point keeps the CRC-32 of its interval (up to the next point, the last one
+// to the end of the member).  All of it is host memory, tied to no ctx.
+struct zb200_index {
+  int fmt = 0;
+  uint64_t payload = 0, len = 0, size = 0, span = 0;
+  uint8_t head[32] = {}, tail[32] = {};
+  std::vector<uint64_t> bit, out;   // per point: absolute bit position in the member, output offset
+  std::vector<uint32_t> crc;        // per point: CRC-32 of its interval
+  std::vector<uint8_t> win;         // per point: 1 = window point
+  std::vector<uint64_t> win_at;     // per point: offset of its window in `windows` (window points with out > 0)
+  std::vector<uint8_t> windows;
+};
+
 // One member compressed from input that arrives piece by piece.  All of its state is on the host; the
 // kernels run on its ctx's scratch, so any number of streams and other calls can share a ctx.
 struct zb200_compress_stream {
@@ -228,6 +244,14 @@ struct zb200_compress_stream {
   uint32_t dict_id = 0;
   bool head_done = false, finished = false;
   int err = ZB200_OK;          // a CUDA failure: the stream is unusable
+  // begun with an index (zb200_compress_stream_begin_index): the points so far, written launch by launch
+  std::unique_ptr<zb200_index> ix;
+  uint64_t ix_next = 0;        // the next window point is the first point at or past this output offset
+  uint64_t ix_lo = 0;          // the first output offset the next launch's first block start may own
+  uint32_t ix_raw = 0;         // ix_open: the raw CRC-32 of the last point's interval so far
+  bool ix_open = false;
+  std::vector<uint8_t> ix_in;  // the last <= 32 KiB of input compressed (windows need input, not history)
+  std::vector<uint8_t> ix_tail;  // the last <= 32 bytes of the member written
 };
 
 // One member decoded from compressed input that arrives piece by piece.  All of its state is on the host; the
@@ -507,10 +531,11 @@ struct DictScope {
 // on three streams; each group's output offset is chained on the device (out_base_ptr), so
 // the only host waits are for the small per-group offset arrays that size the D2H copies.
 // sp (host buffers, n == 1 only): the member is one part of a stream; null for every batch call.
+// ix: null, or the records of a compress-time index (k_index_rec after k_scan; ix->rec_first counts the batch's members).
 int compress_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint8_t *h_src, const uint64_t *src_offsets,
                     size_t n, int level, int data_format, const uint8_t *fname_lens, uint8_t *d_dst,
                     size_t dst_cap, uint8_t *h_dst, size_t h_dst_cap, uint64_t *dst_offsets, int *statuses,
-                    size_t max_group_chunks, StreamPart *sp = nullptr) {
+                    size_t max_group_chunks, StreamPart *sp = nullptr, const ZbIndexWork *ix = nullptr) {
   const auto t_entry = std::chrono::steady_clock::now();
   if (level < -2 || level > 9) return ZB200_ERR_INVALID_LEVEL;
   if (data_format != ZB200_DF_GZIP && data_format != ZB200_DF_ZLIB && data_format != ZB200_DF_DEFLATE)
@@ -723,7 +748,7 @@ int compress_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint8_t *h_src, 
       ctx->timing.plan_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t_entry).count();
       CK(cudaEventRecord(ctx->ev[0], s));
     }
-    CK(zb_launch_lz(w, s));
+    CK(zb_launch_lz(w, s, ix != nullptr));
     if (timed) CK(cudaEventRecord(ctx->ev[1], s));
     CK(zb_launch_huff(w, s));
     if (timed) CK(cudaEventRecord(ctx->ev[2], s));
@@ -736,6 +761,12 @@ int compress_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint8_t *h_src, 
                        cudaMemcpyDeviceToHost, s));
     if (sp) CK(cudaMemcpyAsync(pin_carry, w.carry_out, sizeof(ZbMemberCarry), cudaMemcpyDeviceToHost, s));
     CK(cudaEventRecord(ctx->gev[3 * gi + 2], s));
+    if (ix) {
+      ZbIndexWork x = *ix;
+      x.rec_first += g.m0;
+      CK(zb_launch_index_rec(w, x, s));
+      ctx->timing.kernel_launches += 1;
+    }
     if (timed) CK(cudaEventRecord(ctx->ev[4], s));
     CK(zb_launch_pack(w, s));
     if (timed) CK(cudaEventRecord(ctx->ev[5], s));
@@ -772,6 +803,131 @@ int compress_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint8_t *h_src, 
   return ZB200_OK;
 }
 
+// ---- compress-time index ----
+// The rule that turns access-point records into an index's points, shared by zb200_index_build and the compress
+// calls that write an index: (b, o) is the point recorded for the next multiple k * 32768, k increasing.  A record
+// that repeats the last point adds nothing.  A new point is a window point when it is the first at or past
+// next_win (the next multiple of the span); one with o > 0 gets 32 KiB of idx->windows (win_at) that the caller
+// fills with the output in front of it.  Returns 1 for a new point, 0 for a repeat, -1 for records out of order.
+int index_add_point(zb200_index *idx, uint64_t b, uint64_t o, uint64_t &next_win) {
+  if (!idx->bit.empty() && idx->bit.back() == b) return 0;
+  if (!idx->bit.empty() && (b < idx->bit.back() || o <= idx->out.back())) return -1;
+  idx->bit.push_back(b);
+  idx->out.push_back(o);
+  const bool win = o >= next_win;
+  idx->win.push_back(win ? 1 : 0);
+  idx->win_at.push_back(~0ull);
+  if (win) {
+    next_win = (o / idx->span + 1) * idx->span;
+    if (o > 0) {
+      idx->win_at.back() = idx->windows.size();
+      idx->windows.resize(idx->windows.size() + 32768);
+    }
+  }
+  return 1;
+}
+
+// the header bytes in front of a member's first block
+uint64_t frame_head(int data_format, uint8_t fname_len) {
+  return data_format == ZB200_DF_GZIP ? 11u + fname_len : data_format == ZB200_DF_ZLIB ? 2u : 0u;
+}
+
+// ZbIndexWork's device arrays for nrec records of the members whose first records are rec_first: the records
+// prefilled with ~0, the launch words zeroed (k0, lo0 and byte_base are the caller's)
+int index_rec_prepare(zb200_ctx *ctx, const std::vector<uint64_t> &rec_first, size_t nrec, ZbIndexWork &x) {
+  ENSURE(ctx->cix_rec, nrec * 16 + 16);
+  ENSURE(ctx->cix_crc, nrec * 4 + 4);
+  ENSURE(ctx->cix_first, rec_first.size() * 8 + 8);
+  ENSURE(ctx->cix_out, 16);
+  CK(cudaMemcpyAsync(ctx->cix_first.p, rec_first.data(), rec_first.size() * 8, cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemsetAsync(ctx->cix_rec.p, 0xff, nrec * 16, ctx->stream));
+  CK(cudaMemsetAsync(ctx->cix_out.p, 0, 16, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));   // rec_first is pageable host memory
+  memset(&x, 0, sizeof(x));
+  x.rec = (uint64_t *)ctx->cix_rec.p;
+  x.crc = (uint32_t *)ctx->cix_crc.p;
+  x.rec_first = (const uint64_t *)ctx->cix_first.p;
+  x.launch_out = (uint64_t *)ctx->cix_out.p;
+  return ZB200_OK;
+}
+
+int index_rec_fetch(zb200_ctx *ctx, size_t nrec, std::vector<uint64_t> &rec, std::vector<uint32_t> &crc, uint64_t *launch_out) {
+  rec.resize(nrec * 2);
+  crc.resize(nrec);
+  CK(cudaMemcpyAsync(rec.data(), ctx->cix_rec.p, nrec * 16, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaMemcpyAsync(crc.data(), ctx->cix_crc.p, nrec * 4, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaMemcpyAsync(launch_out, ctx->cix_out.p, 16, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  return ZB200_OK;
+}
+
+// A stream launch that wrote the member's input [start, start + nbytes) (`in`) and dst_len bytes at dst, with
+// nrec records from multiple k0 on: its points join the stream's index.  The interval of the last point stays open
+// (a raw CRC) until a later launch records the next point or ends the member.
+int stream_index_launch(zb200_compress_stream *st, const uint8_t *in, size_t nbytes, bool last, const uint8_t *dst,
+                        size_t dst_len, size_t nrec) {
+  zb200_ctx *ctx = st->ctx;
+  std::vector<uint64_t> rec;
+  std::vector<uint32_t> crc;
+  uint64_t lout[2];
+  int rc = index_rec_fetch(ctx, nrec, rec, crc, lout);
+  if (rc) return rc;
+  zb200_index *idx = st->ix.get();
+  const uint64_t start = st->carry.bytes, end = start + nbytes;
+  bool none = true;
+  for (size_t r = 0; r < nrec; r++) {
+    const uint64_t b = rec[2 * r], o = rec[2 * r + 1];
+    if (b == ~0ull) continue;
+    const size_t before = idx->bit.size();
+    const int a = index_add_point(idx, b, o, st->ix_next);
+    if (a < 0) {
+      ctx->last_err = "compress-time index: records out of order";
+      return ZB200_ERR_CUDA;
+    }
+    if (!a) continue;
+    if (none) {  // the open interval ends here
+      none = false;
+      st->ix_raw = zb_gf2_mul(st->ix_raw, zb_xpow8(o - start)) ^ (uint32_t)lout[1];
+      if (st->ix_open) idx->crc.back() = zb_crc32_finalize(st->ix_raw, o - idx->out[before - 1]);
+    }
+    idx->crc.push_back(crc[r]);
+    if (idx->win_at.back() != ~0ull) {   // the 32 KiB of input in front of the point: held input, then this launch's
+      uint8_t *w = idx->windows.data() + idx->win_at.back();
+      const uint64_t lo = o - 32768ull;
+      const size_t held = lo < start ? (size_t)(start - lo) : 0;
+      if (held) memcpy(w, st->ix_in.data() + st->ix_in.size() - held, held);
+      memcpy(w + held, in + (lo + held - start), 32768 - held);
+    }
+  }
+  if (none) {
+    st->ix_raw = zb_gf2_mul(st->ix_raw, zb_xpow8(nbytes)) ^ (uint32_t)lout[1];
+  } else {
+    st->ix_open = !last;
+    if (!last) st->ix_raw = idx->crc.back();
+  }
+  if (last && st->ix_open) {
+    idx->crc.back() = zb_crc32_finalize(st->ix_raw, end - idx->out.back());
+    st->ix_open = false;
+  }
+  st->ix_lo = lout[0] + 1;
+  if (nbytes >= 32768) {
+    st->ix_in.assign(in + nbytes - 32768, in + nbytes);
+  } else {
+    st->ix_in.insert(st->ix_in.end(), in, in + nbytes);
+    if (st->ix_in.size() > 32768) st->ix_in.erase(st->ix_in.begin(), st->ix_in.end() - 32768);
+  }
+  for (size_t i = 0; i < dst_len && idx->len + i < 32; i++) idx->head[idx->len + i] = dst[i];
+  st->ix_tail.insert(st->ix_tail.end(), dst + (dst_len > 32 ? dst_len - 32 : 0), dst + dst_len);
+  if (st->ix_tail.size() > 32) st->ix_tail.erase(st->ix_tail.begin(), st->ix_tail.end() - 32);
+  idx->len += dst_len;
+  if (last) {
+    idx->size = end;
+    memset(idx->tail, 0, 32);
+    memcpy(idx->tail, st->ix_tail.data(), st->ix_tail.size());
+  }
+  return ZB200_OK;
+}
+
 // Compress the stream's next `nbytes` pending bytes into dst; ctx locked.  They are whole chunks, unless the run
 // ends the member (`last`) or a flush segment (a flush: every pending byte, last = false).  On success the carry
 // advances and the compressed input leaves the buffer: its last 32 KiB stay as history, none after a full flush
@@ -792,11 +948,26 @@ int stream_run(zb200_compress_stream *st, size_t nbytes, bool last, uint8_t *dst
   sp.carry_in = st->carry;
   sp.has_dict = st->has_dict;
   sp.dict_id = st->dict_id;
+  ZbIndexWork x;
+  size_t nrec = 0;
+  if (st->ix) {   // the multiples this launch's block starts can own: from the first one past the last block start on
+    const uint64_t k0 = (st->ix_lo + 32767ull) >> 15, kend = (st->carry.bytes + nbytes) >> 15;
+    nrec = kend >= k0 ? (size_t)(kend - k0 + 1) : 0;
+    int rc = index_rec_prepare(ctx, std::vector<uint64_t>(1, 0), nrec, x);
+    if (rc) return rc;
+    x.k0 = k0;
+    x.lo0 = st->ix_lo;
+    x.byte_base = st->ix->len;
+  }
   int rc = compress_locked(ctx, (const uint8_t *)ctx->in_stage.p, st->buf.data(), offs, 1, st->level, st->data_format,
                            &st->fname_len, (uint8_t *)ctx->out_stage.p, ctx->out_stage.cap & ~(size_t)3, dst, dst_cap,
-                           dst_offs, nullptr, ctx->host_group_chunks, &sp);
+                           dst_offs, nullptr, ctx->host_group_chunks, &sp, st->ix ? &x : nullptr);
   if (rc) return rc;
   *dst_len = (size_t)dst_offs[1];
+  if (st->ix) {
+    rc = stream_index_launch(st, st->buf.data() + st->hist, nbytes, last, dst, *dst_len, nrec);
+    if (rc) return rc;
+  }
   st->carry = sp.carry_out;
   st->head_done = true;
   const bool lz = st->level == -1 || st->level >= 2;
@@ -2488,7 +2659,7 @@ void zb200_shutdown(zb200_ctx *ctx) {
   DevBuf *bufs[] = {&ctx->desc, &ctx->member_first, &ctx->fname, &ctx->masks, &ctx->recs, &ctx->hist, &ctx->chk,
                     &ctx->cb, &ctx->chunk_off, &ctx->member_off, &ctx->member_check, &ctx->member_isize,
                     &ctx->src_off, &ctx->dst_off, &ctx->out_len, &ctx->status, &ctx->expect, &ctx->kind,
-                    &ctx->counter, &ctx->ck_out, &ctx->ck_pieces, &ctx->ck_first, &ctx->ck_piece_out, &ctx->ck_partials, &ctx->in_stage, &ctx->out_stage, &ctx->lz2_tables, &ctx->carry,
+                    &ctx->counter, &ctx->cix_rec, &ctx->cix_crc, &ctx->cix_first, &ctx->cix_out, &ctx->ck_out, &ctx->ck_pieces, &ctx->ck_first, &ctx->ck_piece_out, &ctx->ck_partials, &ctx->in_stage, &ctx->out_stage, &ctx->lz2_tables, &ctx->carry,
                     &ctx->seg_src, &ctx->seg_dst, &ctx->seg_len, &ctx->seg_status, &ctx->seg_kind, &ctx->seg_expect, &ctx->seg_cand, &ctx->skip_mask, &ctx->order, &ctx->mark_scratch, &ctx->mark_segs, &ctx->seg_bits, &ctx->mark_win, &ctx->gate,
                     &ctx->idx_desc, &ctx->idx_out, &ctx->dict_win, &ctx->dict_win16};
   for (DevBuf *b : bufs)
@@ -3433,21 +3604,6 @@ int zb200_adler32(zb200_ctx *ctx, const void *src, size_t len, uint32_t *out) {
 }  // extern "C"
 
 // ---- random access (zb200_index_*) ----
-// Segment points: for k = 0, 1, ..., the first block start whose output offset is >= k * 32768 (duplicates removed).
-// Window points: for j = 0, 1, ..., the first segment point whose output offset is >= j * span; each keeps the 32 KiB
-// of output in front of it.  Every segment point keeps the CRC-32 of its interval (up to the next point, the last one
-// to the end of the member).  All of it is host memory, tied to no ctx.
-struct zb200_index {
-  int fmt = 0;
-  uint64_t payload = 0, len = 0, size = 0, span = 0;
-  uint8_t head[32] = {}, tail[32] = {};
-  std::vector<uint64_t> bit, out;   // per point: absolute bit position in the member, output offset
-  std::vector<uint32_t> crc;        // per point: CRC-32 of its interval
-  std::vector<uint8_t> win;         // per point: 1 = window point
-  std::vector<uint64_t> win_at;     // per point: offset of its window in `windows` (window points with out > 0)
-  std::vector<uint8_t> windows;
-};
-
 namespace {
 
 void index_edges(const uint8_t *src, uint64_t len, uint8_t *head, uint8_t *tail) {
@@ -3596,6 +3752,8 @@ int index_build_locked(zb200_ctx *ctx, const uint8_t *src, size_t len, int data_
   CK(cudaMemcpyAsync(rec.data(), d_rec, (size_t)nrec * 16, cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
   std::unique_ptr<zb200_index> idx(new zb200_index());
+  idx->span = span;
+  uint64_t next = 0;
   for (uint32_t k = 0; k < nrec; k++) {
     uint64_t b = rec[2 * k], o = rec[2 * k + 1];
     if (b == ~0ull) {   // no block start of its segment reaches the multiple: the next segment's start
@@ -3605,36 +3763,24 @@ int index_build_locked(zb200_ctx *ctx, const uint8_t *src, size_t len, int data_
       b = bits[j];
       o = base[j];
     }
-    if (!idx->bit.empty() && idx->bit.back() == b) continue;
-    if (!idx->bit.empty() && (b < idx->bit.back() || o <= idx->out.back())) return ZB200_ERR_UNCOMPRESS;
-    idx->bit.push_back(b);
-    idx->out.push_back(o);
+    if (index_add_point(idx.get(), b, o, next) < 0) return ZB200_ERR_UNCOMPRESS;
   }
   const size_t np = idx->bit.size();
   if (np == 0 || idx->out[0] != 0) return ZB200_ERR_UNCOMPRESS;
-  // 2. window flags, windows and interval CRCs, from the decoded output in out_stage
-  idx->win.assign(np, 0);
-  idx->win_at.assign(np, ~0ull);
+  // 2. windows and interval CRCs, from the decoded output in out_stage
   std::vector<uint64_t> ranges;
-  uint64_t next = 0, wbytes = 0;
-  for (size_t p = 0; p < np; p++) {
-    if (idx->out[p] < next) continue;
-    idx->win[p] = 1;
-    next = (idx->out[p] / span + 1) * span;
-    if (idx->out[p] > 0) {
-      idx->win_at[p] = wbytes;
+  for (size_t p = 0; p < np; p++)
+    if (idx->win_at[p] != ~0ull) {
       ranges.push_back(idx->out[p] - 32768ull);
-      ranges.push_back(wbytes);
+      ranges.push_back(idx->win_at[p]);
       ranges.push_back(32768ull);
-      wbytes += 32768ull;
     }
-  }
+  const uint64_t wbytes = idx->windows.size();
   idx->crc.assign(np, 0);
   std::vector<uint64_t> offs(idx->out);
   offs.push_back(size);
   rc = checksum_device_locked(ctx, (const uint8_t *)ctx->out_stage.p, offs.data(), np, 0, idx->crc.data());
   if (rc) return rc;
-  idx->windows.resize(wbytes);
   if (wbytes) {
     ENSURE(ctx->idx_out, wbytes);
     rc = index_gather(ctx, (const uint8_t *)ctx->out_stage.p, ranges, false, ctx->idx_out.p);
@@ -3647,7 +3793,6 @@ int index_build_locked(zb200_ctx *ctx, const uint8_t *src, size_t len, int data_
   idx->payload = payload;
   idx->len = len;
   idx->size = size;
-  idx->span = span;
   index_edges(src, len, idx->head, idx->tail);
   *out = idx.release();
   return ZB200_OK;
@@ -3916,9 +4061,186 @@ int index_extract_locked(zb200_ctx *ctx, const zb200_index *idx, const uint8_t *
   return ZB200_OK;
 }
 
+// zb200_compress_batch_index (h_src / h_dst: d_src is in_stage, rebased to src_offsets[0]) and
+// zb200_compress_batch_device_index (device buffers): the call without an index, with k_index_rec's records, then
+// one index per member.  Windows are copied from the input, head and tail from the output.
+int compress_index_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint8_t *h_src, const uint64_t *src_offsets,
+                          size_t n, int level, int data_format, const uint8_t *fname_lens, uint8_t *d_dst,
+                          size_t dst_cap, uint8_t *h_dst, size_t h_dst_cap, uint64_t *dst_offsets, int *statuses,
+                          size_t max_group_chunks, uint64_t span, zb200_index **indexes) {
+  std::vector<uint64_t> rec_first(n + 1, 0);
+  for (size_t i = 0; i < n; i++) {
+    if (src_offsets[i + 1] < src_offsets[i]) return ZB200_ERR_ARG;
+    rec_first[i + 1] = rec_first[i] + (src_offsets[i + 1] - src_offsets[i]) / 32768ull + 1ull;
+  }
+  const size_t nrec = (size_t)rec_first[n];
+  ZbIndexWork x;
+  int rc = index_rec_prepare(ctx, rec_first, nrec, x);
+  if (rc) return rc;
+  rc = compress_locked(ctx, d_src, h_src, src_offsets, n, level, data_format, fname_lens, d_dst, dst_cap, h_dst,
+                       h_dst_cap, dst_offsets, statuses, max_group_chunks, nullptr, &x);
+  if (rc) return rc;
+  std::vector<uint64_t> rec;
+  std::vector<uint32_t> crc;
+  uint64_t lout[2];
+  rc = index_rec_fetch(ctx, nrec, rec, crc, lout);
+  if (rc) return rc;
+  std::vector<std::unique_ptr<zb200_index>> out(n);
+  std::vector<uint64_t> wranges, eranges;   // device buffers: (source offset, destination offset, length) to gather
+  std::vector<uint64_t> wfirst(n + 1, 0);
+  for (size_t m = 0; m < n; m++) {
+    std::unique_ptr<zb200_index> idx(new zb200_index());
+    idx->fmt = data_format;
+    idx->payload = frame_head(data_format, fname_lens && data_format == ZB200_DF_GZIP ? fname_lens[m] : 0);
+    idx->len = dst_offsets[m + 1] - dst_offsets[m];
+    idx->size = src_offsets[m + 1] - src_offsets[m];
+    idx->span = span;
+    // every window point but the first at output 0 takes 32 KiB: reserve them at once rather than grow the vector
+    idx->windows.reserve((size_t)std::min<uint64_t>(idx->size / span, rec_first[m + 1] - rec_first[m]) * 32768);
+    uint64_t next = 0;
+    for (uint64_t r = rec_first[m]; r < rec_first[m + 1]; r++) {
+      if (rec[2 * r] == ~0ull) continue;   // past the member's last block start
+      const int a = index_add_point(idx.get(), rec[2 * r], rec[2 * r + 1], next);
+      if (a < 0) {
+        ctx->last_err = "compress-time index: records out of order";
+        return ZB200_ERR_CUDA;
+      }
+      if (a) idx->crc.push_back(crc[r]);
+    }
+    for (size_t p = 0; p < idx->bit.size(); p++) {
+      if (idx->win_at[p] == ~0ull) continue;
+      const uint64_t from = src_offsets[m] + idx->out[p] - 32768ull;
+      if (h_src) {
+        memcpy(idx->windows.data() + idx->win_at[p], h_src + from, 32768);
+      } else {
+        wranges.push_back(from);
+        wranges.push_back(wfirst[m] + idx->win_at[p]);
+        wranges.push_back(32768ull);
+      }
+    }
+    wfirst[m + 1] = wfirst[m] + (h_src ? 0 : idx->windows.size());
+    if (h_dst) {
+      index_edges(h_dst + dst_offsets[m], idx->len, idx->head, idx->tail);
+    } else {
+      const uint64_t k = std::min<uint64_t>(idx->len, 32);
+      eranges.insert(eranges.end(), {dst_offsets[m], 64ull * m, k, dst_offsets[m] + idx->len - k, 64ull * m + 32, k});
+    }
+    out[m] = std::move(idx);
+  }
+  cudaStream_t s = ctx->stream;
+  if (wfirst[n]) {
+    ENSURE(ctx->idx_out, (size_t)wfirst[n]);
+    rc = index_gather(ctx, d_src, wranges, false, ctx->idx_out.p);
+    if (rc) return rc;
+    for (size_t m = 0; m < n; m++)   // straight into each index: the windows are most of its bytes
+      if (!out[m]->windows.empty())
+        CK(cudaMemcpyAsync(out[m]->windows.data(), (const uint8_t *)ctx->idx_out.p + wfirst[m], out[m]->windows.size(),
+                           cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+  }
+  if (!h_dst && n) {
+    ENSURE(ctx->idx_out, 64 * n);
+    CK(cudaMemsetAsync(ctx->idx_out.p, 0, 64 * n, s));
+    rc = index_gather(ctx, d_dst, eranges, false, ctx->idx_out.p);
+    if (rc) return rc;
+    std::vector<uint8_t> eb(64 * n);
+    CK(cudaMemcpyAsync(eb.data(), ctx->idx_out.p, eb.size(), cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    for (size_t m = 0; m < n; m++) {
+      memcpy(out[m]->head, eb.data() + 64 * m, 32);
+      memcpy(out[m]->tail, eb.data() + 64 * m + 32, 32);
+    }
+  }
+  for (size_t m = 0; m < n; m++) indexes[m] = out[m].release();
+  return ZB200_OK;
+}
+
+// a compress-time index's span: the build's rule
+bool index_span_ok(uint64_t span) { return span >= 32768 && span % 32768 == 0; }
+
 }  // namespace
 
 extern "C" {
+
+int zb200_compress_batch_index(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n, int level,
+                               int data_format, const uint8_t *fname_lens, uint8_t *dst_base, size_t dst_cap,
+                               uint64_t *dst_offsets, int *statuses, uint64_t span, zb200_index **indexes) {
+  return guarded(ctx, [&]() -> int {
+    if (!ctx || !src_offsets || !dst_offsets || !indexes || (n && (!src_base || !dst_base))) return ZB200_ERR_ARG;
+    for (size_t i = 0; i < n; i++) indexes[i] = nullptr;
+    if (level < -2 || level > 9) return ZB200_ERR_INVALID_LEVEL;
+    if (data_format != ZB200_DF_GZIP && data_format != ZB200_DF_ZLIB && data_format != ZB200_DF_DEFLATE)
+      return ZB200_ERR_INVALID_FORMAT;
+    if (!index_span_ok(span)) return ZB200_ERR_ARG;
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    DeviceGuard g(ctx->device);
+    memset(&ctx->timing, 0, sizeof(ctx->timing));
+    if (n == 0) {
+      dst_offsets[0] = 0;
+      return ZB200_OK;
+    }
+    for (size_t i = 0; i < n; i++)
+      if (src_offsets[i + 1] < src_offsets[i]) return ZB200_ERR_ARG;
+    const uint64_t in_bytes = src_offsets[n] - src_offsets[0];
+    uint64_t bound = 0;
+    for (size_t i = 0; i < n; i++)
+      bound += zb200_compress_bound((size_t)(src_offsets[i + 1] - src_offsets[i]), data_format) + 64;
+    ENSURE(ctx->in_stage, (size_t)in_bytes + 64);
+    ENSURE(ctx->out_stage, (size_t)bound + 64);
+    return compress_index_locked(ctx, (const uint8_t *)ctx->in_stage.p, src_base, src_offsets, n, level, data_format,
+                                 fname_lens, (uint8_t *)ctx->out_stage.p, ctx->out_stage.cap & ~(size_t)3, dst_base,
+                                 dst_cap, dst_offsets, statuses, ctx->host_group_chunks, span, indexes);
+  });
+}
+
+int zb200_compress_batch_device_index(zb200_ctx *ctx, const uint8_t *d_src, const uint64_t *src_offsets, size_t n,
+                                      int level, int data_format, const uint8_t *fname_lens, uint8_t *d_dst,
+                                      size_t dst_cap, uint64_t *dst_offsets, int *statuses, uint64_t span,
+                                      zb200_index **indexes) {
+  return guarded(ctx, [&]() -> int {
+    if (!ctx || !src_offsets || !dst_offsets || !indexes || (n && (!d_src || !d_dst))) return ZB200_ERR_ARG;
+    for (size_t i = 0; i < n; i++) indexes[i] = nullptr;
+    if (level < -2 || level > 9) return ZB200_ERR_INVALID_LEVEL;
+    if (data_format != ZB200_DF_GZIP && data_format != ZB200_DF_ZLIB && data_format != ZB200_DF_DEFLATE)
+      return ZB200_ERR_INVALID_FORMAT;
+    if (!index_span_ok(span)) return ZB200_ERR_ARG;
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    DeviceGuard g(ctx->device);
+    ctx->timing.kernel_launches = 0;
+    if (n == 0) {
+      dst_offsets[0] = 0;
+      return ZB200_OK;
+    }
+    return compress_index_locked(ctx, d_src, nullptr, src_offsets, n, level, data_format, fname_lens, d_dst, dst_cap,
+                                 nullptr, 0, dst_offsets, statuses, ctx->dev_group_chunks, span, indexes);
+  });
+}
+
+int zb200_compress_stream_begin_index(zb200_ctx *ctx, int level, int data_format, int fname_len, uint64_t span,
+                                      zb200_compress_stream **out) {
+  if (ctx && out && level >= -2 && level <= 9 &&
+      (data_format == ZB200_DF_GZIP || data_format == ZB200_DF_ZLIB || data_format == ZB200_DF_DEFLATE) &&
+      !index_span_ok(span)) {
+    *out = nullptr;
+    return ZB200_ERR_ARG;
+  }
+  const int rc = zb200_compress_stream_begin(ctx, level, data_format, fname_len, out);
+  if (rc) return rc;
+  zb200_compress_stream *st = *out;
+  st->ix.reset(new zb200_index());
+  st->ix->fmt = data_format;
+  st->ix->payload = frame_head(data_format, st->fname_len);
+  st->ix->span = span;
+  return ZB200_OK;
+}
+
+int zb200_compress_stream_index(zb200_compress_stream *st, zb200_index **out) {
+  if (!st || !out) return ZB200_ERR_ARG;
+  *out = nullptr;
+  if (!st->ix || !st->finished) return ZB200_ERR_ARG;
+  *out = new zb200_index(*st->ix);
+  return ZB200_OK;
+}
 
 int zb200_index_build(zb200_ctx *ctx, const uint8_t *src, size_t len, int data_format, uint64_t span, zb200_index **out) {
   return guarded(ctx, [&]() -> int {

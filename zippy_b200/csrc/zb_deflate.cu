@@ -1019,7 +1019,127 @@ __global__ void __launch_bounds__(128)
 }
 
 // ------------------------------------------------------------------------------------
-#define PK_ROW_WORDS 17   // a 32-byte window encodes to at most 32 x 15 bits = 15 words (+ partial)
+// k_index_rec: a compress-time index (ZbIndexWork), one thread per chunk.  A chunk's block starts follow from its
+// codebook: a coded block at the chunk's first byte, then (not final) the empty sync block after its end-of-block
+// code; or stored pieces of at most 65535 bytes, each 5 header bytes + its bytes.  Output offsets are input
+// offsets.  A chunk's output is one part, or two for a 65536-byte stored chunk (65535 + 1: its second piece is a
+// block start); the raw CRC-32 of a part is the chunk's (k_lz / k_lz2), or for the two parts derived from it and
+// the last byte: raw(A || b) = raw(A) * x^8 + raw(b).
+#define IX_XINV8 0x6567cb95u  // x^-8 mod P (reflected): raw(A) = (raw(A || b) + raw(b)) * x^-8
+
+struct IxChunk {
+  uint64_t o0, byte0;  // output offset of the chunk's first byte; member byte offset of its first block
+  uint32_t len, np;    // input bytes; parts (stored pieces, 1 for a coded block)
+  bool sync;           // a coded block that is not final: the sync block follows it
+};
+
+__device__ __forceinline__ bool ix_owns(uint64_t lo, uint64_t o) { return (o >> 15) << 15 >= lo; }  // k*32768 in [lo, o]
+
+__global__ void __launch_bounds__(128) k_index_rec(ZbCompressWork w, ZbIndexWork x) {
+  const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= w.n_chunks) return;
+  const uint32_t m = w.desc[c].member, c0 = w.member_first[m], c1 = w.member_first[m + 1];
+  const uint64_t obase = w.carry_in ? w.carry_in[m].bytes : 0ull, src0 = w.desc[c0].src_off;
+  const uint64_t mbyte = w.member_off[m];
+  auto chunk = [&](uint32_t cc) {
+    IxChunk k;
+    const ZbChunkDesc d = w.desc[cc];
+    const ZbCodebook *cb = &w.cb[cc];
+    k.o0 = obase + (d.src_off - src0);
+    k.byte0 = x.byte_base + w.chunk_off[cc] - mbyte;
+    k.len = d.len;
+    const bool stored = cb->block_type == 0u;
+    k.np = stored && d.len > 65535u ? 2u : 1u;
+    k.sync = !stored && !cb->is_final;
+    return k;
+  };
+  // block j of chunk cc: j < np a part's start, j == np the sync block
+  auto block = [&](uint32_t cc, const IxChunk &k, uint32_t j, uint64_t &bit) -> uint64_t {
+    if (j < k.np) {
+      bit = (k.byte0 + (uint64_t)j * 65540ull) * 8ull;
+      return k.o0 + (uint64_t)j * 65535ull;
+    }
+    const ZbCodebook *cb = &w.cb[cc];
+    bit = k.byte0 * 8ull + cb->eob_bit_start + (cb->ll[256] >> 16);
+    return k.o0 + k.len;
+  };
+  auto part_raw = [&](uint32_t cc, const IxChunk &k, uint32_t j, uint32_t &plen) -> uint32_t {
+    const uint32_t raw = w.chk[cc].crc_raw;
+    if (k.np == 1u) {
+      plen = k.len;
+      return raw;
+    }
+    const uint32_t rb = zb_crc_raw_byte(0u, w.src[w.desc[cc].src_off + 65535u]);
+    plen = j ? 1u : 65535u;
+    return j ? rb : zb_gf2_mul(raw ^ rb, IX_XINV8);
+  };
+  // raw CRC-32 and length of the output from block j of chunk cc up to the next point; closed: the interval ends
+  // at that point or at the member's end (false: at the end of a stream launch that does not end the member)
+  auto walk = [&](uint32_t cc, uint32_t j, uint64_t &n, bool &closed) -> uint32_t {
+    uint32_t raw = 0;
+    n = 0;
+    IxChunk k = chunk(cc);
+    uint64_t lo = 0, bit;
+    for (bool first = true;; first = false) {
+      const uint64_t o = block(cc, k, j, bit);
+      if (!first && ix_owns(lo, o)) {
+        closed = true;
+        return raw;
+      }
+      lo = o + 1ull;
+      if (j < k.np) {
+        uint32_t plen;
+        const uint32_t pr = part_raw(cc, k, j, plen);
+        raw = zb_gf2_mul(raw, plen == ZB_CHUNK_BYTES ? w.tabs->sub_mul[0] : zb_xpow8_t(w.tabs->pow2, plen)) ^ pr;
+        n += plen;
+      }
+      if (++j < k.np + (k.sync ? 1u : 0u)) continue;
+      if (++cc >= c1) {
+        closed = (w.desc[c1 - 1].flags & ZB_CHUNK_LAST) != 0u;
+        return raw;
+      }
+      k = chunk(cc);
+      j = 0;
+    }
+  };
+
+  const ZbChunkDesc d = w.desc[c];
+  const IxChunk k = chunk(c);
+  uint64_t lo;  // the first output offset this chunk's first block start may own
+  if (c == c0) {
+    lo = (d.flags & ZB_CHUNK_HEAD) ? 0ull : x.lo0;
+  } else {
+    const IxChunk p = chunk(c - 1);
+    lo = (p.sync ? k.o0 : p.o0 + (uint64_t)(p.np - 1u) * 65535ull) + 1ull;
+  }
+  const uint32_t nb = k.np + (k.sync ? 1u : 0u);
+  uint64_t o = 0;
+  for (uint32_t j = 0; j < nb; j++) {
+    uint64_t bit;
+    o = block(c, k, j, bit);
+    if (ix_owns(lo, o)) {
+      const uint64_t r0 = x.rec_first[m] - x.k0;
+      const uint64_t kmin = (lo + 32767ull) >> 15, kmax = o >> 15;
+      for (uint64_t kk = kmin; kk <= kmax; kk++) {
+        x.rec[2ull * (r0 + kk)] = bit;
+        x.rec[2ull * (r0 + kk) + 1ull] = o;
+      }
+      uint64_t n;
+      bool closed;
+      const uint32_t raw = walk(c, j, n, closed);
+      x.crc[r0 + kmin] = closed ? ~(zb_gf2_mul(zb_xpow8_t(w.tabs->pow2, n), 0xffffffffu) ^ raw) : raw;
+    } else if (c == c0 && j == 0u && !(d.flags & ZB_CHUNK_HEAD)) {
+      uint64_t n;
+      bool closed;
+      x.launch_out[1] = walk(c, 0u, n, closed);  // the stream's open interval continues up to the first point
+    }
+    lo = o + 1ull;
+  }
+  if (c == w.n_chunks - 1u) x.launch_out[0] = o;
+}
+
+// ------------------------------------------------------------------------------------
+#define PK_ROW_WORDS 17  // a 32-byte window encodes to at most 32 x 15 bits = 15 words (+ partial)
 #define PK_STG_WORDS (PK_ROW_WORDS * 32 + 4)   // one batch of 32 rows + the carried partial word
 #define PK_EDGES 10       // piece boundaries of a chunk: header+warp 0, warps 1..7, tail, end
 // While a batch's tokens are walked, stg holds only its carried word (stg[0]) and zeros, so the batch's inputs are
@@ -1373,7 +1493,10 @@ size_t zb_lz2_table_bytes(int *grid_out) {
 // the k_lz instance for a level's matcher (MODE) and a format's checksum (CK)
 typedef void (*ZbLzKernel)(const uint8_t *, const ZbChunkDesc *, uint2 *, uint32_t *, uint16_t *, ZbChunkCheck *,
                            const ZbCrcTables *);
-static ZbLzKernel zb_lz_kernel(int mode, int data_format) {
+// (index_crc: the raw CRC-32 too, for a compress-time index: zlib takes both checksums, raw DEFLATE gzip's instance)
+static ZbLzKernel zb_lz_kernel(int mode, int data_format, bool index_crc = false) {
+  if (index_crc && data_format == ZB_DF_ZLIB) return mode ? k_lz<1, ZB_CK_CRC | ZB_CK_ADLER> : k_lz<0, ZB_CK_CRC | ZB_CK_ADLER>;
+  if (index_crc) data_format = ZB_DF_GZIP;
   const int ck = data_format == ZB_DF_GZIP ? ZB_CK_CRC : data_format == ZB_DF_ZLIB ? ZB_CK_ADLER : 0;
   if (mode) return ck == ZB_CK_CRC ? k_lz<1, ZB_CK_CRC> : ck == ZB_CK_ADLER ? k_lz<1, ZB_CK_ADLER> : k_lz<1, 0>;
   return ck == ZB_CK_CRC ? k_lz<0, ZB_CK_CRC> : ck == ZB_CK_ADLER ? k_lz<0, ZB_CK_ADLER> : k_lz<0, 0>;
@@ -1383,8 +1506,8 @@ cudaError_t zb_setup_deflate_attrs() {
   cudaError_t e = cudaSuccess;
   static const int fmts[3] = {ZB_DF_GZIP, ZB_DF_ZLIB, ZB_DF_DEFLATE};
   for (int mode = 0; mode < 2; mode++)
-    for (int f = 0; f < 3; f++) {
-      const ZbLzKernel k = zb_lz_kernel(mode, fmts[f]);
+    for (int f = 0; f < 4; f++) {
+      const ZbLzKernel k = f < 3 ? zb_lz_kernel(mode, fmts[f]) : zb_lz_kernel(mode, ZB_DF_ZLIB, true);
       if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, LZ_SM_TOTAL);
       // three CTAs of 75 KiB: ask for the largest shared-memory carve-out
       if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
@@ -1397,9 +1520,10 @@ cudaError_t zb_setup_deflate_attrs() {
   if (e == cudaSuccess) e = cudaFuncGetAttributes(&fa, k_scan);
   if (e == cudaSuccess) e = cudaFuncGetAttributes(&fa, k_member_check);
   if (e == cudaSuccess) e = cudaFuncGetAttributes(&fa, k_pack);
+  if (e == cudaSuccess) e = cudaFuncGetAttributes(&fa, k_index_rec);
   return e;
 }
-cudaError_t zb_launch_lz(const ZbCompressWork &w, cudaStream_t s) {
+cudaError_t zb_launch_lz(const ZbCompressWork &w, cudaStream_t s, bool index_crc) {
   if (w.n_chunks == 0) return cudaSuccess;
   if (zb_is_lz_level(w.level)) {
     int grid = 0;
@@ -1412,7 +1536,7 @@ cudaError_t zb_launch_lz(const ZbCompressWork &w, cudaStream_t s) {
       k_lz2<false><<<grid, LZ_THREADS, LZ2_SM_TOTAL, s>>>(w.src, w.desc, w.masks, w.recs, w.hist, w.chk, w.tabs, w.lz2_tables,
                                                           w.n_chunks, zb_lz2_params(w.level), nullptr, 0u, 0u);
   } else {
-    const ZbLzKernel k = zb_lz_kernel((w.level == -2 || w.level == 0) ? 0 : 1, w.data_format);
+    const ZbLzKernel k = zb_lz_kernel((w.level == -2 || w.level == 0) ? 0 : 1, w.data_format, index_crc);
     k<<<w.n_chunks, LZ_THREADS, LZ_SM_TOTAL, s>>>(w.src, w.desc, w.masks, w.recs, w.hist, w.chk, w.tabs);
   }
   return cudaGetLastError();
@@ -1425,6 +1549,11 @@ cudaError_t zb_launch_huff(const ZbCompressWork &w, cudaStream_t s) {
 cudaError_t zb_launch_scan(const ZbCompressWork &w, cudaStream_t s) {
   k_scan<<<1, SCAN_THREADS, 0, s>>>(w);
   if (w.n_members) k_member_check<<<(w.n_members + 3) / 4, 128, 0, s>>>(w);  // one warp per member
+  return cudaGetLastError();
+}
+cudaError_t zb_launch_index_rec(const ZbCompressWork &w, const ZbIndexWork &x, cudaStream_t s) {
+  if (w.n_chunks == 0) return cudaSuccess;
+  k_index_rec<<<(w.n_chunks + 127) / 128, 128, 0, s>>>(w, x);
   return cudaGetLastError();
 }
 cudaError_t zb_launch_pack(const ZbCompressWork &w, cudaStream_t s) {

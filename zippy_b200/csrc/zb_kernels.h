@@ -83,10 +83,30 @@ struct ZbLz2Params {
 };
 ZbLz2Params zb_lz2_params(int level);
 size_t zb_lz2_table_bytes(int *grid_out);
-cudaError_t zb_launch_lz(const ZbCompressWork &w, cudaStream_t s);
+// index_crc: the chunk checksums also hold the raw CRC-32 whatever the format (a compress-time index needs it)
+cudaError_t zb_launch_lz(const ZbCompressWork &w, cudaStream_t s, bool index_crc = false);
 cudaError_t zb_launch_huff(const ZbCompressWork &w, cudaStream_t s);
 cudaError_t zb_launch_scan(const ZbCompressWork &w, cudaStream_t s);
 cudaError_t zb_launch_pack(const ZbCompressWork &w, cudaStream_t s);
+// A compress-time index (k_index_rec, after k_scan): the access-point records of zb200_index_build's recorder
+// (ZbInflateWork::rec), taken from the block layout the compressor wrote instead of a decode.  A block start
+// owns the multiples k * 32768 in (the previous block start's output offset, its own]; a member's first block owns
+// k = 0.  For each owned k, record r = rec_first[member] + k - k0 receives rec[2r] = the bit position in the member,
+// rec[2r + 1] = the member output offset; a block start that owns a multiple is a point, and crc[r] of its first
+// one receives the CRC-32 of its interval (up to the next point or the member end) -- the raw (init 0) CRC
+// instead when the interval runs past the end of a stream launch.  Records nobody owns stay as they were.
+struct ZbIndexWork {
+  uint64_t *rec;
+  uint32_t *crc;
+  const uint64_t *rec_first;   // [n_members] of the launch group
+  uint64_t k0;                 // 0; a stream launch: the first multiple it can own
+  uint64_t lo0;                // a stream launch that continues a member: the previous block start's output offset + 1
+  uint64_t byte_base;          // a stream launch: the member bytes earlier launches wrote
+  // [0]: the output offset of the launch's last block start; [1]: the raw CRC-32 of the output from the start of
+  // a launch that continues a member up to its first point (or its end), 0 when that is empty (zeroed by the host)
+  uint64_t *launch_out;
+};
+cudaError_t zb_launch_index_rec(const ZbCompressWork &w, const ZbIndexWork &x, cudaStream_t s);
 // ---- inflate ----
 struct ZbInflateWork {
   const uint8_t *src;          // device
