@@ -161,13 +161,24 @@ struct StageRing {
   size_t next = 0;
 };
 
+// The small device words of the decode paths (zb200_ctx::counter).  Whoever uses a word sets it before a kernel reads
+// it; the launch wrappers zero the work-queue counters and candidate counts themselves.
+struct ZbCounters {
+  uint32_t member;      // work-queue counter of a whole-member inflate launch
+  uint32_t segment;     // work-queue counter of a segment launch (seg_pass)
+  uint32_t cand;        // candidates found by k_find_sync / k_find_blocks (find_candidates)
+  int bad;              // the marker resolve: a marker points before the start of the stream
+  uint64_t resume[2];   // ZbInflateWork::resume of a decompress stream's counting pass
+};
+
 struct zb200_ctx {
   int device = 0;
   cudaStream_t stream = nullptr;
   cudaStream_t own_stream = nullptr;
   ZbCrcTables *d_tabs = nullptr;
   DevBuf desc, member_first, fname, masks, recs, hist, chk, cb, chunk_off, member_off, member_check, member_isize;
-  DevBuf src_off, dst_off, out_len, status, expect, kind, counter, ck_out, ck_pieces, ck_first, ck_piece_out, ck_partials;
+  DevBuf src_off, dst_off, out_len, status, expect, kind, ck_out, ck_pieces, ck_first, ck_piece_out, ck_partials;
+  DevBuf counter;           // ZbCounters (allocated with the ctx), then uncompress_host_pipelined's per-group counters
   DevBuf in_stage, out_stage, lz2_tables;
   DevBuf carry;             // a compress stream's member carry: [0] in, [1] out
   size_t stream_batch_bytes = ZB_STREAM_BATCH_BYTES;  // pending input at which a stream write launches
@@ -321,6 +332,8 @@ int ensure(zb200_ctx *ctx, DevBuf &b, size_t bytes) {
     int _rc = ensure(ctx, (buf), (bytes));         \
     if (_rc != ZB200_OK) return _rc;               \
   } while (0)
+
+ZbCounters *counters(zb200_ctx *ctx) { return (ZbCounters *)ctx->counter.p; }
 
 struct DeviceGuard {
   int prev = -1;
@@ -1090,6 +1103,142 @@ struct BigResult {
   int status = ZB200_OK;
 };
 
+// ---- the mechanics every parallel segment decode shares ----
+// (The large-member, decompress stream and index paths decide what to launch; the helpers launch it.  Launch counts
+// stay with the callers, in timing.kernel_launches, where each path keeps its own convention.)
+
+// Segment start candidates in src, sorted: with `blocks`, the bit positions in [lo, hi) where a dynamic block could
+// start (k_find_blocks; bytes from limit_byte on read as zero), else the byte positions in [lo, hi) just past a
+// 00 00 ff ff (k_find_sync).  Empty when there are none, or more than cap (then the list is incomplete).
+int find_candidates(zb200_ctx *ctx, bool blocks, const uint8_t *src, uint64_t lo, uint64_t hi, uint64_t limit_byte,
+                    uint32_t cap, std::vector<uint64_t> &cand) {
+  cudaStream_t s = ctx->stream;
+  cand.clear();
+  ENSURE(ctx->seg_cand, (size_t)cap * 8 + 16);
+  uint32_t *d_cnt = &counters(ctx)->cand;
+  if (blocks) CK(zb_launch_find_blocks(src, lo, hi, limit_byte, (uint64_t *)ctx->seg_cand.p, cap, d_cnt, s));
+  else CK(zb_launch_find_sync(src, lo, hi, (uint64_t *)ctx->seg_cand.p, cap, d_cnt, s));
+  uint32_t cnt = 0;
+  CK(cudaMemcpyAsync(&cnt, d_cnt, 4, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  if (cnt == 0 || cnt > cap) return ZB200_OK;
+  cand.resize(cnt);
+  CK(cudaMemcpyAsync(cand.data(), ctx->seg_cand.p, (size_t)cnt * 8, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  std::sort(cand.begin(), cand.end());
+  return ZB200_OK;
+}
+
+// Uploads segment (start, end) bit pairs to seg_bits, for w.seg_bits.
+int seg_bits_upload(zb200_ctx *ctx, const std::vector<uint64_t> &pairs, ZbInflateWork &w) {
+  ENSURE(ctx->seg_bits, pairs.size() * 8);
+  CK(cudaMemcpyAsync(ctx->seg_bits.p, pairs.data(), pairs.size() * 8, cudaMemcpyHostToDevice, ctx->stream));
+  w.seg_bits = (const uint64_t *)ctx->seg_bits.p;
+  return ZB200_OK;
+}
+
+// The n segments [b[0], b[1]), ..., [b[n - 1], end) of n consecutive boundaries and an end (bit positions), uploaded.
+int seg_bounds_upload(zb200_ctx *ctx, const uint64_t *b, size_t n, uint64_t end, ZbInflateWork &w) {
+  std::vector<uint64_t> pairs(2 * n);
+  for (size_t i = 0; i < n; i++) {
+    pairs[2 * i] = b[i];
+    pairs[2 * i + 1] = i + 1 < n ? b[i + 1] : end;
+  }
+  return seg_bits_upload(ctx, pairs, w);
+}
+
+// One segment-mode k_inflate launch over n segments of the raw DEFLATE stream at w.src.  w holds only what the caller
+// decides: src, seg_bits (uploaded) or src_off, seg_limit, seg_win0, dst (its offsets are seg_dst), count_only / mark,
+// rec*.  Returns every segment's output length, status and kind after one synchronise.  resume: null, or host [2]
+// uploaded as ZbInflateWork::resume before the launch and read back with the rest.
+int seg_pass(zb200_ctx *ctx, ZbInflateWork w, size_t n, std::vector<uint64_t> &sl, std::vector<int> &sst,
+             std::vector<uint32_t> &sk, uint64_t *resume = nullptr) {
+  cudaStream_t s = ctx->stream;
+  ENSURE(ctx->seg_len, n * 8);
+  ENSURE(ctx->seg_status, n * 4);
+  ENSURE(ctx->seg_kind, n * 4);
+  ENSURE(ctx->seg_expect, n * 4);
+  if (resume) {
+    w.resume = counters(ctx)->resume;
+    CK(cudaMemcpyAsync(w.resume, resume, 16, cudaMemcpyHostToDevice, s));
+  }
+  w.dst_off = (const uint64_t *)ctx->seg_dst.p;
+  w.out_len = (uint64_t *)ctx->seg_len.p;
+  w.status = (int *)ctx->seg_status.p;
+  w.expect = (uint32_t *)ctx->seg_expect.p;
+  w.kind = (uint32_t *)ctx->seg_kind.p;
+  w.counter = &counters(ctx)->segment;
+  w.tabs = ctx->d_tabs;
+  w.n = (uint32_t)n;
+  w.data_format = ZB200_DF_DEFLATE;
+  w.seg_mode = 1;
+  CK(zb_launch_inflate(w, s));
+  sl.resize(n);
+  sst.resize(n);
+  sk.resize(n);
+  CK(cudaMemcpyAsync(sl.data(), ctx->seg_len.p, n * 8, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(sst.data(), ctx->seg_status.p, n * 4, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(sk.data(), ctx->seg_kind.p, n * 4, cudaMemcpyDeviceToHost, s));
+  if (resume) CK(cudaMemcpyAsync(resume, w.resume, 16, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  return ZB200_OK;
+}
+
+// Uploads a marker layout for a marker pass and the resolve -- segs to mark_segs, every segment's first element
+// offset in the scratch to seg_dst (dof.back(): the scratch's size in elements) -- and fills the marker symbols in
+// front of every segment (k_mark_prefill).
+int mark_upload(zb200_ctx *ctx, const std::vector<ZbMarkSegHost> &segs, const std::vector<uint64_t> &dof) {
+  cudaStream_t s = ctx->stream;
+  ENSURE(ctx->mark_scratch, (size_t)dof.back() * 2 + 64);
+  ENSURE(ctx->mark_segs, segs.size() * sizeof(ZbMarkSegHost) + 16);
+  ENSURE(ctx->seg_dst, dof.size() * 8);
+  CK(cudaMemcpyAsync(ctx->seg_dst.p, dof.data(), dof.size() * 8, cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(ctx->mark_segs.p, segs.data(), segs.size() * sizeof(ZbMarkSegHost), cudaMemcpyHostToDevice, s));
+  CK(zb_launch_mark_prefill((uint16_t *)ctx->mark_scratch.p, ctx->mark_segs.p, (uint32_t)segs.size(), s));
+  return ZB200_OK;
+}
+
+// The marker layout of n consecutive segments of sizes[i] output bytes, [32768 markers | sizes[i] symbols] each, whose
+// bytes go to dst0 on in order; uploaded and prefilled (mark_upload).  max_n: the largest size.
+int mark_segments(zb200_ctx *ctx, const uint64_t *sizes, size_t n, uint64_t dst0, std::vector<ZbMarkSegHost> &segs,
+                  uint32_t &max_n) {
+  segs.resize(n);
+  std::vector<uint64_t> dof(n + 1);
+  uint64_t se = 0, de = dst0;
+  max_n = 0;
+  for (size_t i = 0; i < n; i++) {
+    se += 32768ull;
+    segs[i].scr = se;
+    segs[i].dst = de;
+    segs[i].n = (uint32_t)sizes[i];
+    segs[i].pad = 0;
+    dof[i] = se;
+    se += sizes[i];
+    de += sizes[i];
+    max_n = std::max<uint32_t>(max_n, (uint32_t)sizes[i]);
+  }
+  dof[n] = se;
+  return mark_upload(ctx, segs, dof);
+}
+
+// The parallel window resolve (zb_resolve.h) of the n segments in mark_segs into dst, in groups of ceil(sqrt(n))
+// segments; base / w0 as in zb_kernels.h.  bad: null, or where to read the `bad` flag after the resolve (one
+// synchronise); the flag is cleared by the caller, once for all the windows it gathers.
+int resolve_window(zb200_ctx *ctx, size_t n, uint32_t max_n, uint64_t base, uint64_t w0, uint8_t *dst, int *bad) {
+  cudaStream_t s = ctx->stream;
+  const uint32_t gsz = std::max<uint32_t>(1u, (uint32_t)std::ceil(std::sqrt((double)n)));
+  const size_t ngroups = (n + gsz - 1) / gsz;
+  ENSURE(ctx->mark_win, ngroups * 32768ull * 3);
+  int *d_bad = &counters(ctx)->bad;
+  CK(zb_launch_resolve_groups((uint16_t *)ctx->mark_scratch.p, ctx->mark_segs.p, (uint32_t)n, max_n, gsz, base, w0,
+                              (uint16_t *)ctx->mark_win.p, (uint8_t *)ctx->mark_win.p + ngroups * 65536ull, dst, d_bad, s));
+  if (bad) {
+    CK(cudaMemcpyAsync(bad, d_bad, 4, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+  }
+  return ZB200_OK;
+}
+
 // ---- a large member WITHOUT sync markers (any foreign gzip / zlib / raw stream) ----
 // 1. k_find_blocks lists every plausible dynamic-block start in the payload; the list is thinned to one
 //    boundary per >= 16 KiB of input.  2. A counting pass decodes every segment [boundary i, boundary i+1)
@@ -1110,19 +1259,11 @@ int inflate_member_speculative(zb200_ctx *ctx, const uint8_t *d_src, uint64_t m0
   cudaStream_t s = ctx->stream;
   const uint64_t lo_bit = (m0 + hw.pos) * 8ull, hi_bit = (m0 + hw.end) * 8ull, limit_byte = m0 + hw.end;
   const uint32_t cap = (uint32_t)std::min<uint64_t>((hw.end - hw.pos) / 64 + 1024, 1u << 24);
-  ENSURE(ctx->seg_cand, (size_t)cap * 8 + 16);
-  ENSURE(ctx->counter, 64);
-  uint32_t *d_cnt = (uint32_t *)ctx->counter.p + 8;
-  CK(zb_launch_find_blocks(d_src, lo_bit, hi_bit, limit_byte, (uint64_t *)ctx->seg_cand.p, cap, d_cnt, s));
-  uint32_t cnt = 0;
-  CK(cudaMemcpyAsync(&cnt, d_cnt, 4, cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
+  std::vector<uint64_t> cand;
+  int rc = find_candidates(ctx, true, d_src, lo_bit, hi_bit, limit_byte, cap, cand);
+  if (rc) return rc;
   ctx->timing.kernel_launches += 1;
-  if (cnt == 0 || cnt > cap) return ZB200_OK;
-  std::vector<uint64_t> cand(cnt);
-  CK(cudaMemcpyAsync(cand.data(), ctx->seg_cand.p, (size_t)cnt * 8, cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
-  std::sort(cand.begin(), cand.end());
+  if (cand.empty()) return ZB200_OK;
   // boundaries: the payload start, then candidates at least min_gap apart (a segment costs a 64 KiB marker prefill)
   // (at most 60000 segments: the resolve kernels index them with a grid dimension)
   // a single input is all the GPU has: cut it as finely as its blocks allow
@@ -1132,56 +1273,24 @@ int inflate_member_speculative(zb200_ctx *ctx, const uint8_t *d_src, uint64_t m0
     if (c >= bits.back() + min_gap && c + min_gap / 4 < hi_bit) bits.push_back(c);
   const size_t S = bits.size();
   if (S < 2) return ZB200_OK;
-  std::vector<uint64_t> sb(2 * S);
-  for (size_t i = 0; i < S; i++) {
-    sb[2 * i] = bits[i];
-    sb[2 * i + 1] = i + 1 < S ? bits[i + 1] : hi_bit;
-  }
-  ENSURE(ctx->seg_bits, 2 * S * 8);
-  ENSURE(ctx->seg_dst, (S + 1) * 8);
-  ENSURE(ctx->seg_len, S * 8);
-  ENSURE(ctx->seg_status, S * 4);
-  ENSURE(ctx->seg_kind, S * 4);
-  ENSURE(ctx->seg_expect, S * 4);
-  CK(cudaMemcpyAsync(ctx->seg_bits.p, sb.data(), 2 * S * 8, cudaMemcpyHostToDevice, s));
   ZbInflateWork w;
   memset(&w, 0, sizeof(w));
   w.src = d_src;
-  w.seg_bits = (const uint64_t *)ctx->seg_bits.p;
   w.seg_limit = limit_byte;
-  w.dst_off = (const uint64_t *)ctx->seg_dst.p;
-  w.out_len = (uint64_t *)ctx->seg_len.p;
-  w.status = (int *)ctx->seg_status.p;
-  w.expect = (uint32_t *)ctx->seg_expect.p;
-  w.kind = (uint32_t *)ctx->seg_kind.p;
-  w.counter = (uint32_t *)ctx->counter.p + 4;
-  w.tabs = ctx->d_tabs;
-  w.n = (uint32_t)S;
-  w.data_format = ZB200_DF_DEFLATE;
-  w.seg_mode = 1;
-  std::vector<uint64_t> sl(S);
-  std::vector<int> sst(S);
-  std::vector<uint32_t> sk(S);
-  auto fetch = [&]() -> int {
-    CK(cudaMemcpyAsync(sl.data(), ctx->seg_len.p, S * 8, cudaMemcpyDeviceToHost, s));
-    CK(cudaMemcpyAsync(sst.data(), ctx->seg_status.p, S * 4, cudaMemcpyDeviceToHost, s));
-    CK(cudaMemcpyAsync(sk.data(), ctx->seg_kind.p, S * 4, cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
-    return ZB200_OK;
-  };
+  rc = seg_bounds_upload(ctx, bits.data(), S, hi_bit, w);
+  if (rc) return rc;
+  std::vector<uint64_t> sl;
+  std::vector<int> sst;
+  std::vector<uint32_t> sk;
   // 2. the counting pass
   w.count_only = 1;
-  CK(zb_launch_inflate(w, s));
-  int rc = fetch();
+  rc = seg_pass(ctx, w, S, sl, sst, sk);
   if (rc) return rc;
   ctx->timing.kernel_launches += 1;
-  uint64_t total = 0, scr_elems = 0;
-  uint32_t max_n = 0;
+  uint64_t total = 0;
   for (size_t i = 0; i < S; i++) {
     if (sst[i] != ZB200_OK || (sk[i] != 0) != (i + 1 == S) || sl[i] > 0xf0000000ull) return ZB200_OK;
     total += sl[i];
-    scr_elems += 32768ull + sl[i];
-    max_n = std::max<uint32_t>(max_n, (uint32_t)sl[i]);
   }
   if (count_only) {
     ok = true;
@@ -1193,33 +1302,17 @@ int inflate_member_speculative(zb200_ctx *ctx, const uint8_t *d_src, uint64_t m0
     return ZB200_OK;
   }
   // 3. uint16 symbols, markers in front of every segment
-  ENSURE(ctx->mark_scratch, (size_t)scr_elems * 2 + 64);
-  ENSURE(ctx->mark_segs, S * sizeof(ZbMarkSegHost) + 16);
-  std::vector<ZbMarkSegHost> segs(S);
-  std::vector<uint64_t> dof(S + 1);
-  uint64_t se = 0, de = dst0;
-  for (size_t i = 0; i < S; i++) {
-    se += 32768ull;
-    segs[i].scr = se;
-    segs[i].dst = de;
-    segs[i].n = (uint32_t)sl[i];
-    segs[i].pad = 0;
-    dof[i] = se;
-    se += sl[i];
-    de += sl[i];
-  }
-  dof[S] = se;
   const std::vector<uint64_t> want = sl;
-  CK(cudaMemcpyAsync(ctx->mark_segs.p, segs.data(), S * sizeof(ZbMarkSegHost), cudaMemcpyHostToDevice, s));
-  CK(cudaMemcpyAsync(ctx->seg_dst.p, dof.data(), (S + 1) * 8, cudaMemcpyHostToDevice, s));
-  int *d_bad = (int *)((uint32_t *)ctx->counter.p + 12);
+  int *d_bad = &counters(ctx)->bad;
   CK(cudaMemsetAsync(d_bad, 0, 4, s));
-  CK(zb_launch_mark_prefill((uint16_t *)ctx->mark_scratch.p, ctx->mark_segs.p, (uint32_t)S, s));
+  std::vector<ZbMarkSegHost> segs;
+  uint32_t max_n = 0;
+  rc = mark_segments(ctx, want.data(), S, dst0, segs, max_n);
+  if (rc) return rc;
   w.count_only = 0;
   w.mark = 1;
   w.dst = (uint8_t *)ctx->mark_scratch.p;
-  CK(zb_launch_inflate(w, s));
-  rc = fetch();
+  rc = seg_pass(ctx, w, S, sl, sst, sk);
   if (rc) return rc;
   ctx->timing.kernel_launches += 2;
   for (size_t i = 0; i < S; i++)
@@ -1247,7 +1340,7 @@ int inflate_member_speculative(zb200_ctx *ctx, const uint8_t *d_src, uint64_t m0
 // The member is processed in windows of segments (ctx->mark_window_segs, and about as much output as that many
 // full chunks): every window starts from the resolved output in front of it, so the scratch depends on the
 // window, not on the member.  Anything irregular leaves the member to the speculative and serial paths.
-// bounds: absolute byte offsets of the S + 1 segment boundaries in d_src.
+// bounds: absolute bit offsets of the S + 1 (byte-aligned) segment boundaries in d_src.
 int inflate_member_joints(zb200_ctx *ctx, const uint8_t *d_src, uint64_t limit_byte, std::vector<uint64_t> bounds,
                           uint8_t *d_dst, uint64_t dst0, uint64_t mcap, bool count_only, bool guess, bool &ok,
                           uint64_t &out_len, bool &too_small) {
@@ -1258,48 +1351,18 @@ int inflate_member_joints(zb200_ctx *ctx, const uint8_t *d_src, uint64_t limit_b
   memset(&w, 0, sizeof(w));
   w.src = d_src;
   w.seg_limit = limit_byte;
-  w.tabs = ctx->d_tabs;
-  w.data_format = ZB200_DF_DEFLATE;
-  w.seg_mode = 1;
-  std::vector<uint64_t> sl, sb;
+  std::vector<uint64_t> sl;
   std::vector<int> sst;
   std::vector<uint32_t> sk;
   // one decode launch over segments [a, b): counting, or marker symbols into mark_scratch at seg_dst
   auto run = [&](size_t a, size_t b, bool count) -> int {
-    const size_t nw = b - a;
-    sb.resize(2 * nw);
-    for (size_t i = 0; i < nw; i++) {
-      sb[2 * i] = bounds[a + i] * 8ull;
-      sb[2 * i + 1] = bounds[a + i + 1] * 8ull;
-    }
-    ENSURE(ctx->seg_bits, 2 * nw * 8);
-    ENSURE(ctx->seg_len, nw * 8);
-    ENSURE(ctx->seg_status, nw * 4);
-    ENSURE(ctx->seg_kind, nw * 4);
-    ENSURE(ctx->seg_expect, nw * 4);
-    ENSURE(ctx->counter, 64);
-    CK(cudaMemcpyAsync(ctx->seg_bits.p, sb.data(), 2 * nw * 8, cudaMemcpyHostToDevice, s));
-    w.seg_bits = (const uint64_t *)ctx->seg_bits.p;
+    int rc = seg_bounds_upload(ctx, bounds.data() + a, b - a, bounds[b], w);
+    if (rc) return rc;
     w.dst = count ? nullptr : (uint8_t *)ctx->mark_scratch.p;
-    w.dst_off = (const uint64_t *)ctx->seg_dst.p;
-    w.out_len = (uint64_t *)ctx->seg_len.p;
-    w.status = (int *)ctx->seg_status.p;
-    w.expect = (uint32_t *)ctx->seg_expect.p;
-    w.kind = (uint32_t *)ctx->seg_kind.p;
-    w.counter = (uint32_t *)ctx->counter.p + 4;
-    w.n = (uint32_t)nw;
     w.seg_win0 = a > 0;
     w.count_only = count ? 1 : 0;
     w.mark = count ? 0 : 1;
-    CK(zb_launch_inflate(w, s));
-    sl.resize(nw);
-    sst.resize(nw);
-    sk.resize(nw);
-    CK(cudaMemcpyAsync(sl.data(), ctx->seg_len.p, nw * 8, cudaMemcpyDeviceToHost, s));
-    CK(cudaMemcpyAsync(sst.data(), ctx->seg_status.p, nw * 4, cudaMemcpyDeviceToHost, s));
-    CK(cudaMemcpyAsync(sk.data(), ctx->seg_kind.p, nw * 4, cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
-    return ZB200_OK;
+    return seg_pass(ctx, w, b - a, sl, sst, sk);
   };
   // exact sizes of every segment, with the repair rounds; counted = false: give up on this path
   std::vector<uint64_t> size;
@@ -1355,11 +1418,9 @@ int inflate_member_joints(zb200_ctx *ctx, const uint8_t *d_src, uint64_t limit_b
     return ZB200_OK;
   }
   const uint64_t W = ctx->mark_window_segs, win_elems = W * (32768ull + ZB_CHUNK_BYTES);
-  ENSURE(ctx->counter, 64);
-  int *d_bad = (int *)((uint32_t *)ctx->counter.p + 12);
-  CK(cudaMemsetAsync(d_bad, 0, 4, s));
+  CK(cudaMemsetAsync(&counters(ctx)->bad, 0, 4, s));
+  int bad = 0;   // every window's resolve sets the flag; it is read after the last one
   std::vector<ZbMarkSegHost> segs;
-  std::vector<uint64_t> dof;
   uint64_t dpos = dst0;
   for (size_t a = 0; a < bounds.size() - 1;) {
     const size_t S = bounds.size() - 1;
@@ -1372,30 +1433,13 @@ int inflate_member_joints(zb200_ctx *ctx, const uint8_t *d_src, uint64_t limit_b
       b++;
     }
     const size_t nw = b - a;
-    segs.resize(nw);
-    dof.resize(nw + 1);
-    uint64_t se = 0, dp = dpos;
+    std::vector<uint64_t> guessed;
+    if (!counted) guessed.assign(nw, ZB_CHUNK_BYTES);
     uint32_t max_n = 0;
-    for (size_t i = 0; i < nw; i++) {
-      const uint64_t n = counted ? size[a + i] : ZB_CHUNK_BYTES;
-      se += 32768ull;
-      segs[i].scr = se;
-      segs[i].dst = dp;
-      segs[i].n = (uint32_t)n;
-      segs[i].pad = 0;
-      dof[i] = se;
-      se += n;
-      dp += n;
-      max_n = std::max<uint32_t>(max_n, (uint32_t)n);
-    }
-    dof[nw] = se;
-    ENSURE(ctx->mark_scratch, (size_t)se * 2 + 64);
-    ENSURE(ctx->mark_segs, nw * sizeof(ZbMarkSegHost) + 16);
-    ENSURE(ctx->seg_dst, (nw + 1) * 8);
-    CK(cudaMemcpyAsync(ctx->seg_dst.p, dof.data(), (nw + 1) * 8, cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(ctx->mark_segs.p, segs.data(), nw * sizeof(ZbMarkSegHost), cudaMemcpyHostToDevice, s));
-    CK(zb_launch_mark_prefill((uint16_t *)ctx->mark_scratch.p, ctx->mark_segs.p, (uint32_t)nw, s));
-    int rc = run(a, b, false);
+    int rc = mark_segments(ctx, counted ? size.data() + a : guessed.data(), nw, dpos, segs, max_n);
+    if (rc) return rc;
+    uint64_t dp = segs[nw - 1].dst + segs[nw - 1].n;
+    rc = run(a, b, false);
     if (rc) return rc;
     ctx->timing.kernel_launches += 2;
     bool wok = true;
@@ -1428,19 +1472,12 @@ int inflate_member_joints(zb200_ctx *ctx, const uint8_t *d_src, uint64_t limit_b
       CK(cudaMemcpyAsync((ZbMarkSegHost *)ctx->mark_segs.p + (nw - 1), &segs[nw - 1], sizeof(ZbMarkSegHost),
                          cudaMemcpyHostToDevice, s));
     }
-    const uint32_t gsz = std::max<uint32_t>(1u, (uint32_t)std::ceil(std::sqrt((double)nw)));
-    const size_t ngroups = (nw + gsz - 1) / gsz;
-    ENSURE(ctx->mark_win, ngroups * 32768ull * 3);
-    CK(zb_launch_resolve_groups((uint16_t *)ctx->mark_scratch.p, ctx->mark_segs.p, (uint32_t)nw, max_n, gsz, dst0,
-                                dpos - dst0, (uint16_t *)ctx->mark_win.p, (uint8_t *)ctx->mark_win.p + ngroups * 65536ull,
-                                d_dst, d_bad, s));
+    rc = resolve_window(ctx, nw, max_n, dst0, dpos - dst0, d_dst, b == S ? &bad : nullptr);
+    if (rc) return rc;
     ctx->timing.kernel_launches += 4;
     dpos = dp;
     a = b;
   }
-  int bad = 0;
-  CK(cudaMemcpyAsync(&bad, d_bad, 4, cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
   if (bad) return ZB200_OK;
   ok = true;
   out_len = dpos - dst0;
@@ -1501,66 +1538,35 @@ int inflate_big_members(zb200_ctx *ctx, const uint8_t *d_src, const uint64_t *sr
   }
     // 1. candidate boundaries
     const uint32_t cap = (uint32_t)std::min<uint64_t>((hw.end - hw.pos) / 32 + 64, 1u << 24);
-    ENSURE(ctx->seg_cand, (size_t)cap * 8 + 16);
-    ENSURE(ctx->counter, 64);
-    uint32_t *d_cnt = (uint32_t *)ctx->counter.p + 8;
-    CK(zb_launch_find_sync(d_src + m0, hw.pos, hw.end, (uint64_t *)ctx->seg_cand.p, cap, d_cnt, s));
-    uint32_t cnt = 0;
-    CK(cudaMemcpyAsync(&cnt, d_cnt, 4, cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
-    if (cnt == 0 || cnt > cap) ZB_TRY_SPECULATIVE();
-    std::vector<uint64_t> bounds(cnt + 2);
-    CK(cudaMemcpyAsync(bounds.data() + 1, ctx->seg_cand.p, (size_t)cnt * 8, cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
-    std::sort(bounds.begin() + 1, bounds.begin() + 1 + cnt);
-    bounds[0] = hw.pos;
-    size_t S = cnt + 1;
-    if (bounds[cnt] >= hw.end) S = cnt;  // the payload ends with a marker: no trailing segment
-    else bounds[cnt + 1] = hw.end;
+    std::vector<uint64_t> bounds;
+    int rc = find_candidates(ctx, false, d_src + m0, hw.pos, hw.end, 0, cap, bounds);
+    if (rc) return rc;
+    if (bounds.empty()) ZB_TRY_SPECULATIVE();
+    bounds.insert(bounds.begin(), hw.pos);
+    if (bounds.back() < hw.end) bounds.push_back(hw.end);   // (a payload that ends with a marker: no trailing segment)
+    const size_t S = bounds.size() - 1;
     if (S < 2) ZB_TRY_SPECULATIVE();
     for (size_t j = 0; j <= S; j++) bounds[j] += m0;  // absolute in d_src
     ENSURE(ctx->seg_src, (S + 1) * 8);
     ENSURE(ctx->seg_dst, (S + 1) * 8);
-    ENSURE(ctx->seg_len, S * 8);
-    ENSURE(ctx->seg_status, S * 4);
-    ENSURE(ctx->seg_kind, S * 4);
-    ENSURE(ctx->seg_expect, S * 4);
     CK(cudaMemcpyAsync(ctx->seg_src.p, bounds.data(), (S + 1) * 8, cudaMemcpyHostToDevice, s));
     ZbInflateWork w;
     memset(&w, 0, sizeof(w));
     w.src = d_src;
     w.src_off = (const uint64_t *)ctx->seg_src.p;
     w.dst = d_dst;
-    w.dst_off = (const uint64_t *)ctx->seg_dst.p;
-    w.out_len = (uint64_t *)ctx->seg_len.p;
-    w.status = (int *)ctx->seg_status.p;
-    w.expect = (uint32_t *)ctx->seg_expect.p;
-    w.kind = (uint32_t *)ctx->seg_kind.p;
-    w.counter = (uint32_t *)ctx->counter.p + 4;
-    w.tabs = ctx->d_tabs;
-    w.n = (uint32_t)S;
-    w.data_format = ZB200_DF_DEFLATE;
-    w.pos = 0;
-    w.seg_mode = 1;
-    std::vector<uint64_t> sl(S), dof(S + 1);
-    std::vector<int> sst(S);
-    std::vector<uint32_t> sk(S);
-    auto fetch = [&]() -> int {
-      CK(cudaMemcpyAsync(sl.data(), ctx->seg_len.p, S * 8, cudaMemcpyDeviceToHost, s));
-      CK(cudaMemcpyAsync(sst.data(), ctx->seg_status.p, S * 4, cudaMemcpyDeviceToHost, s));
-      CK(cudaMemcpyAsync(sk.data(), ctx->seg_kind.p, S * 4, cudaMemcpyDeviceToHost, s));
-      CK(cudaStreamSynchronize(s));
-      return ZB200_OK;
-    };
+    std::vector<uint64_t> sl, dof(S + 1);
+    std::vector<int> sst;
+    std::vector<uint32_t> sk;
     const uint64_t dst0 = count_only ? 0 : dst_offsets[m], mcap = count_only ? ~0ull : dst_offsets[m + 1] - dst_offsets[m];
     bool ok = false;
-    int rc;
     // segments that refer back across their joints: marker segments (inflate_member_joints); 1 = not handled there
     auto joints = [&](bool guess) -> int {
       if (!ctx->joint_markers) return 1;
       bool jok = false, small = false;
       uint64_t jlen = 0;
-      std::vector<uint64_t> jb(bounds.begin(), bounds.begin() + S + 1);
+      std::vector<uint64_t> jb(S + 1);
+      for (size_t j = 0; j <= S; j++) jb[j] = bounds[j] * 8ull;
       int rc_ = inflate_member_joints(ctx, d_src, m0 + hw.end, jb, d_dst, dst0, mcap, count_only, guess, jok, jlen, small);
       if (rc_) return -rc_;
       if (!jok && !small) return 1;
@@ -1589,8 +1595,7 @@ int inflate_big_members(zb200_ctx *ctx, const uint8_t *d_src, const uint64_t *sr
       dof[S] = dst0 + mcap;
       CK(cudaMemcpyAsync(ctx->seg_dst.p, dof.data(), (S + 1) * 8, cudaMemcpyHostToDevice, s));
       w.count_only = 0;
-      CK(zb_launch_inflate(w, s));
-      rc = fetch();
+      rc = seg_pass(ctx, w, S, sl, sst, sk);
       if (rc) return rc;
       ctx->timing.kernel_launches += 2;
       ok = true;
@@ -1609,8 +1614,7 @@ int inflate_big_members(zb200_ctx *ctx, const uint8_t *d_src, const uint64_t *sr
     if (!ok) {
       // 3. sizes from a count pass, then the real pass with every segment at its place
       w.count_only = 1;
-      CK(zb_launch_inflate(w, s));
-      rc = fetch();
+      rc = seg_pass(ctx, w, S, sl, sst, sk);
       if (rc) return rc;
       ctx->timing.kernel_launches += 2;
       ok = true;
@@ -1625,8 +1629,7 @@ int inflate_big_members(zb200_ctx *ctx, const uint8_t *d_src, const uint64_t *sr
         std::vector<uint64_t> want = sl;
         CK(cudaMemcpyAsync(ctx->seg_dst.p, dof.data(), (S + 1) * 8, cudaMemcpyHostToDevice, s));
         w.count_only = 0;
-        CK(zb_launch_inflate(w, s));
-        rc = fetch();
+        rc = seg_pass(ctx, w, S, sl, sst, sk);
         if (rc) return rc;
         ctx->timing.kernel_launches += 1;
         for (size_t j = 0; j < S && ok; j++) ok = sst[j] == ZB200_OK && sl[j] == want[j];
@@ -1691,44 +1694,28 @@ constexpr uint64_t kDstreamHeaderBits = 1024 * 8;
 // decode as a closed segment.  `path` names what was found ("joints", "blocks", or "serial": bits = {lo_bit}).
 int find_segment_bits(zb200_ctx *ctx, const uint8_t *d_src, uint64_t lo_bit, uint64_t pay_end, std::vector<uint64_t> &bits,
                       const char *&path) {
-  cudaStream_t s = ctx->stream;
   const uint64_t pay_bit = pay_end * 8ull;
   const uint64_t min_gap = std::max<uint64_t>(16384ull * 8ull, (pay_bit - std::min(pay_bit, lo_bit)) / 60000ull);
   bits.assign(1, lo_bit);
   path = "serial";
   if (pay_bit <= lo_bit + 2 * min_gap) return ZB200_OK;
-  ENSURE(ctx->counter, 128);
-  uint32_t *d_cnt = (uint32_t *)ctx->counter.p + 8;
   const uint64_t lo = (lo_bit + 7) / 8;
-  uint32_t cap = (uint32_t)std::min<uint64_t>((pay_end - lo) / 32 + 64, 1u << 24);
-  ENSURE(ctx->seg_cand, (size_t)cap * 8 + 16);
-  uint32_t cnt = 0;
-  CK(zb_launch_find_sync(d_src, lo, pay_end, (uint64_t *)ctx->seg_cand.p, cap, d_cnt, s));
-  CK(cudaMemcpyAsync(&cnt, d_cnt, 4, cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
-  ctx->timing.kernel_launches += 1;
   std::vector<uint64_t> cand;
-  if (cnt > 0 && cnt <= cap) {
-    cand.resize(cnt);
-    CK(cudaMemcpyAsync(cand.data(), ctx->seg_cand.p, (size_t)cnt * 8, cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
-    std::sort(cand.begin(), cand.end());
+  int rc = find_candidates(ctx, false, d_src, lo, pay_end, 0,
+                           (uint32_t)std::min<uint64_t>((pay_end - lo) / 32 + 64, 1u << 24), cand);
+  if (rc) return rc;
+  ctx->timing.kernel_launches += 1;
+  if (!cand.empty()) {
     for (uint64_t c : cand)
       if (c * 8 >= bits.back() + min_gap && c * 8 < pay_bit) bits.push_back(c * 8);
     path = "joints";
   }
   if (bits.size() < 2) {
-    cap = (uint32_t)std::min<uint64_t>((pay_end - lo) / 64 + 1024, 1u << 24);
-    ENSURE(ctx->seg_cand, (size_t)cap * 8 + 16);
-    CK(zb_launch_find_blocks(d_src, lo_bit, pay_bit, pay_end, (uint64_t *)ctx->seg_cand.p, cap, d_cnt, s));
-    CK(cudaMemcpyAsync(&cnt, d_cnt, 4, cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
+    rc = find_candidates(ctx, true, d_src, lo_bit, pay_bit, pay_end,
+                         (uint32_t)std::min<uint64_t>((pay_end - lo) / 64 + 1024, 1u << 24), cand);
+    if (rc) return rc;
     ctx->timing.kernel_launches += 1;
-    if (cnt > 0 && cnt <= cap) {
-      cand.resize(cnt);
-      CK(cudaMemcpyAsync(cand.data(), ctx->seg_cand.p, (size_t)cnt * 8, cudaMemcpyDeviceToHost, s));
-      CK(cudaStreamSynchronize(s));
-      std::sort(cand.begin(), cand.end());
+    if (!cand.empty()) {
       for (uint64_t c : cand)
         if (c >= bits.back() + min_gap && c + min_gap / 4 < pay_bit) bits.push_back(c);
       path = "blocks";
@@ -1779,12 +1766,9 @@ int dstream_run(zb200_decompress_stream *st, bool last_in, bool &progress, bool 
   const uint64_t lo_bit = st->bit0, end_bit = dec_end * 8ull, pay_bit = pay_end * 8ull;
   if (!last && pay_bit <= lo_bit) return ZB200_OK;
   ENSURE(ctx->in_stage, dec_end + 64);
-  ENSURE(ctx->counter, 128);
   const uint8_t *d_src = (const uint8_t *)ctx->in_stage.p;
   int rc = h2d_copy(ctx, (uint8_t *)ctx->in_stage.p, held, dec_end, s, true);
   if (rc) return rc;
-  uint64_t *d_resume = (uint64_t *)ctx->counter.p + 8;   // bytes 64..79
-  int *d_bad = (int *)((uint32_t *)ctx->counter.p + 12);
   // 1. boundaries
   std::vector<uint64_t> bits;
   const char *path = "serial";
@@ -1794,52 +1778,25 @@ int dstream_run(zb200_decompress_stream *st, bool last_in, bool &progress, bool 
   memset(&w, 0, sizeof(w));
   w.src = d_src;
   w.seg_limit = dec_end;
-  w.tabs = ctx->d_tabs;
-  w.data_format = ZB200_DF_DEFLATE;
-  w.seg_mode = 1;
   w.seg_win0 = st->base_out > 0;
-  std::vector<uint64_t> sl, sb;
+  std::vector<uint64_t> sl;
   std::vector<int> sst;
   std::vector<uint32_t> sk;
   uint64_t res[2] = {0, 0};
   // one decode launch over the first n segments, the last of them ending at bit `last_end`: counting with the last
   // one open, or marker symbols (every segment closed)
   auto pass = [&](size_t n, bool count, uint64_t last_end) -> int {
-    sb.resize(2 * n);
-    for (size_t i = 0; i < n; i++) {
-      sb[2 * i] = bits[i];
-      sb[2 * i + 1] = i + 1 < n ? bits[i + 1] : last_end;
-    }
-    ENSURE(ctx->seg_bits, 2 * n * 8);
-    ENSURE(ctx->seg_len, n * 8);
-    ENSURE(ctx->seg_status, n * 4);
-    ENSURE(ctx->seg_kind, n * 4);
-    ENSURE(ctx->seg_expect, n * 4);
-    CK(cudaMemcpyAsync(ctx->seg_bits.p, sb.data(), 2 * n * 8, cudaMemcpyHostToDevice, s));
-    res[0] = bits[n - 1];
-    res[1] = 0;
-    if (count) CK(cudaMemcpyAsync(d_resume, res, 16, cudaMemcpyHostToDevice, s));
-    w.seg_bits = (const uint64_t *)ctx->seg_bits.p;
+    int rc_ = seg_bounds_upload(ctx, bits.data(), n, last_end, w);
+    if (rc_) return rc_;
     w.dst = count ? nullptr : (uint8_t *)ctx->mark_scratch.p;
-    w.dst_off = (const uint64_t *)ctx->seg_dst.p;
-    w.out_len = (uint64_t *)ctx->seg_len.p;
-    w.status = (int *)ctx->seg_status.p;
-    w.expect = (uint32_t *)ctx->seg_expect.p;
-    w.kind = (uint32_t *)ctx->seg_kind.p;
-    w.counter = (uint32_t *)ctx->counter.p + 4;
-    w.n = (uint32_t)n;
     w.count_only = count ? 1 : 0;
     w.mark = count ? 0 : 1;
-    w.resume = count ? d_resume : nullptr;
-    CK(zb_launch_inflate(w, s));
-    sl.resize(n);
-    sst.resize(n);
-    sk.resize(n);
-    CK(cudaMemcpyAsync(sl.data(), ctx->seg_len.p, n * 8, cudaMemcpyDeviceToHost, s));
-    CK(cudaMemcpyAsync(sst.data(), ctx->seg_status.p, n * 4, cudaMemcpyDeviceToHost, s));
-    CK(cudaMemcpyAsync(sk.data(), ctx->seg_kind.p, n * 4, cudaMemcpyDeviceToHost, s));
-    if (count) CK(cudaMemcpyAsync(res, d_resume, 16, cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
+    if (count) {
+      res[0] = bits[n - 1];
+      res[1] = 0;
+    }
+    rc_ = seg_pass(ctx, w, n, sl, sst, sk, count ? res : nullptr);
+    if (rc_) return rc_;
     ctx->timing.kernel_launches += 1;
     return ZB200_OK;
   };
@@ -1907,27 +1864,11 @@ int dstream_run(zb200_decompress_stream *st, bool last_in, bool &progress, bool 
     const uint64_t stop = with_open ? open_stop : bits[T];
     const bool fin = with_open && open_fin;
     // 4. marker decode of segments [0, T), all closed now, into [32768 markers | output] each
-    std::vector<ZbMarkSegHost> segs(T);
-    std::vector<uint64_t> dof(T + 1);
+    std::vector<ZbMarkSegHost> segs;
+    uint32_t max_n = 0;
     const uint64_t W = st->base_out > 0 ? 32768 : 0;
-    uint64_t se = 0, de = W;
-    for (size_t i = 0; i < T; i++) {
-      se += 32768ull;
-      segs[i].scr = se;
-      segs[i].dst = de;
-      segs[i].n = (uint32_t)size[i];
-      segs[i].pad = 0;
-      dof[i] = se;
-      se += size[i];
-      de += size[i];
-    }
-    dof[T] = se;
-    ENSURE(ctx->mark_scratch, (size_t)se * 2 + 64);
-    ENSURE(ctx->mark_segs, T * sizeof(ZbMarkSegHost) + 16);
-    ENSURE(ctx->seg_dst, (T + 1) * 8);
-    CK(cudaMemcpyAsync(ctx->seg_dst.p, dof.data(), (T + 1) * 8, cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(ctx->mark_segs.p, segs.data(), T * sizeof(ZbMarkSegHost), cudaMemcpyHostToDevice, s));
-    CK(zb_launch_mark_prefill((uint16_t *)ctx->mark_scratch.p, ctx->mark_segs.p, (uint32_t)T, s));
+    rc = mark_segments(ctx, size.data(), T, W, segs, max_n);
+    if (rc) return rc;
     ctx->timing.kernel_launches += 1;
     rc = pass(T, false, fin ? lim_bit : stop);
     if (rc) return rc;
@@ -1945,19 +1886,11 @@ int dstream_run(zb200_decompress_stream *st, bool last_in, bool &progress, bool 
     ENSURE(ctx->out_stage, W + total + 64);
     uint8_t *d_out = (uint8_t *)ctx->out_stage.p;
     if (W) CK(cudaMemcpyAsync(d_out, st->win.data(), W, cudaMemcpyHostToDevice, s));
-    CK(cudaMemsetAsync(d_bad, 0, 4, s));
-    uint32_t max_n = 0;
-    for (size_t i = 0; i < T; i++) max_n = std::max(max_n, segs[i].n);
-    const uint32_t gsz = std::max<uint32_t>(1u, (uint32_t)std::ceil(std::sqrt((double)T)));
-    const size_t ngroups = (T + gsz - 1) / gsz;
-    ENSURE(ctx->mark_win, ngroups * 32768ull * 3);
-    CK(zb_launch_resolve_groups((uint16_t *)ctx->mark_scratch.p, ctx->mark_segs.p, (uint32_t)T, max_n, gsz, 0, W,
-                                (uint16_t *)ctx->mark_win.p, (uint8_t *)ctx->mark_win.p + ngroups * 65536ull, d_out,
-                                d_bad, s));
-    ctx->timing.kernel_launches += 4;
+    CK(cudaMemsetAsync(&counters(ctx)->bad, 0, 4, s));
     int bad = 0;
-    CK(cudaMemcpyAsync(&bad, d_bad, 4, cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
+    rc = resolve_window(ctx, T, max_n, 0, W, d_out, &bad);
+    if (rc) return rc;
+    ctx->timing.kernel_launches += 4;
     if (bad) {
       if (S == 1) return ZB200_ERR_UNCOMPRESS;
       bits.resize(1);
@@ -2106,7 +2039,6 @@ int uncompress_device_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint64_
   ENSURE(ctx->status, n * sizeof(int));
   ENSURE(ctx->expect, n * sizeof(uint32_t));
   ENSURE(ctx->kind, n * sizeof(uint32_t));
-  ENSURE(ctx->counter, 64);
   if (crcs) ENSURE(ctx->ck_out, n * sizeof(uint32_t));
   cudaStream_t s = ctx->stream;
   CK(cudaMemcpyAsync(ctx->src_off.p, src_offsets, (n + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, s));
@@ -2122,7 +2054,7 @@ int uncompress_device_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint64_
   w.status = (int *)ctx->status.p;
   w.expect = (uint32_t *)ctx->expect.p;
   w.kind = (uint32_t *)ctx->kind.p;
-  w.counter = (uint32_t *)ctx->counter.p;
+  w.counter = &counters(ctx)->member;
   w.tabs = ctx->d_tabs;
   w.n = (uint32_t)n;
   w.data_format = data_format;
@@ -2264,7 +2196,8 @@ int uncompress_host_pipelined(zb200_ctx *ctx, const uint8_t *h_src, const std::v
   ENSURE(ctx->expect, n * sizeof(uint32_t));
   ENSURE(ctx->kind, n * sizeof(uint32_t));
   ENSURE(ctx->order, n * sizeof(uint32_t));
-  ENSURE(ctx->counter, (ng + 16) * sizeof(uint32_t));
+  ENSURE(ctx->counter, sizeof(ZbCounters) + ng * sizeof(uint32_t));
+  uint32_t *group_counter = (uint32_t *)(counters(ctx) + 1);
   ENSURE(ctx->ck_pieces, pieces.size() * sizeof(ZbPiece));
   ENSURE(ctx->ck_first, first.size() * sizeof(uint32_t));
   ENSURE(ctx->ck_piece_out, pieces.size() * sizeof(ZbChunkCheck));
@@ -2319,7 +2252,7 @@ int uncompress_host_pipelined(zb200_ctx *ctx, const uint8_t *h_src, const std::v
     w.status = (int *)ctx->status.p;
     w.expect = (uint32_t *)ctx->expect.p;
     w.kind = (uint32_t *)ctx->kind.p;
-    w.counter = (uint32_t *)ctx->counter.p + 16;
+    w.counter = group_counter;
     w.tabs = ctx->d_tabs;
     w.n = (uint32_t)n;
     w.data_format = data_format;
@@ -2422,7 +2355,7 @@ int uncompress_host_pipelined(zb200_ctx *ctx, const uint8_t *h_src, const std::v
     w.status = (int *)ctx->status.p + m0;
     w.expect = (uint32_t *)ctx->expect.p + m0;
     w.kind = (uint32_t *)ctx->kind.p + m0;
-    w.counter = (uint32_t *)ctx->counter.p + 16 + gi;
+    w.counter = group_counter + gi;
     w.tabs = ctx->d_tabs;
     w.n = (uint32_t)nm;
     w.data_format = data_format;
@@ -2636,6 +2569,7 @@ int zb200_init(int device, zb200_ctx **out) {
   if (ok) ok = cudaStreamCreateWithFlags(&ctx->d2h_stream, cudaStreamNonBlocking) == cudaSuccess;
   for (int i = 0; ok && i < 10; i++) ok = cudaEventCreate(&ctx->ev[i]) == cudaSuccess;
   if (ok) ok = cudaMalloc((void **)&ctx->d_tabs, sizeof(ZbCrcTables)) == cudaSuccess;
+  if (ok) ok = ensure(ctx, ctx->counter, sizeof(ZbCounters)) == ZB200_OK;
   // kernel attributes are per device (and cheap to set again): every ctx sets them for its own
   if (ok) ok = zb_setup_deflate_attrs() == cudaSuccess && zb_setup_inflate_attrs() == cudaSuccess;
   if (ok) {
@@ -3638,59 +3572,6 @@ int index_gather(zb200_ctx *ctx, const uint8_t *d_src, const std::vector<uint64_
   return ZB200_OK;
 }
 
-// One counting pass over the segments bits[i] .. bits[i + 1] (the last one to end_bit) of the member staged in
-// in_stage; with `base` the recorder stores access points into rec [2 * nrec].
-int index_count(zb200_ctx *ctx, const std::vector<uint64_t> &bits, uint64_t end_bit, uint64_t len, const uint64_t *base,
-                uint64_t *d_rec, uint32_t nrec, std::vector<uint64_t> &sl, std::vector<int> &sst, std::vector<uint32_t> &sk) {
-  cudaStream_t s = ctx->stream;
-  const size_t S = bits.size();
-  std::vector<uint64_t> sb(2 * S);
-  for (size_t i = 0; i < S; i++) {
-    sb[2 * i] = bits[i];
-    sb[2 * i + 1] = i + 1 < S ? bits[i + 1] : end_bit;
-  }
-  ENSURE(ctx->seg_bits, 2 * S * 8);
-  ENSURE(ctx->seg_dst, (S + 1) * 8);
-  ENSURE(ctx->seg_len, S * 8);
-  ENSURE(ctx->seg_status, S * 4);
-  ENSURE(ctx->seg_kind, S * 4);
-  ENSURE(ctx->seg_expect, S * 4);
-  ENSURE(ctx->counter, 128);
-  CK(cudaMemcpyAsync(ctx->seg_bits.p, sb.data(), 2 * S * 8, cudaMemcpyHostToDevice, s));
-  if (base) CK(cudaMemcpyAsync(ctx->seg_dst.p, base, (S + 1) * 8, cudaMemcpyHostToDevice, s));
-  ZbInflateWork w;
-  memset(&w, 0, sizeof(w));
-  w.src = (const uint8_t *)ctx->in_stage.p;
-  w.seg_bits = (const uint64_t *)ctx->seg_bits.p;
-  w.seg_limit = len;
-  w.dst_off = (const uint64_t *)ctx->seg_dst.p;
-  w.out_len = (uint64_t *)ctx->seg_len.p;
-  w.status = (int *)ctx->seg_status.p;
-  w.expect = (uint32_t *)ctx->seg_expect.p;
-  w.kind = (uint32_t *)ctx->seg_kind.p;
-  w.counter = (uint32_t *)ctx->counter.p + 4;
-  w.tabs = ctx->d_tabs;
-  w.n = (uint32_t)S;
-  w.data_format = ZB200_DF_DEFLATE;
-  w.seg_mode = 1;
-  w.count_only = 1;
-  if (base) {
-    w.rec = d_rec;
-    w.rec_base = (const uint64_t *)ctx->seg_dst.p;
-    w.nrec = nrec;
-  }
-  CK(zb_launch_inflate(w, s));
-  sl.resize(S);
-  sst.resize(S);
-  sk.resize(S);
-  CK(cudaMemcpyAsync(sl.data(), ctx->seg_len.p, S * 8, cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(sst.data(), ctx->seg_status.p, S * 4, cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(sk.data(), ctx->seg_kind.p, S * 4, cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
-  ctx->timing.kernel_launches += 1;
-  return ZB200_OK;
-}
-
 int index_build_locked(zb200_ctx *ctx, const uint8_t *src, size_t len, int data_format, uint64_t span, zb200_index **out) {
   cudaStream_t s = ctx->stream;
   uint64_t size = 0;
@@ -3727,12 +3608,21 @@ int index_build_locked(zb200_ctx *ctx, const uint8_t *src, size_t len, int data_
     }
     return t == size;
   };
+  // counting passes over the segments bits[i] .. bits[i + 1] (the last one to the member's end) staged in in_stage
+  ZbInflateWork w;
+  memset(&w, 0, sizeof(w));
+  w.src = (const uint8_t *)ctx->in_stage.p;
+  w.seg_limit = len;
+  w.count_only = 1;
   for (;;) {
     const size_t S = bits.size();
     base.assign(S + 1, 0);
+    rc = seg_bounds_upload(ctx, bits.data(), S, len * 8ull, w);
+    if (rc) return rc;
     if (S > 1) {   // the sizes first: every segment's output offset
-      rc = index_count(ctx, bits, len * 8ull, len, nullptr, nullptr, 0, sl, sst, sk);
+      rc = seg_pass(ctx, w, S, sl, sst, sk);
       if (rc) return rc;
+      ctx->timing.kernel_launches += 1;
       if (!regular()) {
         bits.resize(1);
         continue;
@@ -3741,9 +3631,17 @@ int index_build_locked(zb200_ctx *ctx, const uint8_t *src, size_t len, int data_
     } else {
       base[1] = size;
     }
+    // then the recorder, with every segment's output offset in the member as rec_base
+    ENSURE(ctx->seg_dst, (S + 1) * 8);
+    CK(cudaMemcpyAsync(ctx->seg_dst.p, base.data(), (S + 1) * 8, cudaMemcpyHostToDevice, s));
     CK(cudaMemsetAsync(d_rec, 0xff, (size_t)nrec * 16, s));
-    rc = index_count(ctx, bits, len * 8ull, len, base.data(), d_rec, nrec, sl, sst, sk);
+    ZbInflateWork r = w;
+    r.rec = d_rec;
+    r.rec_base = (const uint64_t *)ctx->seg_dst.p;
+    r.nrec = nrec;
+    rc = seg_pass(ctx, r, S, sl, sst, sk);
     if (rc) return rc;
+    ctx->timing.kernel_launches += 1;
     if (regular()) break;
     if (S == 1) return ZB200_ERR_UNCOMPRESS;   // a member uncompress accepts counts the same
     bits.resize(1);
@@ -3866,53 +3764,30 @@ int index_extract_group(zb200_ctx *ctx, const zb200_index *idx, const uint8_t *s
   int rc = h2d_copy(ctx, (uint8_t *)ctx->in_stage.p, stage.data(), stage.size(), s, true);
   if (rc) return rc;
   ctx->timing.h2d_bytes += stage.size();
-  ENSURE(ctx->mark_scratch, (size_t)se * 2 + 64);
-  ENSURE(ctx->mark_segs, R * sizeof(ZbMarkSegHost) + 16);
   const size_t T2 = 2 * T;   // every segment is followed by its empty gap segment
-  ENSURE(ctx->seg_bits, T2 * 16);
-  ENSURE(ctx->seg_dst, (T2 + 1) * 8);
-  ENSURE(ctx->seg_len, T2 * 8);
-  ENSURE(ctx->seg_status, T2 * 4);
-  ENSURE(ctx->seg_kind, T2 * 4);
-  ENSURE(ctx->seg_expect, T2 * 4);
-  ENSURE(ctx->counter, 128);
   ENSURE(ctx->out_stage, (size_t)de + 64);
-  CK(cudaMemcpyAsync(ctx->mark_segs.p, segs.data(), R * sizeof(ZbMarkSegHost), cudaMemcpyHostToDevice, s));
-  CK(cudaMemcpyAsync(ctx->seg_bits.p, sb.data(), T2 * 16, cudaMemcpyHostToDevice, s));
-  CK(cudaMemcpyAsync(ctx->seg_dst.p, dof.data(), (T2 + 1) * 8, cudaMemcpyHostToDevice, s));
-  ctx->timing.h2d_bytes += R * sizeof(ZbMarkSegHost) + T2 * 24 + 8;
-  // 2. markers, then the windows as byte symbols, then one marker decode of every segment of every chain
-  CK(zb_launch_mark_prefill((uint16_t *)ctx->mark_scratch.p, ctx->mark_segs.p, (uint32_t)R, s));
-  ctx->timing.kernel_launches += 1;
-  rc = index_gather(ctx, (const uint8_t *)ctx->in_stage.p, wranges, true, ctx->mark_scratch.p);
-  if (rc) return rc;
   ZbInflateWork w;
   memset(&w, 0, sizeof(w));
   w.src = (const uint8_t *)ctx->in_stage.p;
-  w.seg_bits = (const uint64_t *)ctx->seg_bits.p;
   w.seg_limit = stage.size();
   w.seg_win0 = ch[c0].p0 > 0;   // a chain from point 0 has no window: a distance before the member start is an error
-  w.dst = (uint8_t *)ctx->mark_scratch.p;
-  w.dst_off = (const uint64_t *)ctx->seg_dst.p;
-  w.out_len = (uint64_t *)ctx->seg_len.p;
-  w.status = (int *)ctx->seg_status.p;
-  w.expect = (uint32_t *)ctx->seg_expect.p;
-  w.kind = (uint32_t *)ctx->seg_kind.p;
-  w.counter = (uint32_t *)ctx->counter.p + 4;
-  w.tabs = ctx->d_tabs;
-  w.n = (uint32_t)T2;
-  w.data_format = ZB200_DF_DEFLATE;
-  w.seg_mode = 1;
-  w.mark = 1;
-  CK(zb_launch_inflate(w, s));
+  rc = seg_bits_upload(ctx, sb, w);
+  if (rc) return rc;
+  // 2. markers, then the windows as byte symbols, then one marker decode of every segment of every chain
+  rc = mark_upload(ctx, segs, dof);
+  if (rc) return rc;
+  ctx->timing.h2d_bytes += R * sizeof(ZbMarkSegHost) + T2 * 24 + 8;
   ctx->timing.kernel_launches += 1;
-  std::vector<uint64_t> sl(T2);
-  std::vector<int> sst(T2);
-  std::vector<uint32_t> sk(T2);
-  CK(cudaMemcpyAsync(sl.data(), ctx->seg_len.p, T2 * 8, cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(sst.data(), ctx->seg_status.p, T2 * 4, cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(sk.data(), ctx->seg_kind.p, T2 * 4, cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
+  rc = index_gather(ctx, (const uint8_t *)ctx->in_stage.p, wranges, true, ctx->mark_scratch.p);
+  if (rc) return rc;
+  w.dst = (uint8_t *)ctx->mark_scratch.p;
+  w.mark = 1;
+  std::vector<uint64_t> sl;
+  std::vector<int> sst;
+  std::vector<uint32_t> sk;
+  rc = seg_pass(ctx, w, T2, sl, sst, sk);
+  if (rc) return rc;
+  ctx->timing.kernel_launches += 1;
   for (size_t c = c0; c < c1; c++) chain_st[c] = ZB200_OK;
   bool any_failed = false;
   for (size_t t = 0; t < T; t++) {
@@ -3932,18 +3807,11 @@ int index_extract_group(zb200_ctx *ctx, const zb200_index *idx, const uint8_t *s
   // every chain resolves against its own window.  Only the first chain of a group can reach before the member
   // start, and only the chain from point 0 starts a group without a window; it decodes without one, so a marker
   // before the start (`bad`) cannot be produced by a segment that decoded.
-  int *d_bad = (int *)((uint32_t *)ctx->counter.p + 12);
-  CK(cudaMemsetAsync(d_bad, 0, 4, s));
-  const uint32_t gsz = std::max<uint32_t>(1u, (uint32_t)std::ceil(std::sqrt((double)R)));
-  const size_t ngroups = (R + gsz - 1) / gsz;
-  ENSURE(ctx->mark_win, ngroups * 32768ull * 3);
-  CK(zb_launch_resolve_groups((uint16_t *)ctx->mark_scratch.p, ctx->mark_segs.p, (uint32_t)R, max_n, gsz, 0, 0,
-                              (uint16_t *)ctx->mark_win.p, (uint8_t *)ctx->mark_win.p + ngroups * 65536ull,
-                              (uint8_t *)ctx->out_stage.p, d_bad, s));
-  ctx->timing.kernel_launches += 4;
+  CK(cudaMemsetAsync(&counters(ctx)->bad, 0, 4, s));
   int bad = 0;
-  CK(cudaMemcpyAsync(&bad, d_bad, 4, cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
+  rc = resolve_window(ctx, R, max_n, 0, 0, (uint8_t *)ctx->out_stage.p, &bad);
+  if (rc) return rc;
+  ctx->timing.kernel_launches += 4;
   // 4. every decoded interval against its CRC-32
   std::vector<uint64_t> coff(R + 1);
   for (size_t r = 0; r < R; r++) coff[r] = segs[r].dst;
