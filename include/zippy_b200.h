@@ -353,6 +353,43 @@ int zb200_compress_stream_begin_index(zb200_ctx *ctx, int level, int data_format
                                       zb200_compress_stream **out);
 int zb200_compress_stream_index(zb200_compress_stream *st, zb200_index **out);
 
+/* ---- compression strategies: zlib's `strategy` (deflateInit2, zlib.compressobj) ----
+ * The values are zlib's, so Z_FILTERED, Z_HUFFMAN_ONLY, Z_RLE and Z_FIXED pass straight through; any other value
+ * fails with ZB200_ERR_ARG (and leaves statuses alone, as an invalid level does).  A strategy changes the compressed
+ * size, never what the member decodes to: every member is an ordinary stream for any inflater.  Strategy 0 is
+ * exactly the calls without _strategy.  The parse is chosen in zlib's order:
+ *  - level 0: stored blocks, whatever the strategy;
+ *  - level -2, or HUFFMAN_ONLY at any other level: literals only (level -2's bytes);
+ *  - RLE at levels -1 and 1..9: a run-length parse, the same bytes at every level.  Each chunk is cut into 4 KiB
+ *    pieces; walking left to right, position p (not its chunk's first byte) starts a match of distance 1 when the
+ *    byte before it repeats at p, p + 1 and p + 2 inside p's piece, as long as the run goes on (at most 258 and
+ *    never past the piece end); otherwise p is a literal.  That is zlib's deflate_rle with no history across a
+ *    64 KiB chunk start and no match across a piece end.  There is no history, so a sync and a full flush of a
+ *    stream write the same bytes;
+ *  - FILTERED at levels -1 and 2..9: the level's parse, with every match shorter than 6 taken as no match before
+ *    the one-step lazy rule (zlib deflate_slow's match_length <= 5 rule).  Level 1 ignores it, as zlib's fast
+ *    levels do;
+ *  - DEFAULT and FIXED: the level's parse.
+ * Each chunk's block is the smallest of stored, fixed and dynamic, except under FIXED: the smaller of stored and
+ * fixed, never dynamic.  Framing, chunking and the zlib header (78 01) do not change, and zb200_compress_bound covers
+ * every strategy.  Not combined with dictionaries, compress-time indexes, zb200_compress_batch_h2d or multi-GPU.
+ * The _strategy calls take the arguments of the calls without it, plus `strategy` after `level`. */
+enum {
+  ZB200_STRATEGY_DEFAULT = 0,
+  ZB200_STRATEGY_FILTERED = 1,
+  ZB200_STRATEGY_HUFFMAN_ONLY = 2,
+  ZB200_STRATEGY_RLE = 3,
+  ZB200_STRATEGY_FIXED = 4
+};
+int zb200_compress_batch_strategy(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n,
+                                  int level, int strategy, int data_format, const uint8_t *fname_lens,
+                                  uint8_t *dst_base, size_t dst_cap, uint64_t *dst_offsets, int *statuses);
+int zb200_compress_batch_device_strategy(zb200_ctx *ctx, const uint8_t *d_src, const uint64_t *src_offsets, size_t n,
+                                         int level, int strategy, int data_format, const uint8_t *fname_lens,
+                                         uint8_t *d_dst, size_t dst_cap, uint64_t *dst_offsets, int *statuses);
+int zb200_compress_stream_begin_strategy(zb200_ctx *ctx, int level, int strategy, int data_format, int fname_len,
+                                         zb200_compress_stream **out);
+
 /* ---- device-resident variants (pointers prefixed d_ are device memory on ctx's device;
  * offsets / statuses / sizes stay host arrays).  Used when the data already lives in HBM
  * (bench.py's `value`) and by the multi-GPU sharded path.  The call returns after the

@@ -24,6 +24,14 @@ struct ZippyError : std::runtime_error {  // common.nim:2
 
 enum CompressedDataFormat { dfDetect = 0, dfZlib = 1, dfGzip = 2, dfDeflate = 3 };  // common.nim:4-5
 constexpr int NoCompression = 0, BestSpeed = 1, BestCompression = 9, DefaultCompression = -1, HuffmanOnly = -2;
+// zlib's compression strategies, with zlib's values (include/zippy_b200.h "compression strategies")
+enum Strategy {
+  StrategyDefault = ZB200_STRATEGY_DEFAULT,
+  StrategyFiltered = ZB200_STRATEGY_FILTERED,
+  StrategyHuffmanOnly = ZB200_STRATEGY_HUFFMAN_ONLY,
+  StrategyRle = ZB200_STRATEGY_RLE,
+  StrategyFixed = ZB200_STRATEGY_FIXED
+};
 
 namespace detail {
 inline void check(int rc) {
@@ -154,6 +162,25 @@ inline std::string compress(const void *srcp, size_t len, int level, CompressedD
 inline std::string compress(const std::string &src, int level, CompressedDataFormat dataFormat,
                             const std::string &dictionary) {
   return compress(src.data(), src.size(), level, dataFormat, dictionary);
+}
+
+// Under a compression strategy: one member of zb200_compress_batch_strategy (gzip draws its FNAME length at
+// random, as compress() does).  StrategyDefault writes compress()'s bytes.
+inline std::string compress(const void *srcp, size_t len, int level, CompressedDataFormat dataFormat, Strategy strategy) {
+  const uint64_t offs[2] = {0, len};
+  uint64_t out_offs[2] = {0, 0};
+  int st = 0;
+  const uint8_t fl = dataFormat == dfGzip ? (uint8_t)(std::random_device()() % 26) : 0;
+  std::string result(zb200_compress_bound(len, dataFormat) + 64, '\0');
+  uint8_t dummy = 0;
+  detail::check(zb200_compress_batch_strategy(detail::ctx(), len ? static_cast<const uint8_t *>(srcp) : &dummy, offs, 1,
+                                              level, strategy, dataFormat, &fl, reinterpret_cast<uint8_t *>(&result[0]),
+                                              result.size(), out_offs, &st));
+  result.resize(out_offs[1]);
+  return result;
+}
+inline std::string compress(const std::string &src, int level, CompressedDataFormat dataFormat, Strategy strategy) {
+  return compress(src.data(), src.size(), level, dataFormat, strategy);
 }
 
 // gzip.nim:3-88
@@ -299,6 +326,11 @@ class CompressStream {
   CompressStream(int level, CompressedDataFormat dataFormat, const std::string &dictionary, zb200_ctx *ctx = nullptr) {
     detail::check(zb200_compress_stream_begin_dict(ctx ? ctx : detail::ctx(), level, dataFormat, detail::u8(dictionary),
                                                    dictionary.size(), &st_));
+  }
+  // under a compression strategy (zb200_compress_stream_begin_strategy)
+  CompressStream(int level, CompressedDataFormat dataFormat, Strategy strategy, int fnameLen = -1, zb200_ctx *ctx = nullptr) {
+    if (fnameLen < 0) fnameLen = dataFormat == dfGzip ? (int)(std::random_device()() % 26) : 0;
+    detail::check(zb200_compress_stream_begin_strategy(ctx ? ctx : detail::ctx(), level, strategy, dataFormat, fnameLen, &st_));
   }
   // that also writes the member's index (zb200_compress_stream_begin_index): index() after finish()
   CompressStream(int level, CompressedDataFormat dataFormat, int fnameLen, uint64_t indexSpan, zb200_ctx *ctx = nullptr)

@@ -562,3 +562,36 @@ proc newCompressStream*(level: int, dataFormat: CompressedDataFormat, fnameLen: 
 
 proc index*(s: CompressStream): Index {.raises: [ZippyError].} =
   check zb200_compress_stream_index(s.st, result.idx.addr)
+
+# ---- compression strategies (zlib's `strategy`, with zlib's values; include/zippy_b200.h "compression
+# strategies"): a strategy changes the compressed size, never what a member decodes to ----
+type Strategy* = enum
+  StrategyDefault = 0, StrategyFiltered = 1, StrategyHuffmanOnly = 2, StrategyRle = 3, StrategyFixed = 4
+
+proc zb200_compress_batch_strategy(ctx: Zb200Ctx, srcBase: pointer, srcOffsets: ptr uint64, n: csize_t,
+                                   level, strategy, dataFormat: cint, fnameLens: pointer, dstBase: pointer,
+                                   dstCap: csize_t, dstOffsets: ptr uint64,
+                                   statuses: ptr cint): cint {.importc, cdecl, dynlib: lib.}
+proc zb200_compress_stream_begin_strategy(ctx: Zb200Ctx, level, strategy, dataFormat, fnameLen: cint,
+                                          st: ptr Zb200CompressStream): cint {.importc, cdecl, dynlib: lib.}
+
+proc compress*(src: string, level: int, dataFormat: CompressedDataFormat,
+               strategy: Strategy): string {.raises: [ZippyError].} =
+  ## one member of zb200_compress_batch_strategy; gzip draws its FNAME length at random, as compress does
+  var
+    offs = [0'u64, src.len.uint64]
+    outOffs = [0'u64, 0'u64]
+    fl = randomFnameLen(dataFormat).uint8
+    dummy: uint8
+  result = newString(zb200_compress_bound(src.len.csize_t, dataFormat.cint).int + 64)
+  check zb200_compress_batch_strategy(getCtx(), (if src.len > 0: src[0].unsafeAddr else: dummy.addr),
+                                      offs[0].addr, 1, level.cint, strategy.cint, dataFormat.cint, fl.addr,
+                                      result[0].addr, result.len.csize_t, outOffs[0].addr, nil)
+  result.setLen(outOffs[1].int)
+
+proc newCompressStream*(level: int, dataFormat: CompressedDataFormat, strategy: Strategy,
+                        fnameLen = -1): CompressStream {.raises: [ZippyError].} =
+  ## a stream under a compression strategy: zb200_compress_stream_begin_strategy
+  let k = if fnameLen < 0: randomFnameLen(dataFormat) else: fnameLen
+  check zb200_compress_stream_begin_strategy(getCtx(), level.cint, strategy.cint, dataFormat.cint, k.cint,
+                                             result.st.addr)

@@ -27,6 +27,8 @@ dfDetect, dfZlib, dfGzip, dfDeflate = 0, 1, 2, 3                       # common.
 NoCompression, BestSpeed, BestCompression = 0, 1, 9                    # common.nim:7-12
 DefaultCompression, HuffmanOnly = -1, -2
 SyncFlush, FullFlush = 2, 3                                            # zlib's Z_SYNC_FLUSH / Z_FULL_FLUSH
+# zlib's Z_DEFAULT_STRATEGY, Z_FILTERED, Z_HUFFMAN_ONLY, Z_RLE, Z_FIXED (zippy_b200.h, "compression strategies")
+StrategyDefault, StrategyFiltered, StrategyHuffmanOnly, StrategyRle, StrategyFixed = 0, 1, 2, 3, 4
 
 __all__ = ["compress", "uncompress", "crc32", "adler32", "deflate", "inflate", "compress_batch", "uncompress_batch",
            "uncompressed_sizes", "checksum_batch", "ZippyError", "Context", "CompressStream", "DecompressStream",
@@ -34,7 +36,8 @@ __all__ = ["compress", "uncompress", "crc32", "adler32", "deflate", "inflate", "
            "MultiGpu", "Index", "dfDetect",
            "dfZlib", "dfGzip",
            "dfDeflate", "NoCompression", "BestSpeed", "BestCompression", "DefaultCompression", "HuffmanOnly",
-           "SyncFlush", "FullFlush"]
+           "SyncFlush", "FullFlush", "StrategyDefault", "StrategyFiltered", "StrategyHuffmanOnly", "StrategyRle",
+           "StrategyFixed"]
 
 
 class ZippyError(Exception):
@@ -64,6 +67,17 @@ def _dict(dictionary):
     without a dictionary, as zlib writes no FDICT for an empty zdict."""
     d = None if dictionary is None else _as_u8(dictionary)
     return d if d is not None and d.size else None
+
+
+def _strategy_alone(strategy, dictionary=None, index_span=None):
+    """True for a strategy other than the default; such a strategy takes no dictionary and no compress-time index."""
+    if strategy == StrategyDefault:
+        return False
+    if _dict(dictionary) is not None:
+        raise ZippyError(22, "a compression strategy is not combined with a dictionary")
+    if index_span is not None:
+        raise ZippyError(22, "a compression strategy is not combined with a compress-time index")
+    return True
 
 
 def _pack(items):
@@ -108,8 +122,9 @@ class Context:
 
     # ---- batches over host buffers -------------------------------------------------
     def compress_batch(self, base, offsets, level=DefaultCompression, dataFormat=dfGzip, fname_lens=None,
-                       dictionary=None, index_span=None):
+                       dictionary=None, index_span=None, strategy=StrategyDefault):
         """-> (out uint8 array, out_offsets uint64[n+1]).  fname_lens: per-input gzip FNAME letters (0..25).
+        strategy: zlib's compression strategy (Strategy*; zb200_compress_batch_strategy; no dictionary or index).
         dictionary: a preset dictionary shared by every input (zlib / raw only; zb200_compress_batch_dict).
         index_span: also write each member's Index with this span (zb200_compress_batch_index; no dictionary):
         -> (out, out_offsets, list of Index)."""
@@ -123,6 +138,14 @@ class Context:
         out_offs = np.zeros(n + 1, dtype=np.uint64)
         st = np.zeros(max(n, 1), dtype=np.int32)
         d = _dict(dictionary)
+        if _strategy_alone(strategy, d, index_span):
+            fl = np.ascontiguousarray(fname_lens, dtype=np.uint8) if fname_lens is not None else None
+            _check(self._h, L.zb200_compress_batch_strategy(self._h, base.ctypes.data, offsets.ctypes.data, n, level,
+                                                             strategy, dataFormat,
+                                                             fl.ctypes.data if fl is not None else None,
+                                                             out.ctypes.data, out.size, out_offs.ctypes.data,
+                                                             st.ctypes.data))
+            return out[:int(out_offs[n])], out_offs
         if index_span is not None:
             if d is not None:
                 raise ZippyError(22, "a compress-time index is not written with a dictionary")
@@ -263,14 +286,20 @@ class Context:
 
     # ---- device-resident batches (raw device pointers; e.g. torch tensor .data_ptr()) ----
     def compress_batch_device(self, d_src, offsets, level, dataFormat, d_dst, dst_cap, fname_lens=None,
-                              index_span=None):
+                              index_span=None, strategy=StrategyDefault):
         """-> out_offsets; with index_span also each member's Index (zb200_compress_batch_device_index):
-        -> (out_offsets, list of Index)."""
+        -> (out_offsets, list of Index).  strategy: zlib's compression strategy (no index)."""
         L = _native.lib()
         offsets = np.ascontiguousarray(offsets, dtype=np.uint64)
         n = len(offsets) - 1
         out_offs = np.zeros(n + 1, dtype=np.uint64)
         fl = np.ascontiguousarray(fname_lens, dtype=np.uint8) if fname_lens is not None else None
+        if _strategy_alone(strategy, None, index_span):
+            _check(self._h, L.zb200_compress_batch_device_strategy(self._h, d_src, offsets.ctypes.data, n, level,
+                                                                    strategy, dataFormat,
+                                                                    fl.ctypes.data if fl is not None else None, d_dst,
+                                                                    dst_cap, out_offs.ctypes.data, None))
+            return out_offs
         if index_span is not None:
             hs = (ctypes.c_void_p * max(n, 1))()
             _check(self._h, L.zb200_compress_batch_device_index(self._h, d_src, offsets.ctypes.data, n, level,
@@ -336,9 +365,12 @@ class Context:
         return {f: getattr(t, f) for f, _ in t._fields_}
 
     # ---- the single-input seam (deflate.nim:207, inflate.nim:268, crc.nim:53, adler32.nim:6) ----
-    def deflate(self, src, level=DefaultCompression):
+    def deflate(self, src, level=DefaultCompression, strategy=StrategyDefault):
         L = _native.lib()
         src = _as_u8(src)
+        if strategy != StrategyDefault:   # one raw DEFLATE member of the batch call
+            out, _ = self.compress_batch(src, [0, src.size], level, dfDeflate, strategy=strategy)
+            return out.tobytes()
         cap = L.zb200_deflate_bound(src.size)
         out = np.empty(cap + 8, dtype=np.uint8)
         n = ctypes.c_size_t(0)
@@ -389,12 +421,19 @@ class CompressStream:
     length is drawn at random, as compress() does (zippy.nim:28-42)."""
 
     def __init__(self, level=DefaultCompression, dataFormat=dfGzip, fname_len=None, ctx=None, dictionary=None,
-                 index_span=None):
+                 index_span=None, strategy=StrategyDefault):
         """index_span: also write the member's Index with this span (zb200_compress_stream_begin_index; no
-        dictionary), returned by index() after finish()."""
+        dictionary), returned by index() after finish().  strategy: zlib's compression strategy
+        (zb200_compress_stream_begin_strategy; no dictionary or index)."""
         self._ctx = ctx if ctx is not None else default_context()
         self._h = ctypes.c_void_p()
         d = _dict(dictionary)
+        if _strategy_alone(strategy, d, index_span):
+            if fname_len is None:
+                fname_len = os.urandom(1)[0] % 26 if dataFormat == dfGzip else 0
+            _check(self._ctx._h, _native.lib().zb200_compress_stream_begin_strategy(
+                self._ctx._h, level, strategy, dataFormat, fname_len, ctypes.byref(self._h)))
+            return
         if index_span is not None:
             if d is not None:
                 raise ZippyError(22, "a compress-time index is not written with a dictionary")
@@ -714,8 +753,9 @@ def default_context():
 
 
 # ---- the reference's public procs ------------------------------------------------------
-def compress(src, level=DefaultCompression, dataFormat=dfGzip, dictionary=None):
-    """zippy.compress (zippy.nim:11-98).  dictionary: a preset dictionary (zlib / raw only; zlib's zdict)."""
+def compress(src, level=DefaultCompression, dataFormat=dfGzip, dictionary=None, strategy=StrategyDefault):
+    """zippy.compress (zippy.nim:11-98).  dictionary: a preset dictionary (zlib / raw only; zlib's zdict).
+    strategy: zlib's compression strategy (Strategy*), not with a dictionary."""
     if level < -2 or level > 9:
         raise ZippyError(1, "Invalid compression level %d" % level)          # deflate.nim:208-209
     if dataFormat not in (dfGzip, dfZlib, dfDeflate):
@@ -724,7 +764,8 @@ def compress(src, level=DefaultCompression, dataFormat=dfGzip, dictionary=None):
     if dataFormat == dfGzip and _dict(dictionary) is None:
         fl = [os.urandom(1)[0] % 26]                                         # zippy.nim:28-42
     base, offs = _pack([src])
-    out, _ = default_context().compress_batch(base, offs, level, dataFormat, fl, dictionary=dictionary)
+    out, _ = default_context().compress_batch(base, offs, level, dataFormat, fl, dictionary=dictionary,
+                                              strategy=strategy)
     return out.tobytes()
 
 
@@ -758,18 +799,20 @@ def adler32(src):
     return default_context().adler32(src)
 
 
-def deflate(src, level=DefaultCompression):
-    return default_context().deflate(src, level)
+def deflate(src, level=DefaultCompression, strategy=StrategyDefault):
+    return default_context().deflate(src, level, strategy)
 
 
 def inflate(src, pos=0):
     return default_context().inflate(src, pos)
 
 
-def compress_batch(items, level=DefaultCompression, dataFormat=dfGzip, fname_lens=None, dictionary=None):
+def compress_batch(items, level=DefaultCompression, dataFormat=dfGzip, fname_lens=None, dictionary=None,
+                   strategy=StrategyDefault):
     """list of bytes -> list of bytes (one zippy.compress per item, one GPU launch sequence)."""
     base, offs = _pack(items)
-    out, oo = default_context().compress_batch(base, offs, level, dataFormat, fname_lens, dictionary=dictionary)
+    out, oo = default_context().compress_batch(base, offs, level, dataFormat, fname_lens, dictionary=dictionary,
+                                               strategy=strategy)
     return [out[int(oo[i]):int(oo[i + 1])].tobytes() for i in range(len(items))]
 
 

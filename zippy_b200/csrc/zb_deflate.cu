@@ -222,7 +222,10 @@ extern "C" int zb200_lz1_stage_clocks(unsigned long long *out) {
 #define LZ_CLK_PUBLISH()
 #endif
 
-// MODE 1: single-probe hash matcher (level 1); 0: literals only (levels 0, -2).
+// MODE 1: single-probe hash matcher (level 1); 0: literals only (levels 0, -2); 2: the run-length parse
+// (ZB200_STRATEGY_RLE): a position is a match of distance 1 when it is not the chunk's first byte and the run of
+// bytes equal to the byte before it, cut at the piece end and at 258, is at least 3 long -- zlib's deflate_rle with
+// no history across chunk starts and no match across a piece end.  It probes no table.
 // CK: the chunk checksums k_member_check reads for the batch's format (ZB_CK_CRC for gzip, ZB_CK_ADLER for
 // zlib, 0 for raw DEFLATE); the other fields of chk are left 0.
 template <int MODE, int CK>
@@ -355,6 +358,21 @@ __global__ void __launch_bounds__(LZ_THREADS, 3)
         const uint32_t nvalid = min(32u, b1 - wb);
         const uint32_t cur = entry - wb;
         uint32_t m = 0, c = 0, lit = 0;
+        if (MODE == 2) {
+          // run lengths from one ballot per 32 positions: bit i of eq says byte wb + i equals the byte before it (never
+          // at the chunk's first byte); the run at p is the count of consecutive set bits from p, seen 32 bytes ahead
+          const uint32_t x = doff + p;
+          lit = data[x];
+          const uint32_t eq0 = __ballot_sync(ZB_FULL, p != 0u && lit == data[x - 1u]);
+          const uint32_t eq1 = __ballot_sync(ZB_FULL, data[x + 32u] == data[x + 31u]);
+          const uint32_t ahead = __funnelshift_r(eq0, eq1, (uint32_t)lane);  // bits p .. p + 31
+          const uint32_t run = ahead == ~0u ? (uint32_t)LZ_LANE_CAP : (uint32_t)(__ffs((int)~ahead) - 1);
+          // a run that fills the lane cap is at least that long: lz_select extends it (distance 1) and cuts it there
+          const uint32_t limit = p < b1 ? b1 - p : 0u;
+          const uint32_t r = run < (uint32_t)LZ_LANE_CAP ? min(run, limit) : run;
+          if (p >= entry && r >= 3u && limit >= 3u) m = r;
+          c = p - 1u;
+        }
         if (MODE == 1) {
           // this lane's 4 bytes; the word pair stays in registers for the compare below
           const uint32_t *wp = reinterpret_cast<const uint32_t *>(data) + ((doff + p) >> 2);
@@ -429,7 +447,7 @@ __global__ void __launch_bounds__(LZ_THREADS, 3)
         lz_select(data, doff, wb, b1, cur, nvalid, m, p - c, ring + slot * ZB_MATCH_SLOTS, sel, ism, endw);
         entry = wb + max(endw, nvalid);
         // level 1 counts the window's literals here, one atomic per lane, from the byte the probe already holds
-        if (MODE == 1 && ((sel & ~ism) >> lane & 1u)) atomicAdd(&whist[lit >> 1], 1u << ((lit & 1u) * 16u));
+        if (MODE != 0 && ((sel & ~ism) >> lane & 1u)) atomicAdd(&whist[lit >> 1], 1u << ((lit & 1u) * 16u));
         LZ_CLK(LZS_SELECT)
       }
       if (bl == slot) {
@@ -440,7 +458,7 @@ __global__ void __launch_bounds__(LZ_THREADS, 3)
       if (slot == LZ_BATCH_WINDOWS - 1u || wb + 32 >= b1) {
         __syncwarp();
         const uint32_t bwin = win - slot + bl;  // this lane's window
-        lz_batch_pass<LZ_BATCH_LPW, MODE != 1>(data + (uint32_t)(doff + (bwin << 5)), bl <= slot, ksel, kism, ring + bl * ZB_MATCH_SLOTS,
+        lz_batch_pass<LZ_BATCH_LPW, MODE == 0>(data + (uint32_t)(doff + (bwin << 5)), bl <= slot, ksel, kism, ring + bl * ZB_MATCH_SLOTS,
                                     whist, gmask + bwin, grecs, rec_base);
         ksel = kism = 0;
         __syncwarp();
@@ -663,7 +681,9 @@ __device__ __forceinline__ void fix_dict_head(uint8_t *data, const uint8_t *chun
   }
 }
 
-template <bool DICT>
+// MINM: the shortest match kept.  ZB200_STRATEGY_FILTERED instantiates 6: a lane's longest candidate shorter than
+// that counts as no match before the lazy rule compares neighbours (zlib deflate_slow's match_length <= 5 rule).
+template <bool DICT, int MINM = ZB_MIN_MATCH>
 __global__ void __launch_bounds__(LZ_THREADS, 2)
     k_lz2(const uint8_t *__restrict__ src, const ZbChunkDesc *__restrict__ desc, uint2 *__restrict__ masks,
           uint32_t *__restrict__ recs, uint16_t *__restrict__ hist, ZbChunkCheck *__restrict__ chk,
@@ -844,6 +864,7 @@ __global__ void __launch_bounds__(LZ_THREADS, 2)
           for (uint32_t k = 0; k < rounds; k++) {
             if (k < nl && budget > 0 && m < P.stop) lz2_extend(P, data, dlist[k * (uint32_t)LZ_THREADS], prm.good, m, dist, budget);
           }
+          if (MINM > ZB_MIN_MATCH && m < (uint32_t)MINM) m = 0;
           // one-step lazy evaluation (zlib's max_lazy idea)
           const uint32_t mnext = __shfl_down_sync(ZB_FULL, m, 1);
           if (lane < 31 && m != 0 && m < prm.lazy && mnext > m) m = 0;
@@ -1493,19 +1514,24 @@ size_t zb_lz2_table_bytes(int *grid_out) {
 // the k_lz instance for a level's matcher (MODE) and a format's checksum (CK)
 typedef void (*ZbLzKernel)(const uint8_t *, const ZbChunkDesc *, uint2 *, uint32_t *, uint16_t *, ZbChunkCheck *,
                            const ZbCrcTables *);
+template <int MODE>
+static ZbLzKernel zb_lz_kernel_ck(int ck) {
+  return ck == (ZB_CK_CRC | ZB_CK_ADLER) ? k_lz<MODE, ZB_CK_CRC | ZB_CK_ADLER>
+         : ck == ZB_CK_CRC               ? k_lz<MODE, ZB_CK_CRC>
+         : ck == ZB_CK_ADLER             ? k_lz<MODE, ZB_CK_ADLER>
+                                         : k_lz<MODE, 0>;
+}
 // (index_crc: the raw CRC-32 too, for a compress-time index: zlib takes both checksums, raw DEFLATE gzip's instance)
 static ZbLzKernel zb_lz_kernel(int mode, int data_format, bool index_crc = false) {
-  if (index_crc && data_format == ZB_DF_ZLIB) return mode ? k_lz<1, ZB_CK_CRC | ZB_CK_ADLER> : k_lz<0, ZB_CK_CRC | ZB_CK_ADLER>;
-  if (index_crc) data_format = ZB_DF_GZIP;
-  const int ck = data_format == ZB_DF_GZIP ? ZB_CK_CRC : data_format == ZB_DF_ZLIB ? ZB_CK_ADLER : 0;
-  if (mode) return ck == ZB_CK_CRC ? k_lz<1, ZB_CK_CRC> : ck == ZB_CK_ADLER ? k_lz<1, ZB_CK_ADLER> : k_lz<1, 0>;
-  return ck == ZB_CK_CRC ? k_lz<0, ZB_CK_CRC> : ck == ZB_CK_ADLER ? k_lz<0, ZB_CK_ADLER> : k_lz<0, 0>;
+  int ck = data_format == ZB_DF_GZIP ? ZB_CK_CRC : data_format == ZB_DF_ZLIB ? ZB_CK_ADLER : 0;
+  if (index_crc) ck |= ZB_CK_CRC;
+  return mode == 2 ? zb_lz_kernel_ck<2>(ck) : mode == 1 ? zb_lz_kernel_ck<1>(ck) : zb_lz_kernel_ck<0>(ck);
 }
 // function attributes are per device: zb200_init calls this once for the ctx's device
 cudaError_t zb_setup_deflate_attrs() {
   cudaError_t e = cudaSuccess;
   static const int fmts[3] = {ZB_DF_GZIP, ZB_DF_ZLIB, ZB_DF_DEFLATE};
-  for (int mode = 0; mode < 2; mode++)
+  for (int mode = 0; mode < 3; mode++)
     for (int f = 0; f < 4; f++) {
       const ZbLzKernel k = f < 3 ? zb_lz_kernel(mode, fmts[f]) : zb_lz_kernel(mode, ZB_DF_ZLIB, true);
       if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, LZ_SM_TOTAL);
@@ -1514,6 +1540,7 @@ cudaError_t zb_setup_deflate_attrs() {
     }
   if (e == cudaSuccess) e = cudaFuncSetAttribute(k_lz2<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, LZ2_SM_TOTAL);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(k_lz2<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, LZ2_SM_TOTAL);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(k_lz2<false, 6>, cudaFuncAttributeMaxDynamicSharedMemorySize, LZ2_SM_TOTAL);
   // load the remaining kernels now rather than at their first launch (see zb_setup_inflate_attrs)
   cudaFuncAttributes fa;
   if (e == cudaSuccess) e = cudaFuncGetAttributes(&fa, k_huff);
@@ -1529,21 +1556,26 @@ cudaError_t zb_launch_lz(const ZbCompressWork &w, cudaStream_t s, bool index_crc
     int grid = 0;
     (void)zb_lz2_table_bytes(&grid);
     if ((uint32_t)grid > w.n_chunks) grid = (int)w.n_chunks;
-    if (w.win16)
+    if (w.strategy == ZB_STRATEGY_FILTERED)
+      k_lz2<false, 6><<<grid, LZ_THREADS, LZ2_SM_TOTAL, s>>>(w.src, w.desc, w.masks, w.recs, w.hist, w.chk, w.tabs, w.lz2_tables,
+                                                             w.n_chunks, zb_lz2_params(w.level), nullptr, 0u, 0u);
+    else if (w.win16)
       k_lz2<true><<<grid, LZ_THREADS, LZ2_SM_TOTAL, s>>>(w.src, w.desc, w.masks, w.recs, w.hist, w.chk, w.tabs, w.lz2_tables,
                                                          w.n_chunks, zb_lz2_params(w.level), w.win16, w.win_len, w.win_stride);
     else
       k_lz2<false><<<grid, LZ_THREADS, LZ2_SM_TOTAL, s>>>(w.src, w.desc, w.masks, w.recs, w.hist, w.chk, w.tabs, w.lz2_tables,
                                                           w.n_chunks, zb_lz2_params(w.level), nullptr, 0u, 0u);
   } else {
-    const ZbLzKernel k = zb_lz_kernel((w.level == -2 || w.level == 0) ? 0 : 1, w.data_format, index_crc);
+    const int mode = (w.level == -2 || w.level == 0) ? 0 : w.strategy == ZB_STRATEGY_RLE ? 2 : 1;
+    const ZbLzKernel k = zb_lz_kernel(mode, w.data_format, index_crc);
     k<<<w.n_chunks, LZ_THREADS, LZ_SM_TOTAL, s>>>(w.src, w.desc, w.masks, w.recs, w.hist, w.chk, w.tabs);
   }
   return cudaGetLastError();
 }
 cudaError_t zb_launch_huff(const ZbCompressWork &w, cudaStream_t s) {
   if (w.n_chunks == 0) return cudaSuccess;
-  k_huff<<<(w.n_chunks + HW_WARPS - 1) / HW_WARPS, HW_WARPS * 32, 0, s>>>(w.desc, w.hist, w.cb, w.n_chunks, w.level);
+  k_huff<<<(w.n_chunks + HW_WARPS - 1) / HW_WARPS, HW_WARPS * 32, 0, s>>>(w.desc, w.hist, w.cb, w.n_chunks, w.level,
+                                                                     w.strategy == ZB_STRATEGY_FIXED);
   return cudaGetLastError();
 }
 cudaError_t zb_launch_scan(const ZbCompressWork &w, cudaStream_t s) {

@@ -178,7 +178,8 @@ ZB_HD void zb_put_bits(ZbBitSink *s, uint32_t v, int n) {  // n <= 16, LSB first
 // Build everything the packer needs for one chunk.
 //   hist: per-warp histograms, hist[w * ZB_HIST_SYMS + s], s < 286 literal/length,
 //         s >= 286 distance codes; end-of-block is NOT counted (added here).
-//   force_type: -1 choose smallest, 0 force stored (level 0).
+//   force_type: -1 choose smallest, 0 force stored (level 0), 1 the smaller of stored and fixed, never dynamic
+//   (ZB200_STRATEGY_FIXED).
 ZB_HD_NOINLINE void zb_build_codebook(const uint16_t *hist, uint32_t chunk_len, int is_final,
                                       int force_type, ZbCodebook *cb) {
   const uint8_t len_extra[29] = ZB_LENGTH_EXTRA;
@@ -291,7 +292,7 @@ ZB_HD_NOINLINE void zb_build_codebook(const uint16_t *hist, uint32_t chunk_len, 
 
   int type = 2;
   uint64_t best = dyn_bytes;
-  if (fix_bytes < best) {
+  if (fix_bytes < best || force_type == 1) {
     type = 1;
     best = fix_bytes;
   }

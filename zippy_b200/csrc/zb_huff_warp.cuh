@@ -206,7 +206,7 @@ __device__ __forceinline__ uint32_t hw_cost(const uint8_t *lens, int s) {
 }
 
 //   hw: the chunk's eight sub-chunk histograms as words (two u16 counters each), end-of-block not counted
-//   force_type: -1 choose the smallest block, 0 stored (level 0)
+//   force_type: -1 choose the smallest block, 0 stored (level 0), 1 the smaller of stored and fixed (never dynamic)
 __device__ __forceinline__ void hw_build_codebook(HwWarp &ws, const uint32_t *__restrict__ hw, uint32_t chunk_len,
                                                   uint32_t is_final, int force_type, ZbCodebook *cb, HwClk &clk) {
   const int lane = zb_lane();
@@ -442,7 +442,7 @@ __device__ __forceinline__ void hw_build_codebook(HwWarp &ws, const uint32_t *__
   const uint64_t fix_bytes = is_final ? (fix_bits + 7) / 8 : (fix_bits + 3 + 7) / 8 + 4;
   int type = 2;
   uint64_t best = dyn_bytes;
-  if (fix_bytes < best) {
+  if (fix_bytes < best || force_type == 1) {
     type = 1;
     best = fix_bytes;
   }
@@ -545,7 +545,7 @@ __device__ __forceinline__ void hw_build_codebook(HwWarp &ws, const uint32_t *__
 // One warp per chunk, HW_WARPS chunks per CTA.
 __global__ void __launch_bounds__(HW_WARPS * 32)
     k_huff(const ZbChunkDesc *__restrict__ desc, const uint16_t *__restrict__ hist, ZbCodebook *__restrict__ cb,
-           uint32_t n_chunks, int level) {
+           uint32_t n_chunks, int level, bool fixed_only = false) {
   __shared__ HwWarp ws_all[HW_WARPS];
   const uint32_t warp = threadIdx.x >> 5;
   const uint32_t c = blockIdx.x * HW_WARPS + warp;
@@ -554,6 +554,6 @@ __global__ void __launch_bounds__(HW_WARPS * 32)
   HwClk clk;
   clk.start();
   hw_build_codebook(ws_all[warp], reinterpret_cast<const uint32_t *>(hist) + (size_t)c * ZB_WARPS_PER_CHUNK * ZB_HIST_WORDS,
-                    d.len, (d.flags & ZB_CHUNK_LAST) ? 1u : 0u, level == 0 ? 0 : -1, &cb[c], clk);
+                    d.len, (d.flags & ZB_CHUNK_LAST) ? 1u : 0u, level == 0 ? 0 : fixed_only ? 1 : -1, &cb[c], clk);
   clk.publish();
 }

@@ -60,6 +60,9 @@ struct ZbCompressWork {
   uint2 *lz2_tables;           // k_lz2 dictionaries: [grid][8 own tables of 2048 x 4 ways + 12 segment tables of 8192 entries], u16 positions (LZ levels only)
   uint32_t n_chunks, n_members;
   int level, data_format;
+  // ZB_STRATEGY_*, after zb_strategy_level: RLE only at level 1 (k_lz<2>), FILTERED only at the LZ levels (k_lz2<false, 6>),
+  // FIXED at any level but 0 (k_huff: stored or fixed blocks); HUFFMAN_ONLY never (it is level -2)
+  int strategy;
   // A preset dictionary (zb200_compress_batch_dict): has_dict puts FDICT and dict_id in the zlib header.  win16 holds
   // 16 copies of the window W (win_len bytes; win16 256-byte aligned), copy c at
   // win16 + c * win_stride + ZB_WIN16_SLACK + ((c - win_len) & 15), so that W ends at an address that is c modulo 16;
