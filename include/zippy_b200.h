@@ -371,7 +371,7 @@ int zb200_compress_stream_index(zb200_compress_stream *st, zb200_index **out);
  *    levels do;
  *  - DEFAULT and FIXED: the level's parse.
  * Each chunk's block is the smallest of stored, fixed and dynamic, except under FIXED: the smaller of stored and
- * fixed, never dynamic.  Framing, chunking and the zlib header (78 01) do not change, and zb200_compress_bound covers
+ * fixed, never dynamic.  Framing, chunking and the zlib header (78 01 at window 15) do not change, and zb200_compress_bound covers
  * every strategy.  Not combined with dictionaries, compress-time indexes, zb200_compress_batch_h2d or multi-GPU.
  * The _strategy calls take the arguments of the calls without it, plus `strategy` after `level`. */
 enum {
@@ -389,6 +389,33 @@ int zb200_compress_batch_device_strategy(zb200_ctx *ctx, const uint8_t *d_src, c
                                          uint8_t *d_dst, size_t dst_cap, uint64_t *dst_offsets, int *statuses);
 int zb200_compress_stream_begin_strategy(zb200_ctx *ctx, int level, int strategy, int data_format, int fname_len,
                                          zb200_compress_stream **out);
+
+/* ---- window size: zlib's `windowBits` (deflateInit2, the magnitude of zlib.compressobj's wbits) ----
+ * window_bits n in 9..15: no match of any member reaches more than 2^n bytes back, the window RFC 1950 states
+ * through CINFO and the one zlib's inflater with wbits = n accepts (zlib's own deflater stops at 2^n - 262; a
+ * decoder needs no such margin).  n = 8 is accepted for the zlib format only and means 9, as in zlib; any other n
+ * fails with ZB200_ERR_ARG and leaves statuses alone.
+ *  - zlib format: CMF = (n - 8) << 4 | 8, FLEVEL 0, FCHECK recomputed (78 01 at n = 15).  gzip and raw DEFLATE have
+ *    no window field: only the parse changes;
+ *  - n = 15 is exactly the calls without _window, for every level, strategy and format;
+ *  - levels 0 and -2, HUFFMAN_ONLY and RLE make no match beyond distance 1 and are unaffected (their zlib header
+ *    still states n).  Level 1's matches reach at most 6 KiB back (a 4 KiB piece and its 2 KiB pre-seed), so it
+ *    changes only for n <= 12.  Levels -1 and 2..9, FILTERED included, change for every n < 15: a preceding 8 KiB
+ *    segment j (0 = nearest) is looked up only when 8192 j < 2^n;
+ *  - a stream keeps its window for its whole life: sync flushes, full flushes and the history carried across
+ *    writes all respect it.
+ * zb200_compress_bound and zb200_compress_stream_bound cover every window.  Not combined with dictionaries,
+ * compress-time indexes, zb200_compress_batch_h2d or multi-GPU.  The _window calls take the arguments of the
+ * _strategy calls, plus `window_bits` after `strategy`. */
+int zb200_compress_batch_window(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n,
+                                int level, int strategy, int window_bits, int data_format, const uint8_t *fname_lens,
+                                uint8_t *dst_base, size_t dst_cap, uint64_t *dst_offsets, int *statuses);
+int zb200_compress_batch_device_window(zb200_ctx *ctx, const uint8_t *d_src, const uint64_t *src_offsets, size_t n,
+                                       int level, int strategy, int window_bits, int data_format,
+                                       const uint8_t *fname_lens, uint8_t *d_dst, size_t dst_cap, uint64_t *dst_offsets,
+                                       int *statuses);
+int zb200_compress_stream_begin_window(zb200_ctx *ctx, int level, int strategy, int window_bits, int data_format,
+                                       int fname_len, zb200_compress_stream **out);
 
 /* ---- device-resident variants (pointers prefixed d_ are device memory on ctx's device;
  * offsets / statuses / sizes stay host arrays).  Used when the data already lives in HBM

@@ -183,6 +183,27 @@ inline std::string compress(const std::string &src, int level, CompressedDataFor
   return compress(src.data(), src.size(), level, dataFormat, strategy);
 }
 
+// With zlib's window size (windowBits 9..15; 8 for dfZlib means 9): one member of zb200_compress_batch_window, no
+// match reaching more than 2^windowBits back.  windowBits 15 writes the overload above's bytes.
+inline std::string compress(const void *srcp, size_t len, int level, CompressedDataFormat dataFormat, Strategy strategy,
+                            int windowBits) {
+  const uint64_t offs[2] = {0, len};
+  uint64_t out_offs[2] = {0, 0};
+  int st = 0;
+  const uint8_t fl = dataFormat == dfGzip ? (uint8_t)(std::random_device()() % 26) : 0;
+  std::string result(zb200_compress_bound(len, dataFormat) + 64, '\0');
+  uint8_t dummy = 0;
+  detail::check(zb200_compress_batch_window(detail::ctx(), len ? static_cast<const uint8_t *>(srcp) : &dummy, offs, 1,
+                                            level, strategy, windowBits, dataFormat, &fl,
+                                            reinterpret_cast<uint8_t *>(&result[0]), result.size(), out_offs, &st));
+  result.resize(out_offs[1]);
+  return result;
+}
+inline std::string compress(const std::string &src, int level, CompressedDataFormat dataFormat, Strategy strategy,
+                            int windowBits) {
+  return compress(src.data(), src.size(), level, dataFormat, strategy, windowBits);
+}
+
 // gzip.nim:3-88
 inline void uncompressGzip(std::string &dst, const uint8_t *src, size_t len) {
   auto fail = [] { throw ZippyError(ZB200_ERR_UNCOMPRESS, "Invalid buffer, unable to uncompress"); };
@@ -331,6 +352,14 @@ class CompressStream {
   CompressStream(int level, CompressedDataFormat dataFormat, Strategy strategy, int fnameLen = -1, zb200_ctx *ctx = nullptr) {
     if (fnameLen < 0) fnameLen = dataFormat == dfGzip ? (int)(std::random_device()() % 26) : 0;
     detail::check(zb200_compress_stream_begin_strategy(ctx ? ctx : detail::ctx(), level, strategy, dataFormat, fnameLen, &st_));
+  }
+  // with a window size, kept for the stream's whole life (zb200_compress_stream_begin_window); fnameLen -1 draws it
+  // (it has no default: four arguments are the strategy constructor's, with fnameLen)
+  CompressStream(int level, CompressedDataFormat dataFormat, Strategy strategy, int windowBits, int fnameLen,
+                 zb200_ctx *ctx = nullptr) {
+    if (fnameLen < 0) fnameLen = dataFormat == dfGzip ? (int)(std::random_device()() % 26) : 0;
+    detail::check(zb200_compress_stream_begin_window(ctx ? ctx : detail::ctx(), level, strategy, windowBits, dataFormat,
+                                                     fnameLen, &st_));
   }
   // that also writes the member's index (zb200_compress_stream_begin_index): index() after finish()
   CompressStream(int level, CompressedDataFormat dataFormat, int fnameLen, uint64_t indexSpan, zb200_ctx *ctx = nullptr)

@@ -595,3 +595,33 @@ proc newCompressStream*(level: int, dataFormat: CompressedDataFormat, strategy: 
   let k = if fnameLen < 0: randomFnameLen(dataFormat) else: fnameLen
   check zb200_compress_stream_begin_strategy(getCtx(), level.cint, strategy.cint, dataFormat.cint, k.cint,
                                              result.st.addr)
+
+# ---- window size (zlib's `windowBits`, 9..15; 8 for dfZlib means 9; include/zippy_b200.h "window size"): no
+# match reaches more than 2^windowBits back; not combined with dictionaries or compress-time indexes ----
+proc zb200_compress_batch_window(ctx: Zb200Ctx, srcBase: pointer, srcOffsets: ptr uint64, n: csize_t,
+                                 level, strategy, windowBits, dataFormat: cint, fnameLens: pointer, dstBase: pointer,
+                                 dstCap: csize_t, dstOffsets: ptr uint64,
+                                 statuses: ptr cint): cint {.importc, cdecl, dynlib: lib.}
+proc zb200_compress_stream_begin_window(ctx: Zb200Ctx, level, strategy, windowBits, dataFormat, fnameLen: cint,
+                                        st: ptr Zb200CompressStream): cint {.importc, cdecl, dynlib: lib.}
+
+proc compress*(src: string, level: int, dataFormat: CompressedDataFormat, strategy: Strategy,
+               windowBits: int): string {.raises: [ZippyError].} =
+  ## one member of zb200_compress_batch_window; gzip draws its FNAME length at random, as compress does
+  var
+    offs = [0'u64, src.len.uint64]
+    outOffs = [0'u64, 0'u64]
+    fl = randomFnameLen(dataFormat).uint8
+    dummy: uint8
+  result = newString(zb200_compress_bound(src.len.csize_t, dataFormat.cint).int + 64)
+  check zb200_compress_batch_window(getCtx(), (if src.len > 0: src[0].unsafeAddr else: dummy.addr),
+                                    offs[0].addr, 1, level.cint, strategy.cint, windowBits.cint, dataFormat.cint,
+                                    fl.addr, result[0].addr, result.len.csize_t, outOffs[0].addr, nil)
+  result.setLen(outOffs[1].int)
+
+proc newCompressStream*(level: int, dataFormat: CompressedDataFormat, strategy: Strategy, windowBits: int,
+                        fnameLen = -1): CompressStream {.raises: [ZippyError].} =
+  ## a stream with a window size (and a strategy): zb200_compress_stream_begin_window
+  let k = if fnameLen < 0: randomFnameLen(dataFormat) else: fnameLen
+  check zb200_compress_stream_begin_window(getCtx(), level.cint, strategy.cint, windowBits.cint, dataFormat.cint,
+                                           k.cint, result.st.addr)

@@ -69,14 +69,17 @@ def _dict(dictionary):
     return d if d is not None and d.size else None
 
 
-def _strategy_alone(strategy, dictionary=None, index_span=None):
-    """True for a strategy other than the default; such a strategy takes no dictionary and no compress-time index."""
-    if strategy == StrategyDefault:
+def _params_alone(strategy, window_bits=15, dictionary=None, index_span=None):
+    """True for a strategy other than the default or a window other than 15 (the _window calls); either takes no
+    dictionary and no compress-time index."""
+    what = "a compression strategy" if strategy != StrategyDefault else "a window size other than 15" \
+        if window_bits != 15 else None
+    if what is None:
         return False
     if _dict(dictionary) is not None:
-        raise ZippyError(22, "a compression strategy is not combined with a dictionary")
+        raise ZippyError(22, what + " is not combined with a dictionary")
     if index_span is not None:
-        raise ZippyError(22, "a compression strategy is not combined with a compress-time index")
+        raise ZippyError(22, what + " is not combined with a compress-time index")
     return True
 
 
@@ -122,9 +125,11 @@ class Context:
 
     # ---- batches over host buffers -------------------------------------------------
     def compress_batch(self, base, offsets, level=DefaultCompression, dataFormat=dfGzip, fname_lens=None,
-                       dictionary=None, index_span=None, strategy=StrategyDefault):
+                       dictionary=None, index_span=None, strategy=StrategyDefault, window_bits=15):
         """-> (out uint8 array, out_offsets uint64[n+1]).  fname_lens: per-input gzip FNAME letters (0..25).
-        strategy: zlib's compression strategy (Strategy*; zb200_compress_batch_strategy; no dictionary or index).
+        strategy: zlib's compression strategy (Strategy*; zb200_compress_batch_window; no dictionary or index).
+        window_bits: zlib's window size, 9..15 (8 for zlib: 9); no match reaches more than 2^window_bits back
+        (zb200_compress_batch_window; no dictionary or index).
         dictionary: a preset dictionary shared by every input (zlib / raw only; zb200_compress_batch_dict).
         index_span: also write each member's Index with this span (zb200_compress_batch_index; no dictionary):
         -> (out, out_offsets, list of Index)."""
@@ -138,13 +143,13 @@ class Context:
         out_offs = np.zeros(n + 1, dtype=np.uint64)
         st = np.zeros(max(n, 1), dtype=np.int32)
         d = _dict(dictionary)
-        if _strategy_alone(strategy, d, index_span):
+        if _params_alone(strategy, window_bits, d, index_span):
             fl = np.ascontiguousarray(fname_lens, dtype=np.uint8) if fname_lens is not None else None
-            _check(self._h, L.zb200_compress_batch_strategy(self._h, base.ctypes.data, offsets.ctypes.data, n, level,
-                                                             strategy, dataFormat,
-                                                             fl.ctypes.data if fl is not None else None,
-                                                             out.ctypes.data, out.size, out_offs.ctypes.data,
-                                                             st.ctypes.data))
+            _check(self._h, L.zb200_compress_batch_window(self._h, base.ctypes.data, offsets.ctypes.data, n, level,
+                                                           strategy, window_bits, dataFormat,
+                                                           fl.ctypes.data if fl is not None else None,
+                                                           out.ctypes.data, out.size, out_offs.ctypes.data,
+                                                           st.ctypes.data))
             return out[:int(out_offs[n])], out_offs
         if index_span is not None:
             if d is not None:
@@ -286,19 +291,20 @@ class Context:
 
     # ---- device-resident batches (raw device pointers; e.g. torch tensor .data_ptr()) ----
     def compress_batch_device(self, d_src, offsets, level, dataFormat, d_dst, dst_cap, fname_lens=None,
-                              index_span=None, strategy=StrategyDefault):
+                              index_span=None, strategy=StrategyDefault, window_bits=15):
         """-> out_offsets; with index_span also each member's Index (zb200_compress_batch_device_index):
-        -> (out_offsets, list of Index).  strategy: zlib's compression strategy (no index)."""
+        -> (out_offsets, list of Index).  strategy, window_bits: zlib's compression strategy and window size
+        (zb200_compress_batch_device_window; no index)."""
         L = _native.lib()
         offsets = np.ascontiguousarray(offsets, dtype=np.uint64)
         n = len(offsets) - 1
         out_offs = np.zeros(n + 1, dtype=np.uint64)
         fl = np.ascontiguousarray(fname_lens, dtype=np.uint8) if fname_lens is not None else None
-        if _strategy_alone(strategy, None, index_span):
-            _check(self._h, L.zb200_compress_batch_device_strategy(self._h, d_src, offsets.ctypes.data, n, level,
-                                                                    strategy, dataFormat,
-                                                                    fl.ctypes.data if fl is not None else None, d_dst,
-                                                                    dst_cap, out_offs.ctypes.data, None))
+        if _params_alone(strategy, window_bits, None, index_span):
+            _check(self._h, L.zb200_compress_batch_device_window(self._h, d_src, offsets.ctypes.data, n, level,
+                                                                  strategy, window_bits, dataFormat,
+                                                                  fl.ctypes.data if fl is not None else None, d_dst,
+                                                                  dst_cap, out_offs.ctypes.data, None))
             return out_offs
         if index_span is not None:
             hs = (ctypes.c_void_p * max(n, 1))()
@@ -365,11 +371,12 @@ class Context:
         return {f: getattr(t, f) for f, _ in t._fields_}
 
     # ---- the single-input seam (deflate.nim:207, inflate.nim:268, crc.nim:53, adler32.nim:6) ----
-    def deflate(self, src, level=DefaultCompression, strategy=StrategyDefault):
+    def deflate(self, src, level=DefaultCompression, strategy=StrategyDefault, window_bits=15):
         L = _native.lib()
         src = _as_u8(src)
-        if strategy != StrategyDefault:   # one raw DEFLATE member of the batch call
-            out, _ = self.compress_batch(src, [0, src.size], level, dfDeflate, strategy=strategy)
+        if strategy != StrategyDefault or window_bits != 15:   # one raw DEFLATE member of the batch call
+            out, _ = self.compress_batch(src, [0, src.size], level, dfDeflate, strategy=strategy,
+                                         window_bits=window_bits)
             return out.tobytes()
         cap = L.zb200_deflate_bound(src.size)
         out = np.empty(cap + 8, dtype=np.uint8)
@@ -421,18 +428,18 @@ class CompressStream:
     length is drawn at random, as compress() does (zippy.nim:28-42)."""
 
     def __init__(self, level=DefaultCompression, dataFormat=dfGzip, fname_len=None, ctx=None, dictionary=None,
-                 index_span=None, strategy=StrategyDefault):
+                 index_span=None, strategy=StrategyDefault, window_bits=15):
         """index_span: also write the member's Index with this span (zb200_compress_stream_begin_index; no
-        dictionary), returned by index() after finish().  strategy: zlib's compression strategy
-        (zb200_compress_stream_begin_strategy; no dictionary or index)."""
+        dictionary), returned by index() after finish().  strategy, window_bits: zlib's compression strategy and
+        window size, kept for the stream's whole life (zb200_compress_stream_begin_window; no dictionary or index)."""
         self._ctx = ctx if ctx is not None else default_context()
         self._h = ctypes.c_void_p()
         d = _dict(dictionary)
-        if _strategy_alone(strategy, d, index_span):
+        if _params_alone(strategy, window_bits, d, index_span):
             if fname_len is None:
                 fname_len = os.urandom(1)[0] % 26 if dataFormat == dfGzip else 0
-            _check(self._ctx._h, _native.lib().zb200_compress_stream_begin_strategy(
-                self._ctx._h, level, strategy, dataFormat, fname_len, ctypes.byref(self._h)))
+            _check(self._ctx._h, _native.lib().zb200_compress_stream_begin_window(
+                self._ctx._h, level, strategy, window_bits, dataFormat, fname_len, ctypes.byref(self._h)))
             return
         if index_span is not None:
             if d is not None:
@@ -753,9 +760,11 @@ def default_context():
 
 
 # ---- the reference's public procs ------------------------------------------------------
-def compress(src, level=DefaultCompression, dataFormat=dfGzip, dictionary=None, strategy=StrategyDefault):
+def compress(src, level=DefaultCompression, dataFormat=dfGzip, dictionary=None, strategy=StrategyDefault,
+             window_bits=15):
     """zippy.compress (zippy.nim:11-98).  dictionary: a preset dictionary (zlib / raw only; zlib's zdict).
-    strategy: zlib's compression strategy (Strategy*), not with a dictionary."""
+    strategy: zlib's compression strategy (Strategy*), not with a dictionary.  window_bits: zlib's window size
+    (9..15; 8 for zlib means 9): no match reaches more than 2^window_bits back; other than 15 not with a dictionary."""
     if level < -2 or level > 9:
         raise ZippyError(1, "Invalid compression level %d" % level)          # deflate.nim:208-209
     if dataFormat not in (dfGzip, dfZlib, dfDeflate):
@@ -765,7 +774,7 @@ def compress(src, level=DefaultCompression, dataFormat=dfGzip, dictionary=None, 
         fl = [os.urandom(1)[0] % 26]                                         # zippy.nim:28-42
     base, offs = _pack([src])
     out, _ = default_context().compress_batch(base, offs, level, dataFormat, fl, dictionary=dictionary,
-                                              strategy=strategy)
+                                              strategy=strategy, window_bits=window_bits)
     return out.tobytes()
 
 
@@ -799,8 +808,8 @@ def adler32(src):
     return default_context().adler32(src)
 
 
-def deflate(src, level=DefaultCompression, strategy=StrategyDefault):
-    return default_context().deflate(src, level, strategy)
+def deflate(src, level=DefaultCompression, strategy=StrategyDefault, window_bits=15):
+    return default_context().deflate(src, level, strategy, window_bits)
 
 
 def inflate(src, pos=0):
@@ -808,11 +817,11 @@ def inflate(src, pos=0):
 
 
 def compress_batch(items, level=DefaultCompression, dataFormat=dfGzip, fname_lens=None, dictionary=None,
-                   strategy=StrategyDefault):
+                   strategy=StrategyDefault, window_bits=15):
     """list of bytes -> list of bytes (one zippy.compress per item, one GPU launch sequence)."""
     base, offs = _pack(items)
     out, oo = default_context().compress_batch(base, offs, level, dataFormat, fname_lens, dictionary=dictionary,
-                                               strategy=strategy)
+                                               strategy=strategy, window_bits=window_bits)
     return [out[int(oo[i]):int(oo[i + 1])].tobytes() for i in range(len(items))]
 
 

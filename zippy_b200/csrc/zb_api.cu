@@ -246,6 +246,7 @@ struct zb200_compress_stream {
   zb200_ctx *ctx = nullptr;
   int level = 0, data_format = 0;
   int strategy = ZB_STRATEGY_DEFAULT;  // folded with the level by zb_strategy_level
+  int window_bits = 15;        // after zb_window_bits: every launch, flush and carried history keeps to it
   uint8_t fname_len = 0;
   size_t batch_bytes = 0;      // launch once this much input is pending
   std::vector<uint8_t> buf;    // [history | pending input]: pending starts at a chunk boundary of its flush segment
@@ -561,6 +562,13 @@ static int zb_strategy_level(int &level, int &strategy) {
   return ZB200_OK;
 }
 
+// zlib's window size (deflateInit2's windowBits, zlib.compressobj's wbits): 9..15, and 8 for the zlib format, where it
+// means 9 as in zlib.  ZB200_ERR_ARG for anything else.
+static int zb_window_bits(int &window_bits, int data_format) {
+  if (window_bits == 8 && data_format == ZB200_DF_ZLIB) window_bits = 9;
+  return window_bits < 9 || window_bits > 15 ? ZB200_ERR_ARG : ZB200_OK;
+}
+
 // ---- compress: device-resident (h_src == h_dst == nullptr) or pipelined host buffers ----
 // With host buffers the batch is cut into groups and H2D(g+1) || kernels(g) || D2H(g-1) run
 // on three streams; each group's output offset is chained on the device (out_base_ptr), so
@@ -571,9 +579,10 @@ int compress_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint8_t *h_src, 
                     size_t n, int level, int data_format, const uint8_t *fname_lens, uint8_t *d_dst,
                     size_t dst_cap, uint8_t *h_dst, size_t h_dst_cap, uint64_t *dst_offsets, int *statuses,
                     size_t max_group_chunks, StreamPart *sp = nullptr, const ZbIndexWork *ix = nullptr,
-                    int strategy = ZB_STRATEGY_DEFAULT) {
+                    int strategy = ZB_STRATEGY_DEFAULT, int window_bits = 15) {
   const auto t_entry = std::chrono::steady_clock::now();
   if (int rc = zb_strategy_level(level, strategy)) return rc;
+  if (int rc = zb_window_bits(window_bits, data_format)) return rc;
   if (data_format != ZB200_DF_GZIP && data_format != ZB200_DF_ZLIB && data_format != ZB200_DF_DEFLATE)
     return ZB200_ERR_INVALID_FORMAT;
   if (fname_lens)
@@ -734,6 +743,7 @@ int compress_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint8_t *h_src, 
     w.n_members = (uint32_t)(g.m1 - g.m0);
     w.level = level;
     w.strategy = strategy;
+    w.max_dist = 1u << window_bits;
     w.data_format = data_format;
     w.out_base = 0;
     w.out_base_ptr = (const uint64_t *)ctx->group_end.p + gi;
@@ -998,7 +1008,8 @@ int stream_run(zb200_compress_stream *st, size_t nbytes, bool last, uint8_t *dst
   }
   int rc = compress_locked(ctx, (const uint8_t *)ctx->in_stage.p, st->buf.data(), offs, 1, st->level, st->data_format,
                            &st->fname_len, (uint8_t *)ctx->out_stage.p, ctx->out_stage.cap & ~(size_t)3, dst, dst_cap,
-                           dst_offs, nullptr, ctx->host_group_chunks, &sp, st->ix ? &x : nullptr, st->strategy);
+                           dst_offs, nullptr, ctx->host_group_chunks, &sp, st->ix ? &x : nullptr, st->strategy,
+                           st->window_bits);
   if (rc) return rc;
   *dst_len = (size_t)dst_offs[1];
   if (st->ix) {
@@ -2691,17 +2702,25 @@ size_t zb200_compress_bound(size_t len, int data_format) {
   return zb200_deflate_bound(len) + frame;
 }
 
-int zb200_compress_batch_device_strategy(zb200_ctx *ctx, const uint8_t *d_src, const uint64_t *src_offsets, size_t n,
-                                         int level, int strategy, int data_format, const uint8_t *fname_lens,
-                                         uint8_t *d_dst, size_t dst_cap, uint64_t *dst_offsets, int *statuses) {
+int zb200_compress_batch_device_window(zb200_ctx *ctx, const uint8_t *d_src, const uint64_t *src_offsets, size_t n,
+                                       int level, int strategy, int window_bits, int data_format,
+                                       const uint8_t *fname_lens, uint8_t *d_dst, size_t dst_cap, uint64_t *dst_offsets,
+                                       int *statuses) {
   return guarded(ctx, [&]() -> int {
   if (!ctx || !src_offsets || !dst_offsets || (n && (!d_src || !d_dst))) return ZB200_ERR_ARG;
   std::lock_guard<std::mutex> lk(ctx->mu);
   DeviceGuard g(ctx->device);
   ctx->timing.kernel_launches = 0;
   return compress_locked(ctx, d_src, nullptr, src_offsets, n, level, data_format, fname_lens, d_dst, dst_cap, nullptr,
-                         0, dst_offsets, statuses, ctx->dev_group_chunks, nullptr, nullptr, strategy);
+                         0, dst_offsets, statuses, ctx->dev_group_chunks, nullptr, nullptr, strategy, window_bits);
   });
+}
+
+int zb200_compress_batch_device_strategy(zb200_ctx *ctx, const uint8_t *d_src, const uint64_t *src_offsets, size_t n,
+                                         int level, int strategy, int data_format, const uint8_t *fname_lens,
+                                         uint8_t *d_dst, size_t dst_cap, uint64_t *dst_offsets, int *statuses) {
+  return zb200_compress_batch_device_window(ctx, d_src, src_offsets, n, level, strategy, 15, data_format, fname_lens,
+                                            d_dst, dst_cap, dst_offsets, statuses);
 }
 
 int zb200_compress_batch_device(zb200_ctx *ctx, const uint8_t *d_src, const uint64_t *src_offsets, size_t n,
@@ -2715,9 +2734,10 @@ int zb200_compress_batch_device(zb200_ctx *ctx, const uint8_t *d_src, const uint
 static int compress_batch_host(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n, int level,
                                int data_format, const uint8_t *dict, size_t dict_len, const uint8_t *fname_lens,
                                uint8_t *dst_base, size_t dst_cap, uint64_t *dst_offsets, int *statuses,
-                               int strategy = ZB_STRATEGY_DEFAULT) {
+                               int strategy = ZB_STRATEGY_DEFAULT, int window_bits = 15) {
   return guarded(ctx, [&]() -> int {
   if (!ctx || !src_offsets || !dst_offsets || (n && (!src_base || !dst_base)) || (dict_len && !dict)) return ZB200_ERR_ARG;
+  if (zb_window_bits(window_bits, data_format)) return ZB200_ERR_ARG;
   if (dict_len) {  // zlib's deflateSetDictionary refuses gzip too: the format has no field for it
     if (level < -2 || level > 9) return ZB200_ERR_INVALID_LEVEL;
     if (data_format != ZB200_DF_ZLIB && data_format != ZB200_DF_DEFLATE) return ZB200_ERR_INVALID_FORMAT;
@@ -2741,7 +2761,8 @@ static int compress_batch_host(zb200_ctx *ctx, const uint8_t *src_base, const ui
   ENSURE(ctx->out_stage, (size_t)bound + 64);
   int rc = compress_locked(ctx, (const uint8_t *)ctx->in_stage.p, src_base, src_offsets, n, level, data_format,
                            fname_lens, (uint8_t *)ctx->out_stage.p, ctx->out_stage.cap & ~(size_t)3, dst_base,
-                           dst_cap, dst_offsets, statuses, ctx->host_group_chunks, nullptr, nullptr, strategy);
+                           dst_cap, dst_offsets, statuses, ctx->host_group_chunks, nullptr, nullptr, strategy,
+                           window_bits);
   if (rc) return rc;
   ctx->timing.h2d_ms = ev_ms(ctx->ev[6], ctx->ev[7]);
   ctx->timing.d2h_ms = ev_ms(ctx->ev[8], ctx->ev[9]);
@@ -2761,8 +2782,15 @@ int zb200_compress_batch(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t
 int zb200_compress_batch_strategy(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n,
                                   int level, int strategy, int data_format, const uint8_t *fname_lens,
                                   uint8_t *dst_base, size_t dst_cap, uint64_t *dst_offsets, int *statuses) {
+  return zb200_compress_batch_window(ctx, src_base, src_offsets, n, level, strategy, 15, data_format, fname_lens,
+                                     dst_base, dst_cap, dst_offsets, statuses);
+}
+
+int zb200_compress_batch_window(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n,
+                                int level, int strategy, int window_bits, int data_format, const uint8_t *fname_lens,
+                                uint8_t *dst_base, size_t dst_cap, uint64_t *dst_offsets, int *statuses) {
   return compress_batch_host(ctx, src_base, src_offsets, n, level, data_format, nullptr, 0, fname_lens, dst_base, dst_cap,
-                             dst_offsets, statuses, strategy);
+                             dst_offsets, statuses, strategy, window_bits);
 }
 
 int zb200_compress_batch_dict(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n, int level,
@@ -2804,7 +2832,8 @@ int zb200_compress_batch_h2d(zb200_ctx *ctx, const uint8_t *src_base, const uint
 // zb200_compress_stream_begin, and with a non-empty dictionary zb200_compress_stream_begin_dict: the window is the
 // history in front of the first chunk (LZ levels), exactly as after a sync flush of it, and zlib's header carries it
 static int compress_stream_begin(zb200_ctx *ctx, int level, int data_format, int fname_len, const uint8_t *dict,
-                                 size_t dict_len, zb200_compress_stream **out, int strategy = ZB_STRATEGY_DEFAULT) {
+                                 size_t dict_len, zb200_compress_stream **out, int strategy = ZB_STRATEGY_DEFAULT,
+                                 int window_bits = 15) {
   return guarded(ctx, [&]() -> int {
     if (!ctx || !out || (dict_len && !dict)) return ZB200_ERR_ARG;
     *out = nullptr;
@@ -2814,10 +2843,12 @@ static int compress_stream_begin(zb200_ctx *ctx, int level, int data_format, int
       return ZB200_ERR_INVALID_FORMAT;
     if (dict_len && data_format == ZB200_DF_GZIP) return ZB200_ERR_INVALID_FORMAT;
     if (fname_len < 0 || fname_len > 25) return ZB200_ERR_ARG;
+    if (int rc = zb_window_bits(window_bits, data_format)) return rc;
     zb200_compress_stream *st = new zb200_compress_stream();
     st->ctx = ctx;
     st->level = level;
     st->strategy = strategy;
+    st->window_bits = window_bits;
     st->data_format = data_format;
     st->fname_len = (uint8_t)fname_len;
     {
@@ -2844,7 +2875,12 @@ int zb200_compress_stream_begin(zb200_ctx *ctx, int level, int data_format, int 
 
 int zb200_compress_stream_begin_strategy(zb200_ctx *ctx, int level, int strategy, int data_format, int fname_len,
                                          zb200_compress_stream **out) {
-  return compress_stream_begin(ctx, level, data_format, fname_len, nullptr, 0, out, strategy);
+  return zb200_compress_stream_begin_window(ctx, level, strategy, 15, data_format, fname_len, out);
+}
+
+int zb200_compress_stream_begin_window(zb200_ctx *ctx, int level, int strategy, int window_bits, int data_format,
+                                       int fname_len, zb200_compress_stream **out) {
+  return compress_stream_begin(ctx, level, data_format, fname_len, nullptr, 0, out, strategy, window_bits);
 }
 
 int zb200_compress_stream_begin_dict(zb200_ctx *ctx, int level, int data_format, const uint8_t *dict, size_t dict_len,

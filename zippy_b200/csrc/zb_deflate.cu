@@ -228,11 +228,13 @@ extern "C" int zb200_lz1_stage_clocks(unsigned long long *out) {
 // no history across chunk starts and no match across a piece end.  It probes no table.
 // CK: the chunk checksums k_member_check reads for the batch's format (ZB_CK_CRC for gzip, ZB_CK_ADLER for
 // zlib, 0 for raw DEFLATE); the other fields of chk are left 0.
+// max_dist: MODE 1's farthest match (2^window_bits).  Its matches reach at most 4 KiB + 2 KiB back (a piece and its
+// pre-seed), so only windows of 4 KiB and less change its parse.
 template <int MODE, int CK>
 __global__ void __launch_bounds__(LZ_THREADS, 3)
     k_lz(const uint8_t *__restrict__ src, const ZbChunkDesc *__restrict__ desc, uint2 *__restrict__ masks,
          uint32_t *__restrict__ recs, uint16_t *__restrict__ hist, ZbChunkCheck *__restrict__ chk,
-         const ZbCrcTables *__restrict__ tabs) {
+         const ZbCrcTables *__restrict__ tabs, uint32_t max_dist) {
   extern __shared__ __align__(128) uint8_t smem[];
   uint8_t *data = smem + LZ_SM_DATA;
   uint16_t *table_all = reinterpret_cast<uint16_t *>(smem + LZ_SM_TABLE);
@@ -404,7 +406,7 @@ __global__ void __launch_bounds__(LZ_THREADS, 3)
           LZ_CLK(LZS_PROBE)
           // a match may not cross the piece end (another warp starts its own parse there)
           const uint32_t limit = p < b1 ? min((uint32_t)ZB_MAX_MATCH, b1 - p) : 0u;
-          if (can && c < p && p - c <= ZB_MAX_DIST && p >= entry && limit >= ZB_MIN_MATCH) {
+          if (can && c < p && p - c <= max_dist && p >= entry && limit >= ZB_MIN_MATCH) {
             // unaligned compare, 8 bytes per step, carrying the upper word of each side; the first step's four words
             // are loaded with the 4-byte check and every step loads the next one's, so a lane waits for one round of
             // shared-memory loads per 8 bytes (4 before)
@@ -775,10 +777,12 @@ __global__ void __launch_bounds__(LZ_THREADS, 2)
       __syncwarp();
     }
 
-    // ---- phase 1: static tables of every segment that precedes some sub-chunk of this chunk ----
+    // ---- phase 1: static tables of every segment that some sub-chunk of this chunk looks up ----
     {
       const uint32_t nseg = (hg + rlen + LZ2_SEG_BYTES - 1) / LZ2_SEG_BYTES;  // segments of the region; the last is never history
-      for (uint32_t sg = (uint32_t)warp; sg + 1 < nseg; sg += ZB_WARPS_PER_CHUNK) {
+      // the first sub-chunk's segment looks back hist_segs segments (fewer under a small window), the others less far
+      const uint32_t seg0 = (hg + hb) / LZ2_SEG_BYTES, sg0 = seg0 > prm.hist_segs ? seg0 - prm.hist_segs : 0u;
+      for (uint32_t sg = sg0 + (uint32_t)warp; sg + 1 < nseg; sg += ZB_WARPS_PER_CHUNK) {
         uint2 *tab = stat + (size_t)sg * LZ2_BUCKETS;
         lz2_clear_table(tab, (1 << LZ2_STATIC_BITS) * 2);
         __syncwarp();
@@ -841,7 +845,7 @@ __global__ void __launch_bounds__(LZ_THREADS, 2)
           P.poff = off0 + p;
           P.q = q;
           P.v = v;
-          P.lim = min(q, (uint32_t)ZB_MAX_DIST);
+          P.lim = min(q, prm.max_dist);
           P.limit = limit;
           P.stop = min(limit, (uint32_t)LZ_LANE_CAP);
           // candidates, nearest first; the level decides how many are looked at:
@@ -1291,7 +1295,9 @@ __global__ void __launch_bounds__(LZ_THREADS, 6)  // 6 CTAs (48 warps) per SM: <
       for (uint32_t i = 0; i < k; i++) h[10 + i] = (uint8_t)(97 + i);
       h[10 + k] = 0;
     } else if (w.data_format == ZB_DF_ZLIB) {
-      h[0] = 0x78; h[1] = 0x01;
+      // CMF: CM 8, CINFO = window_bits - 8 (0x78 for 32 KiB); FLG: FLEVEL 0 and FCHECK, so that CMF FLG is 31 x k
+      const uint32_t cmf = (uint32_t)(__ffs((int)w.max_dist) - 9) << 4 | 8u;
+      h[0] = (uint8_t)cmf; h[1] = (uint8_t)((31u - (cmf << 8) % 31u) % 31u);
       if (w.has_dict) {  // 0x7820 = 31 x 992: FDICT, FLEVEL 0, then the DICTID big-endian
         const uint32_t id = w.dict_id;
         h[1] = 0x20;
@@ -1500,11 +1506,14 @@ static bool zb_is_lz_level(int level) { return level == -1 || level >= 2; }
 // own bucket, the entries of hist_segs preceding segments) and how many of them may pass the 4-byte check
 // (maxcand); `good` keeps its meaning and `lazy` is the one-step lazy threshold.  Effort and compressed
 // size are monotone in the level.
-ZbLz2Params zb_lz2_params(int level) {
+ZbLz2Params zb_lz2_params(int level, uint32_t max_dist) {
   //                                     own hist maxcand good lazy
   static const ZbLz2Params table[10] = {{4, 4, 4, 8, 16}, {4, 4, 4, 8, 16}, {2, 4, 2, 4, 0},  {2, 4, 3, 4, 6},   {3, 4, 3, 4, 8},
                                         {3, 4, 4, 8, 16}, {4, 4, 4, 8, 16}, {4, 4, 6, 8, 32}, {4, 4, 8, 16, 32}, {4, 4, 8, 32, 64}};
-  return table[(level >= 2 && level <= 9) ? level : 6];  // -1 (Default) = level 6
+  ZbLz2Params p = table[(level >= 2 && level <= 9) ? level : 6];  // -1 (Default) = level 6
+  p.hist_segs = std::min(p.hist_segs, (max_dist + LZ2_SEG_BYTES - 1) / LZ2_SEG_BYTES);
+  p.max_dist = max_dist;
+  return p;
 }
 size_t zb_lz2_table_bytes(int *grid_out) {
   int grid = LZ2_CTAS_PER_SM * zb_sm_count();
@@ -1513,7 +1522,7 @@ size_t zb_lz2_table_bytes(int *grid_out) {
 }
 // the k_lz instance for a level's matcher (MODE) and a format's checksum (CK)
 typedef void (*ZbLzKernel)(const uint8_t *, const ZbChunkDesc *, uint2 *, uint32_t *, uint16_t *, ZbChunkCheck *,
-                           const ZbCrcTables *);
+                           const ZbCrcTables *, uint32_t);
 template <int MODE>
 static ZbLzKernel zb_lz_kernel_ck(int ck) {
   return ck == (ZB_CK_CRC | ZB_CK_ADLER) ? k_lz<MODE, ZB_CK_CRC | ZB_CK_ADLER>
@@ -1558,17 +1567,17 @@ cudaError_t zb_launch_lz(const ZbCompressWork &w, cudaStream_t s, bool index_crc
     if ((uint32_t)grid > w.n_chunks) grid = (int)w.n_chunks;
     if (w.strategy == ZB_STRATEGY_FILTERED)
       k_lz2<false, 6><<<grid, LZ_THREADS, LZ2_SM_TOTAL, s>>>(w.src, w.desc, w.masks, w.recs, w.hist, w.chk, w.tabs, w.lz2_tables,
-                                                             w.n_chunks, zb_lz2_params(w.level), nullptr, 0u, 0u);
+                                                             w.n_chunks, zb_lz2_params(w.level, w.max_dist), nullptr, 0u, 0u);
     else if (w.win16)
       k_lz2<true><<<grid, LZ_THREADS, LZ2_SM_TOTAL, s>>>(w.src, w.desc, w.masks, w.recs, w.hist, w.chk, w.tabs, w.lz2_tables,
-                                                         w.n_chunks, zb_lz2_params(w.level), w.win16, w.win_len, w.win_stride);
+                                                         w.n_chunks, zb_lz2_params(w.level, w.max_dist), w.win16, w.win_len, w.win_stride);
     else
       k_lz2<false><<<grid, LZ_THREADS, LZ2_SM_TOTAL, s>>>(w.src, w.desc, w.masks, w.recs, w.hist, w.chk, w.tabs, w.lz2_tables,
-                                                          w.n_chunks, zb_lz2_params(w.level), nullptr, 0u, 0u);
+                                                          w.n_chunks, zb_lz2_params(w.level, w.max_dist), nullptr, 0u, 0u);
   } else {
     const int mode = (w.level == -2 || w.level == 0) ? 0 : w.strategy == ZB_STRATEGY_RLE ? 2 : 1;
     const ZbLzKernel k = zb_lz_kernel(mode, w.data_format, index_crc);
-    k<<<w.n_chunks, LZ_THREADS, LZ_SM_TOTAL, s>>>(w.src, w.desc, w.masks, w.recs, w.hist, w.chk, w.tabs);
+    k<<<w.n_chunks, LZ_THREADS, LZ_SM_TOTAL, s>>>(w.src, w.desc, w.masks, w.recs, w.hist, w.chk, w.tabs, w.max_dist);
   }
   return cudaGetLastError();
 }

@@ -63,6 +63,8 @@ struct ZbCompressWork {
   // ZB_STRATEGY_*, after zb_strategy_level: RLE only at level 1 (k_lz<2>), FILTERED only at the LZ levels (k_lz2<false, 6>),
   // FIXED at any level but 0 (k_huff: stored or fixed blocks); HUFFMAN_ONLY never (it is level -2)
   int strategy;
+  // 2^window_bits (512..32768): no match reaches further back (k_lz<1>, k_lz2), and a zlib header's CINFO states it
+  uint32_t max_dist;
   // A preset dictionary (zb200_compress_batch_dict): has_dict puts FDICT and dict_id in the zlib header.  win16 holds
   // 16 copies of the window W (win_len bytes; win16 256-byte aligned), copy c at
   // win16 + c * win_stride + ZB_WIN16_SLACK + ((c - win_len) & 15), so that W ends at an address that is c modulo 16;
@@ -83,8 +85,11 @@ struct ZbLz2Params {
   uint32_t maxcand;    // candidates per position that may pass the 4-byte check and be extended
   uint32_t good;       // a match this long leaves room for one more candidate only
   uint32_t lazy;       // matches shorter than this yield to a longer match at the next position (0: greedy)
+  uint32_t max_dist;   // candidates at distance 1..max_dist are in the window (ZbCompressWork::max_dist)
 };
-ZbLz2Params zb_lz2_params(int level);
+// The level's effort under a window of max_dist bytes: a preceding segment j (0 = nearest) is looked at only when
+// some of it can lie within max_dist, i.e. 8192 j < max_dist, so hist_segs is at most ceil(max_dist / 8192).
+ZbLz2Params zb_lz2_params(int level, uint32_t max_dist);
 size_t zb_lz2_table_bytes(int *grid_out);
 // index_crc: the chunk checksums also hold the raw CRC-32 whatever the format (a compress-time index needs it)
 cudaError_t zb_launch_lz(const ZbCompressWork &w, cudaStream_t s, bool index_crc = false);
