@@ -173,6 +173,46 @@ int zb200_uncompress_batch_dict(zb200_ctx *ctx, const uint8_t *src_base, const u
                                 const uint64_t *dst_offsets, uint64_t *dst_lens, int *statuses);
 int zb200_decode_begin_dict(zb200_ctx *ctx, const uint8_t *src, size_t len, int data_format, const uint8_t *dict,
                             size_t dict_len, size_t *out_len);
+/* ---- per-member preset dictionaries: a table of k dictionaries, one entry (or none) per member ----
+ * Entry j is dict_base[dict_offsets[j] .. dict_offsets[j + 1]) (dict_offsets has k + 1 entries); member i uses
+ * entry dict_of[i], -1 for none.  Let D be member i's entry (W, DICTID as above) and M its input.  Members may
+ * share an entry: its DICTID is computed and its bytes uploaded once per call.  The *_dict calls are the k = 1
+ * case with every dict_of[i] = 0, and write and decode exactly what these calls do for that table.
+ *  - compress, window_bits 15: a member with a non-empty D is byte for byte zb200_compress_batch_dict(M alone, D);
+ *    one with dict_of[i] == -1 or an empty D is byte for byte zb200_compress_batch(M alone).  A member's bytes do
+ *    not depend on the other members, its position in the batch or how the table is shared.
+ *  - compress, window_bits n in 9..15 (validated as in zb200_compress_batch_window: 8 means 9 for zlib): a member
+ *    without a dictionary is zb200_compress_batch_window(M alone) at n.  A member with D: its blocks are byte for
+ *    byte what a raw compress stream of the same level and window_bits n writes for M after D was written to it and
+ *    sync-flushed; no match reaches more than 2^n bytes back, into M or into W (W stays the last
+ *    min(32768, |D|) bytes of D); a zlib header is CMF (n - 8) << 4 | 8, FLG with FDICT, FLEVEL 0 and FCHECK, then
+ *    the DICTID.  Levels 0, 1 and -2 keep no history: only their header carries D.
+ *  - bound: zb200_compress_bound(len, fmt) + 4 for every zlib member with a non-empty D.
+ *  - decode: a member decodes (output, size, status) exactly as zb200_uncompress_batch_dict / _sizes_dict do with
+ *    its D alone; a member with -1 as zb200_uncompress_batch / _sizes (FDICT: ZB200_ERR_FDICT).  A DICTID that is
+ *    not D's: ZB200_ERR_DICTIONARY.  gzip members and zlib members without FDICT ignore the entry they name;
+ *    DETECT works as with _dict.  A batch in which some member names a non-empty D decodes every member whole, as
+ *    uncompress_batch_dict does.
+ *  - whole-call errors, statuses left alone: ZB200_ERR_ARG for a dict_of outside -1 .. k - 1, dict_offsets that
+ *    decrease, or a null dict_of with n > 0; ZB200_ERR_INVALID_FORMAT for a gzip compress in which a member names
+ *    a non-empty D.
+ *  - limits: windows go to the device with their launch group and their memory is bounded by the groups in flight,
+ *    not by the batch: a group holds one copy of W (|W| rounded up to 16, plus 48 bytes) per (entry, member address
+ *    modulo 16) its members use (decode: per entry), three groups' worth at a time (a decode keeps every group's
+ *    windows, in one launch, only while they fit that much); a decode group holds at most 256 MiB of windows.  The
+ *    DICTIDs of named entries above 256 KiB in all are computed on the device, from uploads of at most 256 MiB of
+ *    consecutive named entries at a time (an entry larger than that alone).  Plus 16 bytes per member. */
+int zb200_compress_batch_dicts(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n,
+                               int level, int data_format, int window_bits,
+                               const uint8_t *dict_base, const uint64_t *dict_offsets, size_t k, const int32_t *dict_of,
+                               uint8_t *dst_base, size_t dst_cap, uint64_t *dst_offsets, int *statuses);
+int zb200_uncompress_sizes_dicts(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n,
+                                 int data_format, const uint8_t *dict_base, const uint64_t *dict_offsets, size_t k,
+                                 const int32_t *dict_of, uint64_t *sizes, int *statuses);
+int zb200_uncompress_batch_dicts(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n,
+                                 int data_format, const uint8_t *dict_base, const uint64_t *dict_offsets, size_t k,
+                                 const int32_t *dict_of, uint8_t *dst_base, const uint64_t *dst_offsets,
+                                 uint64_t *dst_lens, int *statuses);
 
 /* crc32 (kind 0) or adler32 (kind 1) of every input */
 int zb200_checksum_batch(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n,

@@ -331,6 +331,83 @@ inline std::vector<std::string> compressBatch(const std::vector<std::string> &it
   return res;
 }
 
+namespace detail {
+// a dictionary table (include/zippy_b200.h "per-member preset dictionaries") as base + k + 1 offsets
+inline std::string packDicts(const std::vector<std::string> &dicts, std::vector<uint64_t> &offs) {
+  std::string base;
+  offs.assign(dicts.size() + 1, 0);
+  for (size_t j = 0; j < dicts.size(); j++) {
+    base += dicts[j];
+    offs[j + 1] = base.size();
+  }
+  return base;
+}
+}  // namespace detail
+
+// Per-member preset dictionaries at zlib's window size (zb200_compress_batch_dicts): item i is compressed against
+// dicts[dictOf[i]], or without a dictionary for dictOf[i] == -1; windowBits 9..15 (8 for dfZlib means 9).
+inline std::vector<std::string> compressBatch(const std::vector<std::string> &items, int level,
+                                              CompressedDataFormat dataFormat, int windowBits,
+                                              const std::vector<std::string> &dicts, const std::vector<int32_t> &dictOf) {
+  if (dictOf.size() != items.size()) throw ZippyError(ZB200_ERR_ARG, "dictOf needs one entry per item");
+  std::string base;
+  std::vector<uint64_t> offs(items.size() + 1, 0), out_offs(items.size() + 1, 0), doffs;
+  size_t bound = 64;
+  for (size_t i = 0; i < items.size(); i++) {
+    base += items[i];
+    offs[i + 1] = base.size();
+    bound += zb200_compress_bound(items[i].size(), dataFormat) + 4 + 64;
+  }
+  const std::string dbase = detail::packDicts(dicts, doffs);
+  std::string out(bound, '\0');
+  std::vector<int> st(items.size() + 1, 0);
+  uint8_t dummy = 0;
+  detail::check(zb200_compress_batch_dicts(detail::ctx(), items.empty() ? &dummy : detail::u8(base), offs.data(),
+                                           items.size(), level, dataFormat, windowBits,
+                                           dbase.empty() ? &dummy : detail::u8(dbase), doffs.data(), dicts.size(),
+                                           dictOf.data(), reinterpret_cast<uint8_t *>(&out[0]), out.size(),
+                                           out_offs.data(), st.data()));
+  std::vector<std::string> res;
+  for (size_t i = 0; i < items.size(); i++) res.emplace_back(out.substr(out_offs[i], out_offs[i + 1] - out_offs[i]));
+  return res;
+}
+
+// Members decoded against per-member preset dictionaries (zb200_uncompress_sizes_dicts, then
+// zb200_uncompress_batch_dicts): member i against dicts[dictOf[i]], or none for -1.  A member that does not decode
+// throws its status.
+inline std::vector<std::string> uncompressBatch(const std::vector<std::string> &members, CompressedDataFormat dataFormat,
+                                                const std::vector<std::string> &dicts,
+                                                const std::vector<int32_t> &dictOf) {
+  if (dictOf.size() != members.size()) throw ZippyError(ZB200_ERR_ARG, "dictOf needs one entry per member");
+  const size_t n = members.size();
+  std::string base;
+  std::vector<uint64_t> offs(n + 1, 0), doffs, sizes(n + 1, 0), dst_offs(n + 1, 0), lens(n + 1, 0);
+  for (size_t i = 0; i < n; i++) {
+    base += members[i];
+    offs[i + 1] = base.size();
+  }
+  const std::string dbase = detail::packDicts(dicts, doffs);
+  std::vector<int> st(n + 1, 0);
+  uint8_t dummy = 0;
+  const uint8_t *src = n ? detail::u8(base) : &dummy, *db = dbase.empty() ? &dummy : detail::u8(dbase);
+  detail::check(zb200_uncompress_sizes_dicts(detail::ctx(), src, offs.data(), n, dataFormat, db, doffs.data(),
+                                             dicts.size(), dictOf.data(), sizes.data(), st.data()));
+  for (size_t i = 0; i < n; i++) {
+    detail::check(st[i]);
+    dst_offs[i + 1] = dst_offs[i] + sizes[i];
+  }
+  std::string out(dst_offs[n] + 64, '\0');
+  detail::check(zb200_uncompress_batch_dicts(detail::ctx(), src, offs.data(), n, dataFormat, db, doffs.data(),
+                                             dicts.size(), dictOf.data(), reinterpret_cast<uint8_t *>(&out[0]),
+                                             dst_offs.data(), lens.data(), st.data()));
+  std::vector<std::string> res;
+  for (size_t i = 0; i < n; i++) {
+    detail::check(st[i]);
+    res.emplace_back(out.substr(dst_offs[i], lens[i]));
+  }
+  return res;
+}
+
 // One member compressed from input that arrives piece by piece (zb200_compress_stream_*, no reference
 // counterpart): what write() and finish() return, concatenated, is the member compressBatch writes for the whole
 // input with the same FNAME length.  Small writes are gathered and return "".  fnameLen < 0 with gzip draws the

@@ -298,6 +298,76 @@ proc compressBatch*(items: openArray[string], level = DefaultCompression,
   for i in 0 ..< items.len:
     result.add dst[outOffs[i].int ..< outOffs[i + 1].int]
 
+# ---- per-member preset dictionaries (include/zippy_b200.h): item i against dicts[dictOf[i]], -1 for none ----
+proc zb200_compress_batch_dicts(ctx: Zb200Ctx, srcBase: pointer, srcOffsets: ptr uint64, n: csize_t,
+                                level, dataFormat, windowBits: cint, dictBase: pointer, dictOffsets: ptr uint64,
+                                k: csize_t, dictOf: ptr int32, dstBase: pointer, dstCap: csize_t,
+                                dstOffsets: ptr uint64, statuses: ptr cint): cint {.importc, cdecl, dynlib: lib.}
+proc zb200_uncompress_sizes_dicts(ctx: Zb200Ctx, srcBase: pointer, srcOffsets: ptr uint64, n: csize_t,
+                                  dataFormat: cint, dictBase: pointer, dictOffsets: ptr uint64, k: csize_t,
+                                  dictOf: ptr int32, sizes: ptr uint64, statuses: ptr cint): cint {.importc, cdecl, dynlib: lib.}
+proc zb200_uncompress_batch_dicts(ctx: Zb200Ctx, srcBase: pointer, srcOffsets: ptr uint64, n: csize_t,
+                                  dataFormat: cint, dictBase: pointer, dictOffsets: ptr uint64, k: csize_t,
+                                  dictOf: ptr int32, dstBase: pointer, dstOffsets: ptr uint64, dstLens: ptr uint64,
+                                  statuses: ptr cint): cint {.importc, cdecl, dynlib: lib.}
+
+proc packBatch(items: openArray[string], base: var string, offs: var seq[uint64]) =
+  offs = newSeq[uint64](items.len + 1)
+  for i, item in items:
+    base.add item
+    offs[i + 1] = base.len.uint64
+  if base.len == 0: base.add '\0'
+
+proc compressBatch*(items: openArray[string], level: int, dataFormat: CompressedDataFormat, windowBits: int,
+                    dicts: openArray[string], dictOf: openArray[int32]): seq[string] {.raises: [ZippyError].} =
+  if dictOf.len != items.len: raise newException(ZippyError, "dictOf needs one entry per item")
+  var
+    base, dbase: string
+    offs, doffs: seq[uint64]
+    outOffs = newSeq[uint64](items.len + 1)
+    dof = @dictOf
+    bound = 64
+  packBatch(items, base, offs)
+  packBatch(dicts, dbase, doffs)
+  for item in items:
+    bound += zb200_compress_bound(item.len.csize_t, dataFormat.cint).int + 4 + 64
+  if dof.len == 0: dof.add -1
+  var dst = newString(bound)
+  check zb200_compress_batch_dicts(getCtx(), base[0].addr, offs[0].addr, items.len.csize_t, level.cint,
+                                   dataFormat.cint, windowBits.cint, dbase[0].addr, doffs[0].addr,
+                                   dicts.len.csize_t, dof[0].addr, dst[0].addr, dst.len.csize_t, outOffs[0].addr, nil)
+  for i in 0 ..< items.len:
+    result.add dst[outOffs[i].int ..< outOffs[i + 1].int]
+
+proc uncompressBatch*(members: openArray[string], dataFormat: CompressedDataFormat, dicts: openArray[string],
+                      dictOf: openArray[int32]): seq[string] {.raises: [ZippyError].} =
+  ## a member that does not decode raises its status
+  if dictOf.len != members.len: raise newException(ZippyError, "dictOf needs one entry per member")
+  var
+    base, dbase: string
+    offs, doffs: seq[uint64]
+    dof = @dictOf
+    sizes = newSeq[uint64](members.len + 1)
+    dofs = newSeq[uint64](members.len + 1)
+    lens = newSeq[uint64](members.len + 1)
+    st = newSeq[cint](members.len + 1)
+  packBatch(members, base, offs)
+  packBatch(dicts, dbase, doffs)
+  if dof.len == 0: dof.add -1
+  check zb200_uncompress_sizes_dicts(getCtx(), base[0].addr, offs[0].addr, members.len.csize_t, dataFormat.cint,
+                                     dbase[0].addr, doffs[0].addr, dicts.len.csize_t, dof[0].addr, sizes[0].addr,
+                                     st[0].addr)
+  for i in 0 ..< members.len:
+    check st[i]
+    dofs[i + 1] = dofs[i] + sizes[i]
+  var dst = newString(dofs[members.len].int + 64)
+  check zb200_uncompress_batch_dicts(getCtx(), base[0].addr, offs[0].addr, members.len.csize_t, dataFormat.cint,
+                                     dbase[0].addr, doffs[0].addr, dicts.len.csize_t, dof[0].addr, dst[0].addr,
+                                     dofs[0].addr, lens[0].addr, st[0].addr)
+  for i in 0 ..< members.len:
+    check st[i]
+    result.add dst[dofs[i].int ..< (dofs[i] + lens[i]).int]
+
 proc zb200_inflate_batch_crc32(ctx: Zb200Ctx, srcBase: pointer, srcOffsets: ptr uint64, n: csize_t,
                                dstBase: pointer, dstOffsets: ptr uint64, dstLens: ptr uint64,
                                crcs: ptr uint32, statuses: ptr cint): cint {.importc, cdecl, dynlib: lib.}

@@ -69,6 +69,36 @@ def _dict(dictionary):
     return d if d is not None and d.size else None
 
 
+def _dict_table(dictionaries, n):
+    """`dictionaries=`: n bytes-like or None, one per item -> (base uint8, offsets uint64[k + 1], dict_of int32[n]),
+    the table of the *_dicts calls.  Items that pass the same object share one entry; None and an empty dictionary
+    name none (-1)."""
+    if len(dictionaries) != n:
+        raise ZippyError(22, "dictionaries= needs one entry (bytes-like or None) per item")
+    entry, parts = {}, []
+    dict_of = np.full(max(n, 1), -1, dtype=np.int32)
+    for i, d in enumerate(dictionaries):
+        if d is None:
+            continue
+        j = entry.get(id(d))
+        if j is None:
+            a = _as_u8(d)
+            j = entry[id(d)] = len(parts) if a.size else -1
+            if a.size:
+                parts.append(a)
+        dict_of[i] = j
+    offs = np.zeros(len(parts) + 1, dtype=np.uint64)
+    np.cumsum([p.size for p in parts], out=offs[1:])
+    base = np.concatenate(parts) if parts else np.zeros(1, np.uint8)
+    return base, offs, dict_of
+
+
+def _one_table(dictionary, dictionaries):
+    """dictionary= and dictionaries= exclude each other."""
+    if dictionary is not None and dictionaries is not None:
+        raise ZippyError(22, "dictionary= and dictionaries= are not combined")
+
+
 def _params_alone(strategy, window_bits=15, dictionary=None, index_span=None):
     """True for a strategy other than the default or a window other than 15 (the _window calls); either takes no
     dictionary and no compress-time index."""
@@ -125,12 +155,14 @@ class Context:
 
     # ---- batches over host buffers -------------------------------------------------
     def compress_batch(self, base, offsets, level=DefaultCompression, dataFormat=dfGzip, fname_lens=None,
-                       dictionary=None, index_span=None, strategy=StrategyDefault, window_bits=15):
+                       dictionary=None, index_span=None, strategy=StrategyDefault, window_bits=15, dictionaries=None):
         """-> (out uint8 array, out_offsets uint64[n+1]).  fname_lens: per-input gzip FNAME letters (0..25).
         strategy: zlib's compression strategy (Strategy*; zb200_compress_batch_window; no dictionary or index).
         window_bits: zlib's window size, 9..15 (8 for zlib: 9); no match reaches more than 2^window_bits back
         (zb200_compress_batch_window; no dictionary or index).
         dictionary: a preset dictionary shared by every input (zlib / raw only; zb200_compress_batch_dict).
+        dictionaries: one preset dictionary (bytes-like or None) per input, with any window_bits (zlib / raw only;
+        zb200_compress_batch_dicts; no strategy or index); inputs that pass the same object share it.
         index_span: also write each member's Index with this span (zb200_compress_batch_index; no dictionary):
         -> (out, out_offsets, list of Index)."""
         L = _native.lib()
@@ -139,9 +171,24 @@ class Context:
         n = len(offsets) - 1
         bound = sum(L.zb200_compress_bound(int(offsets[i + 1] - offsets[i]), dataFormat) for i in range(n)) \
             if n <= 4096 else int(L.zb200_compress_bound(int(offsets[-1] - offsets[0]), dataFormat)) + 64 * n
-        out = np.empty(int(bound) + (4 * n if _dict(dictionary) is not None else 0) + 64, dtype=np.uint8)
+        _one_table(dictionary, dictionaries)
+        with_dicts = _dict(dictionary) is not None or dictionaries is not None
+        out = np.empty(int(bound) + (4 * n if with_dicts else 0) + 64, dtype=np.uint8)
         out_offs = np.zeros(n + 1, dtype=np.uint64)
         st = np.zeros(max(n, 1), dtype=np.int32)
+        if dictionaries is not None:
+            if strategy != StrategyDefault:
+                raise ZippyError(22, "a compression strategy is not combined with a dictionary")
+            if index_span is not None:
+                raise ZippyError(22, "a compress-time index is not written with a dictionary")
+            if fname_lens is not None:
+                raise ZippyError(22, "fname_lens is not combined with dictionaries")
+            db, do, dof = _dict_table(dictionaries, n)
+            _check(self._h, L.zb200_compress_batch_dicts(self._h, base.ctypes.data, offsets.ctypes.data, n, level,
+                                                          dataFormat, window_bits, db.ctypes.data, do.ctypes.data,
+                                                          do.size - 1, dof.ctypes.data, out.ctypes.data, out.size,
+                                                          out_offs.ctypes.data, st.ctypes.data))
+            return out[:int(out_offs[n])], out_offs
         d = _dict(dictionary)
         if _params_alone(strategy, window_bits, d, index_span):
             fl = np.ascontiguousarray(fname_lens, dtype=np.uint8) if fname_lens is not None else None
@@ -175,13 +222,27 @@ class Context:
         _check(self._h, rc)
         return out[:int(out_offs[n])], out_offs
 
-    def uncompressed_sizes(self, base, offsets, dataFormat=dfDetect, dictionary=None):
+    def uncompressed_sizes(self, base, offsets, dataFormat=dfDetect, dictionary=None, dictionaries=None):
+        """dictionaries: one preset dictionary (bytes-like or None) per member (zb200_uncompress_sizes_dicts)."""
+        _one_table(dictionary, dictionaries)
+        offsets = np.ascontiguousarray(offsets, dtype=np.uint64)
+        table = _dict_table(dictionaries, len(offsets) - 1) if dictionaries is not None else None
+        return self._sizes(base, offsets, dataFormat, dictionary, table)
+
+    def _sizes(self, base, offsets, dataFormat, dictionary, table):
+        """uncompressed_sizes with the dictionary table (_dict_table) already built, or None."""
         L = _native.lib()
         base = _as_u8(base)
         offsets = np.ascontiguousarray(offsets, dtype=np.uint64)
         n = len(offsets) - 1
         sizes = np.zeros(max(n, 1), dtype=np.uint64)
         st = np.zeros(max(n, 1), dtype=np.int32)
+        if table is not None:
+            db, do, dof = table
+            _check(self._h, L.zb200_uncompress_sizes_dicts(self._h, base.ctypes.data, offsets.ctypes.data, n,
+                                                            dataFormat, db.ctypes.data, do.ctypes.data, do.size - 1,
+                                                            dof.ctypes.data, sizes.ctypes.data, st.ctypes.data))
+            return sizes[:n], st[:n]
         d = _dict(dictionary)
         if d is not None:
             _check(self._h, L.zb200_uncompress_sizes_dict(self._h, base.ctypes.data, offsets.ctypes.data, n, dataFormat,
@@ -191,17 +252,21 @@ class Context:
                                                   sizes.ctypes.data, st.ctypes.data))
         return sizes[:n], st[:n]
 
-    def uncompress_batch(self, base, offsets, dataFormat=dfDetect, max_total=None, sizes=None, dictionary=None):
+    def uncompress_batch(self, base, offsets, dataFormat=dfDetect, max_total=None, sizes=None, dictionary=None,
+                         dictionaries=None):
         """-> (out uint8 array, out_offsets uint64[n+1], out_lens uint64[n], statuses int32[n]).
         `sizes`: uncompressed sizes known to the caller (a container's directory); skips the sizing pass.
-        `dictionary`: a preset dictionary for every raw member and every zlib member with FDICT."""
+        `dictionary`: a preset dictionary for every raw member and every zlib member with FDICT.
+        `dictionaries`: one such dictionary (bytes-like or None) per member (zb200_uncompress_batch_dicts)."""
         L = _native.lib()
         base = _as_u8(base)
         offsets = np.ascontiguousarray(offsets, dtype=np.uint64)
         n = len(offsets) - 1
+        _one_table(dictionary, dictionaries)
         d = _dict(dictionary)
+        table = _dict_table(dictionaries, n) if dictionaries is not None else None   # built once for both calls
         if sizes is None:
-            sizes, st0 = self.uncompressed_sizes(base, offsets, dataFormat, dictionary=d)
+            sizes, st0 = self._sizes(base, offsets, dataFormat, d, table)
         else:
             sizes, st0 = np.ascontiguousarray(sizes, dtype=np.uint64), np.zeros(n, dtype=np.int32)
         sizes = np.where(st0 == 0, sizes, 0).astype(np.uint64)
@@ -216,7 +281,13 @@ class Context:
         out = np.empty(int(dst_offs[n]) + 64, dtype=np.uint8)
         lens = np.zeros(max(n, 1), dtype=np.uint64)
         st = np.zeros(max(n, 1), dtype=np.int32)
-        if d is None:
+        if table is not None:
+            db, do, dof = table
+            _check(self._h, L.zb200_uncompress_batch_dicts(self._h, base.ctypes.data, offsets.ctypes.data, n,
+                                                            dataFormat, db.ctypes.data, do.ctypes.data, do.size - 1,
+                                                            dof.ctypes.data, out.ctypes.data, dst_offs.ctypes.data,
+                                                            lens.ctypes.data, st.ctypes.data))
+        elif d is None:
             _check(self._h, L.zb200_uncompress_batch(self._h, base.ctypes.data, offsets.ctypes.data, n, dataFormat,
                                                       out.ctypes.data, dst_offs.ctypes.data, lens.ctypes.data,
                                                       st.ctypes.data))
@@ -226,10 +297,11 @@ class Context:
                                                            lens.ctypes.data, st.ctypes.data))
         st = np.where(st0 != 0, st0, st[:n]).astype(np.int32)
         out, dst_offs = self._redo_too_small(base, offsets, dataFormat, out[:int(dst_offs[n])], dst_offs, lens[:n], st,
-                                             dictionary=d)
+                                             dictionary=d, dictionaries=dictionaries)
         return out, dst_offs, lens[:n], st
 
-    def _redo_too_small(self, base, offsets, dataFormat, out, dst_offs, lens, st, crcs=None, dictionary=None):
+    def _redo_too_small(self, base, offsets, dataFormat, out, dst_offs, lens, st, crcs=None, dictionary=None,
+                        dictionaries=None):
         """A size claim (gzip ISIZE, a container's directory) understated the content (status 19): the reference
         inflates anyway and lets its checksum / size checks decide (gzip.nim:80-88) -- redo those members one by
         one.  lens / st / crcs are updated in place; -> (out, dst_offs) with the redone outputs appended."""
@@ -241,7 +313,8 @@ class Context:
         dst_offs = dst_offs.copy()
         for i in small:
             try:
-                b = self.decode_one(base[int(offsets[i]):int(offsets[i + 1])], dataFormat, dictionary=dictionary)
+                b = self.decode_one(base[int(offsets[i]):int(offsets[i + 1])], dataFormat,
+                                    dictionary=dictionary if dictionaries is None else dictionaries[i])
                 st[i] = 0
                 dst_offs[i] = end          # appended behind the slots; callers use out[off : off + len]
                 lens[i] = len(b)
@@ -817,27 +890,31 @@ def inflate(src, pos=0):
 
 
 def compress_batch(items, level=DefaultCompression, dataFormat=dfGzip, fname_lens=None, dictionary=None,
-                   strategy=StrategyDefault, window_bits=15):
-    """list of bytes -> list of bytes (one zippy.compress per item, one GPU launch sequence)."""
+                   strategy=StrategyDefault, window_bits=15, dictionaries=None):
+    """list of bytes -> list of bytes (one zippy.compress per item, one GPU launch sequence).  dictionaries: one
+    preset dictionary (bytes-like or None) per item, with any window_bits (zb200_compress_batch_dicts)."""
     base, offs = _pack(items)
     out, oo = default_context().compress_batch(base, offs, level, dataFormat, fname_lens, dictionary=dictionary,
-                                               strategy=strategy, window_bits=window_bits)
+                                               strategy=strategy, window_bits=window_bits, dictionaries=dictionaries)
     return [out[int(oo[i]):int(oo[i + 1])].tobytes() for i in range(len(items))]
 
 
-def uncompress_batch(items, dataFormat=dfDetect, dictionary=None):
-    """list of bytes -> list of (bytes | ZippyError)."""
+def uncompress_batch(items, dataFormat=dfDetect, dictionary=None, dictionaries=None):
+    """list of bytes -> list of (bytes | ZippyError).  dictionaries: one preset dictionary (bytes-like or None) per
+    item (zb200_uncompress_batch_dicts)."""
     base, offs = _pack(items)
-    out, do, lens, st = default_context().uncompress_batch(base, offs, dataFormat, dictionary=dictionary)
+    out, do, lens, st = default_context().uncompress_batch(base, offs, dataFormat, dictionary=dictionary,
+                                                           dictionaries=dictionaries)
     res = []
     for i in range(len(items)):
         res.append(ZippyError(int(st[i])) if st[i] != 0 else out[int(do[i]):int(do[i]) + int(lens[i])].tobytes())
     return res
 
 
-def uncompressed_sizes(items, dataFormat=dfDetect, dictionary=None):
+def uncompressed_sizes(items, dataFormat=dfDetect, dictionary=None, dictionaries=None):
     base, offs = _pack(items)
-    return default_context().uncompressed_sizes(base, offs, dataFormat, dictionary=dictionary)
+    return default_context().uncompressed_sizes(base, offs, dataFormat, dictionary=dictionary,
+                                                dictionaries=dictionaries)
 
 
 def checksum_batch(items, kind="crc32"):

@@ -64,6 +64,12 @@ SYMBOLS = {
                                             c_intp]),
     "zb200_uncompress_batch_dict": (c_int, [ctypes.c_void_p, c_u8p, c_u64p, c_size_t, c_int, c_u8p, c_size_t, c_u8p,
                                             c_u64p, c_u64p, c_intp]),
+    "zb200_compress_batch_dicts": (c_int, [ctypes.c_void_p, c_u8p, c_u64p, c_size_t, c_int, c_int, c_int, c_u8p, c_u64p,
+                                           c_size_t, c_intp, c_u8p, c_size_t, c_u64p, c_intp]),
+    "zb200_uncompress_sizes_dicts": (c_int, [ctypes.c_void_p, c_u8p, c_u64p, c_size_t, c_int, c_u8p, c_u64p, c_size_t,
+                                             c_intp, c_u64p, c_intp]),
+    "zb200_uncompress_batch_dicts": (c_int, [ctypes.c_void_p, c_u8p, c_u64p, c_size_t, c_int, c_u8p, c_u64p, c_size_t,
+                                             c_intp, c_u8p, c_u64p, c_u64p, c_intp]),
     "zb200_decode_begin_dict": (c_int, [ctypes.c_void_p, c_u8p, c_size_t, c_int, c_u8p, c_size_t,
                                         ctypes.POINTER(c_size_t)]),
     "zb200_compress_batch_device": (c_int, [ctypes.c_void_p, c_u8p, c_u64p, c_size_t, c_int, c_int, c_u8p, c_u8p,

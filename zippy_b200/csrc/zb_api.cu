@@ -20,6 +20,7 @@
 #include <memory>
 #include <mutex>
 #include <thread>
+#include <unordered_map>
 #include <string>
 #include <vector>
 
@@ -205,11 +206,17 @@ struct zb200_ctx {
   DevBuf cix_rec, cix_crc, cix_first, cix_out;  // a compress-time index: ZbIndexWork's arrays
   uint64_t index_group_bytes = kDstreamMaxOut;  // output budget of one extraction launch group (env ZB200_INDEX_GROUP_BYTES)
   bool index_log = false;            // env ZB200_INDEX_LOG: one stderr line per extraction launch group
-  // the preset dictionary of the *_dict call in progress (DictScope): its window W on the device, once as is
-  // (k_inflate) and once as the 16 alignment copies k_lz2 stages from (ZbCompressWork::win16); dict_on is false
-  // outside such a call, so every other call runs exactly as without dictionaries
-  DevBuf dict_win, dict_win16;
-  uint32_t dict_len = 0, dict_id = 0;
+  // the dictionary table of the *_dict / *_dicts call in progress (DictScope, the caller's dict_base / dict_offsets):
+  // dict_win holds the windows of the launch groups in flight (DictWindows), dict_md the ZbMemberDict per member.
+  // dict_member / dict_entry: per member of the call, its ZbMemberDict (wend set by DictWindows::plan) and its table
+  // entry (-1: none, or an empty one).  dict_on is false outside such a call, and in a call where no member names a
+  // non-empty dictionary: every such call runs exactly as without them
+  DevBuf dict_win, dict_md;
+  std::vector<ZbMemberDict> dict_member;
+  std::vector<int32_t> dict_entry;
+  const uint8_t *dict_base = nullptr;
+  const uint64_t *dict_offs = nullptr;
+  size_t dict_k = 0;
   bool dict_on = false;
   uint64_t pending_skip = 0;         // zb200_decode_begin_dict: output bytes in front of the result (the window)
   cudaEvent_t ev[10] = {};
@@ -508,37 +515,172 @@ uint32_t host_adler32(const uint8_t *p, size_t n) {
   return (uint32_t)(b << 16 | a);
 }
 
-// A *_dict call's dictionary D: the window W (the last min(32768, |D|) bytes) is uploaded once for the call -- as
-// is for the decode calls, as the 16 copies of ZbCompressWork::win16 for an LZ-level compress, not at all for
-// compress at levels 0 / 1 / -2 (only the header carries D) -- and its DICTID is the Adler-32 of all of D.  An empty D leaves
-// the ctx as it is (the call is the one without a dictionary).  The destructor turns the dictionary off again.
+int checksum_device_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint64_t *src_offsets, size_t n, int kind,
+                           uint32_t *out);
+
+// A call's dictionary table (zb200_*_dicts; the *_dict calls are its k = 1 case with every member naming entry 0, of
+// == null): entry j is base[offs[j] .. offs[j + 1]), member i names of[i] in -1 .. k - 1.  ZB200_ERR_ARG for a name
+// out of range, offsets that decrease, or bytes without a base; *any: some member names a non-empty entry.
+static int check_dicts(const uint8_t *base, const uint64_t *offs, size_t k, const int32_t *of, size_t n, bool &any) {
+  any = false;
+  if (k && !offs) return ZB200_ERR_ARG;
+  for (size_t j = 0; j < k; j++)
+    if (offs[j + 1] < offs[j]) return ZB200_ERR_ARG;
+  if (!of) return n && k ? ZB200_ERR_ARG : ZB200_OK;   // (no table: the calls without dictionaries)
+  for (size_t i = 0; i < n; i++) {
+    if (of[i] < -1 || of[i] >= (int64_t)k) return ZB200_ERR_ARG;
+    any = any || (of[i] >= 0 && offs[of[i] + 1] > offs[of[i]]);
+  }
+  if (any && !base) return ZB200_ERR_ARG;
+  return ZB200_OK;
+}
+
+// Above this many bytes of named dictionaries the DICTIDs come from the batched Adler-32 on the device, below it from
+// a host loop.  The device pass uploads runs of consecutive named entries, at most kDictSlabBytes at a time (an entry
+// larger than that alone), into dict_win before any window needs it.
+constexpr uint64_t kDictHostAdlerBytes = 256u << 10;
+constexpr uint64_t kDictSlabBytes = 256ull << 20;
+
+// A call's dictionary table (check_dicts has passed).  Every entry that a member names and that is not empty gets its
+// DICTID (the Adler-32 of all of it) once; each member gets its ZbMemberDict in ctx->dict_member without a window
+// (DictWindows places the windows launch group by launch group).  A table no member names non-empty leaves the ctx
+// as it is (the call is the one without dictionaries).  The destructor turns the table off again.
 struct DictScope {
   zb200_ctx *ctx;
   explicit DictScope(zb200_ctx *c) : ctx(c) {}
-  // lz_compress: the call runs k_lz2 (the 16 copies); decode calls need W as is, compress at levels 0 / 1 / -2 neither
-  int set(const uint8_t *dict, size_t dict_len, bool lz_compress = false) {
-    if (!dict_len) return ZB200_OK;
+  int set(const uint8_t *base, const uint64_t *offs, size_t k, const int32_t *of, size_t n) {
     zb200_ctx *ctx = this->ctx;   // (CK / ENSURE)
-    const uint32_t wl = (uint32_t)std::min<size_t>(dict_len, 32768);
-    const uint8_t *w = dict + (dict_len - wl);
-    if (lz_compress) {
-      const uint32_t stride = zb_win16_stride(wl);
-      std::vector<uint8_t> h16((size_t)16 * stride, 0);
-      for (uint32_t c = 0; c < 16; c++) memcpy(h16.data() + (size_t)c * stride + ZB_WIN16_SLACK + ((c - wl) & 15u), w, wl);
-      ENSURE(ctx->dict_win16, h16.size() + 64);
-      CK(cudaMemcpyAsync(ctx->dict_win16.p, h16.data(), h16.size(), cudaMemcpyHostToDevice, ctx->stream));
-      CK(cudaStreamSynchronize(ctx->stream));  // the host copies go out of scope
-    } else {
-      ENSURE(ctx->dict_win, wl + 64);
-      CK(cudaMemcpyAsync(ctx->dict_win.p, w, wl, cudaMemcpyHostToDevice, ctx->stream));
-      CK(cudaStreamSynchronize(ctx->stream));
+    ctx->dict_entry.assign(n, -1);
+    uint64_t named = 0;
+    std::vector<uint8_t> is_named(k, 0);
+    bool any = false;
+    for (size_t i = 0; i < n; i++) {
+      const int32_t j = of ? of[i] : 0;
+      if (j < 0 || offs[j + 1] == offs[j]) continue;
+      ctx->dict_entry[i] = j;
+      if (!is_named[j]) named += offs[j + 1] - offs[j];
+      is_named[j] = 1;
+      any = true;
     }
-    ctx->dict_len = wl;
-    ctx->dict_id = host_adler32(dict, dict_len);
+    if (!any) return ZB200_OK;
+    auto len = [&](size_t j) { return offs[j + 1] - offs[j]; };
+    std::vector<uint32_t> ids(k, 0);
+    if (named > kDictHostAdlerBytes) {
+      for (size_t ja = 0; ja < k;) {
+        if (!is_named[ja]) {
+          ja++;
+          continue;
+        }
+        size_t jb = ja + 1;
+        uint64_t bytes = len(ja);
+        while (jb < k && is_named[jb] && bytes + len(jb) <= kDictSlabBytes) bytes += len(jb++);
+        std::vector<uint64_t> rel(jb - ja + 1);
+        for (size_t j = ja; j <= jb; j++) rel[j - ja] = offs[j] - offs[ja];
+        ENSURE(ctx->dict_win, (size_t)bytes + 64);
+        CK(cudaMemcpyAsync(ctx->dict_win.p, base + offs[ja], (size_t)bytes, cudaMemcpyHostToDevice, ctx->stream));
+        if (int rc = checksum_device_locked(ctx, (const uint8_t *)ctx->dict_win.p, rel.data(), jb - ja, 1, ids.data() + ja))
+          return rc;
+        ja = jb;
+      }
+    } else {
+      for (size_t j = 0; j < k; j++)
+        if (is_named[j]) ids[j] = host_adler32(base + offs[j], (size_t)len(j));
+    }
+    ctx->dict_member.assign(n, ZbMemberDict{nullptr, 0u, 0u});
+    for (size_t i = 0; i < n; i++) {
+      const int32_t j = ctx->dict_entry[i];
+      if (j < 0) continue;
+      ctx->dict_member[i].win_len = (uint32_t)std::min<uint64_t>(len((size_t)j), 32768);
+      ctx->dict_member[i].dict_id = ids[(size_t)j];
+    }
+    ctx->dict_base = base;
+    ctx->dict_offs = offs;
+    ctx->dict_k = k;
     ctx->dict_on = true;
     return ZB200_OK;
   }
   ~DictScope() { ctx->dict_on = false; }
+};
+
+// The windows of the call's members, launch group by launch group, so that device memory for windows is bounded by
+// the groups in flight and not by the batch.  Group g (members [gb[g], gb[g + 1])) gets slot g % slots of
+// ctx->dict_win: one copy of W per (entry, class) its members use, class being the member's first-chunk address
+// modulo 16 for k_lz2 (stage_dict_chunk needs W to end at an address congruent to it) and 0 for k_inflate, each copy
+// zb_win_stride(|W|) bytes with W ending at an address congruent to its class.  plan() sizes the slots and sets every
+// member's ZbMemberDict::wend in ctx->dict_member; upload(g) packs the group's windows on the host and copies them into
+// its slot on a stream, which the caller orders after the last reader of the slot's previous group.
+constexpr uint64_t kDictGroupWindowBytes = 256ull << 20;   // a decode group's windows (uncompress_batch_host)
+constexpr size_t kDictSlots = 3;
+struct DictWindows {
+  struct Copy {
+    int32_t entry;
+    uint64_t end;   // of W in the slot
+  };
+  std::vector<size_t> gb, c0;   // per group: members, first copy
+  std::vector<Copy> copies;
+  std::vector<uint64_t> bytes;  // per group
+  std::vector<uint8_t> host;
+  uint64_t slot_cap = 0;
+  size_t slots = 1;
+
+  std::vector<uint64_t> end_of;   // per member: W's end in its group's slot
+
+  // cls: per member (null: 0).  nslots: slots in ctx->dict_win (place(), at most one per group)
+  int plan(zb200_ctx *ctx, const std::vector<size_t> &groups, const uint8_t *cls, size_t nslots) {
+    layout(ctx, groups, cls);
+    return place(ctx, nslots);
+  }
+  void layout(zb200_ctx *ctx, const std::vector<size_t> &groups, const uint8_t *cls) {
+    gb = groups;
+    const size_t ng = gb.size() - 1;
+    c0.assign(1, 0);
+    bytes.clear();
+    copies.clear();
+    end_of.assign(ctx->dict_member.size(), 0);
+    std::unordered_map<uint64_t, uint64_t> seen;
+    for (size_t g = 0; g < ng; g++) {
+      seen.clear();
+      uint64_t b = 0;
+      for (size_t i = gb[g]; i < gb[g + 1]; i++) {
+        const int32_t j = ctx->dict_entry[i];
+        if (j < 0) continue;
+        const uint32_t c = cls ? cls[i] : 0u, wl = ctx->dict_member[i].win_len;
+        auto it = seen.find((uint64_t)j * 16u + c);
+        if (it == seen.end()) {
+          const uint64_t end = b + ZB_WIN_SLACK + ((c - wl) & 15u) + wl;
+          copies.push_back(Copy{j, end});
+          b += zb_win_stride(wl);
+          it = seen.emplace((uint64_t)j * 16u + c, end).first;
+        }
+        end_of[i] = it->second;
+      }
+      bytes.push_back(b);
+      c0.push_back(copies.size());
+      slot_cap = std::max(slot_cap, b);
+    }
+  }
+  int place(zb200_ctx *ctx, size_t nslots) {
+    const size_t ng = gb.size() - 1;
+    slots = std::max<size_t>(1, std::min(nslots, ng));
+    ENSURE(ctx->dict_win, (size_t)(slots * slot_cap) + 64);
+    for (size_t g = 0; g < ng; g++)
+      for (size_t i = gb[g]; i < gb[g + 1]; i++)
+        if (ctx->dict_entry[i] >= 0)
+          ctx->dict_member[i].wend = (const uint8_t *)ctx->dict_win.p + (g % slots) * slot_cap + end_of[i];
+    return ZB200_OK;
+  }
+
+  int upload(zb200_ctx *ctx, size_t g, cudaStream_t st) {
+    if (!bytes[g]) return ZB200_OK;
+    host.resize(bytes[g]);
+    for (size_t t = c0[g]; t < c0[g + 1]; t++) {
+      const size_t j = (size_t)copies[t].entry;
+      const uint64_t wl = std::min<uint64_t>(ctx->dict_offs[j + 1] - ctx->dict_offs[j], 32768);
+      memcpy(host.data() + copies[t].end - wl, ctx->dict_base + ctx->dict_offs[j + 1] - wl, (size_t)wl);
+    }
+    // through the pinned staging ring: `host` may be refilled as soon as this returns
+    return h2d_copy(ctx, (uint8_t *)ctx->dict_win.p + (g % slots) * slot_cap, host.data(), (size_t)bytes[g], st, true);
+  }
 };
 
 // A compression strategy (ZB_STRATEGY_*) folded into the level, in zlib's order: stored at level 0 whatever the
@@ -598,11 +740,14 @@ int compress_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint8_t *h_src, 
   const uint64_t hist = sp ? sp->hist : 0;
   const bool head = !sp || sp->head, last = !sp || sp->last;
   const bool lz = level == -1 || level >= 2;
-  // a batch's dictionary: every member's first chunk sees the window as its history (LZ levels), and zlib headers
+  // a batch's dictionaries: a member's first chunk sees its window as its history (LZ levels), and zlib headers
   // carry FDICT; a stream's dictionary is history in its own buffer, so only its header is the stream's business
-  const bool dict_hist = !sp && ctx->dict_on && lz;
-  const bool has_dict = data_format == ZB200_DF_ZLIB && (sp ? sp->has_dict : ctx->dict_on);
-  const uint32_t dict_id = sp ? sp->dict_id : ctx->dict_id;
+  // (any non-zero win_len marks FDICT)
+  const bool dict_hist = !sp && ctx->dict_on && lz && h_src;
+  std::vector<ZbMemberDict> mdict;   // set once the windows are placed (dict_hist) or now
+  if (sp && sp->has_dict && data_format == ZB200_DF_ZLIB) mdict.assign(1, ZbMemberDict{nullptr, 1u, sp->dict_id});
+  else if (!sp && ctx->dict_on && !dict_hist) mdict = ctx->dict_member;
+  DictWindows dw;
   const uint64_t src_lo = src_offsets[0] - hist;  // d_src holds [src_lo, src_hi) rebased to 0 when staging from the host
   const bool src_pageable = h_src && is_pageable(h_src + src_lo), dst_pageable = h_dst && is_pageable(h_dst);
 
@@ -655,8 +800,8 @@ int compress_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint8_t *h_src, 
         d.member = (uint32_t)(m1 - m0);
         d.flags = (k == 0 ? ZB_CHUNK_FIRST | (head ? ZB_CHUNK_HEAD : 0u) : 0u) | (k == nc - 1 && last ? ZB_CHUNK_LAST : 0u);
         d.pad = lz ? (uint32_t)std::min<uint64_t>(32768, hist + (uint64_t)k * ZB_CHUNK_BYTES) : 0u;
-        if (dict_hist && k == 0) {
-          d.pad = ctx->dict_len;
+        if (dict_hist && k == 0 && ctx->dict_member[m1].win_len) {
+          d.pad = ctx->dict_member[m1].win_len;
           d.flags |= ZB_CHUNK_DICT;
         }
       }
@@ -674,6 +819,16 @@ int compress_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint8_t *h_src, 
     m0 = m1;
   }
   const size_t ng = groups.size(), nc_all = nd;
+  if (dict_hist) {
+    // each launch group's windows go up with its input (DictWindows), in slots reused kDictSlots groups later
+    std::vector<size_t> gbounds(1, 0);
+    std::vector<uint8_t> cls(n);
+    for (const Group &g : groups) gbounds.push_back(g.m1);
+    for (size_t i = 0; i < n; i++) cls[i] = (uint8_t)((uintptr_t)(d_src + src_offsets[i] - src_lo) & 15u);
+    if (int rc = dw.plan(ctx, gbounds, cls.data(), kDictSlots)) return rc;
+    mdict = ctx->dict_member;
+  }
+  if (!mdict.empty()) ENSURE(ctx->dict_md, mdict.size() * sizeof(ZbMemberDict));
 
   ENSURE(ctx->desc, nc_all * sizeof(ZbChunkDesc));
   ENSURE(ctx->member_first, nfirst * sizeof(uint32_t));
@@ -706,6 +861,8 @@ int compress_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint8_t *h_src, 
   } sync_on_return{s};
   CK(cudaMemcpyAsync(ctx->desc.p, desc, nc_all * sizeof(ZbChunkDesc), cudaMemcpyHostToDevice, s));
   CK(cudaMemcpyAsync(ctx->member_first.p, first, nfirst * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
+  if (!mdict.empty())
+    CK(cudaMemcpyAsync(ctx->dict_md.p, mdict.data(), mdict.size() * sizeof(ZbMemberDict), cudaMemcpyHostToDevice, s));
   if (fname_lens && data_format == ZB200_DF_GZIP)
     CK(cudaMemcpyAsync(ctx->fname.p, fname_lens, n, cudaMemcpyHostToDevice, s));
   if (sp) CK(cudaMemcpyAsync(d_carry, &sp->carry_in, sizeof(ZbMemberCarry), cudaMemcpyHostToDevice, s));
@@ -747,11 +904,8 @@ int compress_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint8_t *h_src, 
     w.data_format = data_format;
     w.out_base = 0;
     w.out_base_ptr = (const uint64_t *)ctx->group_end.p + gi;
-    w.win16 = dict_hist ? (const uint8_t *)ctx->dict_win16.p : nullptr;
-    w.win_len = dict_hist ? ctx->dict_len : 0u;
-    w.win_stride = dict_hist ? zb_win16_stride(ctx->dict_len) : 0u;
-    w.dict_id = dict_id;
-    w.has_dict = has_dict ? 1 : 0;
+    w.mdict = mdict.empty() ? nullptr : (const ZbMemberDict *)ctx->dict_md.p + g.m0;
+    w.dict_hist = dict_hist ? 1 : 0;
     return w;
   };
 
@@ -782,6 +936,10 @@ int compress_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint8_t *h_src, 
   for (size_t gi = 0; gi < ng; gi++) {
     const Group &g = groups[gi];
     if (h_src) {
+      if (dict_hist) {   // the slot's previous group has been packed (its k_lz2 is done)
+        if (gi >= dw.slots) CK(cudaStreamWaitEvent(sh, ctx->gev[3 * (gi - dw.slots) + 1], 0));
+        if (int rc2 = dw.upload(ctx, gi, sh)) return rc2;
+      }
       if (g.in_hi > g.in_lo) {
         int rc2 = h2d_copy(ctx, (uint8_t *)d_src + g.in_lo, h_src + src_lo + g.in_lo, (size_t)(g.in_hi - g.in_lo), sh, src_pageable);
         if (rc2) return rc2;
@@ -2036,12 +2194,11 @@ bool longest_first_order(const uint64_t *src_offsets, size_t n, std::vector<uint
 // With d_crcs it is the plain crc32 configuration instead (no kinds, no expected values): d_crcs[i] gets the CRC-32 of
 // every output that inflated, raw deflate included, and nothing is compared -- a ZIP entry's CRC lives in the
 // archive's headers, not behind the stream.
-// the dictionary of the *_dict call in progress, if any, for a whole-member inflate launch
-void set_dict(const zb200_ctx *ctx, ZbInflateWork &w) {
+// the dictionaries of the *_dict / *_dicts call in progress, if any, for a whole-member inflate launch over the
+// call's members from m0 on
+void set_dict(const zb200_ctx *ctx, ZbInflateWork &w, size_t m0) {
   if (!ctx->dict_on) return;
-  w.dict = (const uint8_t *)ctx->dict_win.p;
-  w.dict_len = ctx->dict_len;
-  w.dict_id = ctx->dict_id;
+  w.mdict = (const ZbMemberDict *)ctx->dict_md.p + m0;
 }
 
 void set_check_pass(ZbChecksumWork &cw, const ZbInflateWork &w, uint32_t *d_crcs) {
@@ -2065,7 +2222,8 @@ void set_check_pass(ZbChecksumWork &cw, const ZbInflateWork &w, uint32_t *d_crcs
 int uncompress_device_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint64_t *src_offsets, size_t n,
                              int data_format, uint64_t raw_pos, uint8_t *d_dst, const uint64_t *dst_offsets,
                              uint64_t *dst_lens, int *statuses, bool count_only,
-                             const std::function<int()> *after_launch = nullptr, uint32_t *crcs = nullptr) {
+                             const std::function<int()> *after_launch = nullptr, uint32_t *crcs = nullptr,
+                             size_t dict_m0 = 0) {
   if (data_format < ZB200_DF_DETECT || data_format > ZB200_DF_DEFLATE) return ZB200_ERR_INVALID_FORMAT;
   if (n == 0) return ZB200_OK;
   ENSURE(ctx->src_off, (n + 1) * sizeof(uint64_t));
@@ -2098,7 +2256,7 @@ int uncompress_device_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint64_
   w.skip = nullptr;
   w.seg_mode = 0;
   w.order = nullptr;
-  set_dict(ctx, w);
+  set_dict(ctx, w, dict_m0);   // (with dictionaries: a group of uncompress_sizes_host, its first member)
   {
     std::vector<uint32_t> order;
     if (longest_first_order(src_offsets, n, order)) {
@@ -2181,9 +2339,26 @@ int uncompress_host_pipelined(zb200_ctx *ctx, const uint8_t *h_src, const std::v
                               int data_format, uint8_t *h_dst, const std::vector<uint64_t> &dreb, uint64_t *dst_lens,
                               int *statuses, const std::vector<size_t> &gb, uint32_t *crcs) {
   const size_t ng = gb.size() - 1;
+  // With dictionaries each group's windows go up with its input (DictWindows).  The gated launch keeps every group's
+  // windows (no slot is reused: a reuse would have to wait for the kernel to finish a group, and the kernel's warps
+  // can wait for a later group's gate, which would then wait for that copy), so it is used only while all of them
+  // fit kDictSlots slots' worth; otherwise the launches go group by group and a slot is reused kDictSlots groups
+  // later, once the launch that read it has finished.
+  DictWindows dw;
+  bool resident = true;
+  if (ctx->dict_on) {
+    dw.layout(ctx, gb, nullptr);
+    resident = (uint64_t)ng * dw.slot_cap <= kDictSlots * kDictGroupWindowBytes;
+  }
   // gated: ONE inflate launch walks the whole batch behind the copy-in (no per-group launch tails), the D2H
   // stream waits on the per-group done counts; otherwise one launch per group, chained with events
-  const bool gated = ctx->memops.ok && ctx->gated_unc && n < 0xffffffffull;
+  const bool gated = ctx->memops.ok && ctx->gated_unc && n < 0xffffffffull && resident;
+  if (ctx->dict_on) {
+    if (int rc = dw.place(ctx, gated ? ng : kDictSlots)) return rc;
+    ENSURE(ctx->dict_md, n * sizeof(ZbMemberDict));
+    CK(cudaMemcpyAsync(ctx->dict_md.p, ctx->dict_member.data(), n * sizeof(ZbMemberDict), cudaMemcpyHostToDevice,
+                       ctx->stream));
+  }
   cudaStream_t s = ctx->stream, sh = ctx->h2d_stream, sd = ctx->d2h_stream;
   const uint8_t *d_src = (const uint8_t *)ctx->in_stage.p;
   uint8_t *d_dst = (uint8_t *)ctx->out_stage.p;
@@ -2261,7 +2436,7 @@ int uncompress_host_pipelined(zb200_ctx *ctx, const uint8_t *h_src, const std::v
   if (gated) {
     // nothing that may synchronise the device (allocations, registrations) can happen while the gated kernel waits
     // for input: the staging rings of pageable callers are set up first
-    if (src_pageable) {
+    if (src_pageable || ctx->dict_on) {   // (the windows always go through the staging ring)
       int rc = ring_ready(ctx, ctx->ring_in);
       if (rc) return rc;
     }
@@ -2296,7 +2471,7 @@ int uncompress_host_pipelined(zb200_ctx *ctx, const uint8_t *h_src, const std::v
     w.gate_done = d_gate + 1;
     w.gate_first = d_gate + 1 + ng;
     w.n_gates = (uint32_t)ng;
-    set_dict(ctx, w);
+    set_dict(ctx, w, 0);
     CK(zb_launch_inflate(w, s));
     // from here on the kernel may be waiting for copies: if this function leaves early (a failed copy, a failed
     // enqueue), open every gate so that the kernel drains instead of waiting out its timeout
@@ -2323,6 +2498,9 @@ int uncompress_host_pipelined(zb200_ctx *ctx, const uint8_t *h_src, const std::v
     ctx->timing.kernel_launches += 3;
     auto copy_in = [&](size_t gi) -> int {
       const uint64_t b0 = reb[gb[gi]], b1 = reb[gb[gi + 1]];
+      if (ctx->dict_on) {   // (one slot per group here: nothing waits for the kernel)
+        if (int rc = dw.upload(ctx, gi, sh)) return rc;
+      }
       int rc = h2d_copy(ctx, (uint8_t *)ctx->in_stage.p + b0, h_src + b0, (size_t)(b1 - b0), sh, src_pageable);
       if (rc) return rc;
       if (ctx->memops.write32((CUstream)sh, (CUdeviceptr)(uintptr_t)d_gate, (cuuint32_t)(gi + 1), 0) != CUDA_SUCCESS) return ZB200_ERR_CUDA;
@@ -2372,6 +2550,10 @@ int uncompress_host_pipelined(zb200_ctx *ctx, const uint8_t *h_src, const std::v
   }
   for (size_t gi = 0; gi < ng && !gated; gi++) {
     const size_t m0 = gb[gi], m1 = gb[gi + 1], nm = m1 - m0;
+    if (ctx->dict_on) {   // the slot's previous group has been decoded and checked
+      if (gi >= dw.slots) CK(cudaStreamWaitEvent(sh, ctx->gev[2 * (gi - dw.slots) + 1], 0));
+      if (int rc = dw.upload(ctx, gi, sh)) return rc;
+    }
     {
       const uint64_t b0 = reb[m0], b1 = reb[m1];
       int rc = h2d_copy(ctx, (uint8_t *)ctx->in_stage.p + b0, h_src + b0, (size_t)(b1 - b0), sh, src_pageable);
@@ -2395,7 +2577,7 @@ int uncompress_host_pipelined(zb200_ctx *ctx, const uint8_t *h_src, const std::v
     w.n = (uint32_t)nm;
     w.data_format = data_format;
     w.order = has_order[gi] ? (const uint32_t *)ctx->order.p + m0 : nullptr;
-    set_dict(ctx, w);
+    set_dict(ctx, w, m0);
     CK(zb_launch_inflate(w, s));
     // the checksum pass of every member that inflated
     ZbChecksumWork cw;
@@ -2630,7 +2812,7 @@ void zb200_shutdown(zb200_ctx *ctx) {
                     &ctx->src_off, &ctx->dst_off, &ctx->out_len, &ctx->status, &ctx->expect, &ctx->kind,
                     &ctx->counter, &ctx->cix_rec, &ctx->cix_crc, &ctx->cix_first, &ctx->cix_out, &ctx->ck_out, &ctx->ck_pieces, &ctx->ck_first, &ctx->ck_piece_out, &ctx->ck_partials, &ctx->in_stage, &ctx->out_stage, &ctx->lz2_tables, &ctx->carry,
                     &ctx->seg_src, &ctx->seg_dst, &ctx->seg_len, &ctx->seg_status, &ctx->seg_kind, &ctx->seg_expect, &ctx->seg_cand, &ctx->skip_mask, &ctx->order, &ctx->mark_scratch, &ctx->mark_segs, &ctx->seg_bits, &ctx->mark_win, &ctx->gate,
-                    &ctx->idx_desc, &ctx->idx_out, &ctx->dict_win, &ctx->dict_win16};
+                    &ctx->idx_desc, &ctx->idx_out, &ctx->dict_win, &ctx->dict_md};
   for (DevBuf *b : bufs)
     if (b->p) cudaFree(b->p);
   if (ctx->d_tabs) cudaFree(ctx->d_tabs);
@@ -2730,15 +2912,26 @@ int zb200_compress_batch_device(zb200_ctx *ctx, const uint8_t *d_src, const uint
                                               fname_lens, d_dst, dst_cap, dst_offsets, statuses);
 }
 
-// zb200_compress_batch, and with a non-empty dictionary zb200_compress_batch_dict
+// zb200_compress_batch, and with a dictionary table zb200_compress_batch_dicts (dict_of: the member's entry; null:
+// every member names entry 0, zb200_compress_batch_dict)
 static int compress_batch_host(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n, int level,
-                               int data_format, const uint8_t *dict, size_t dict_len, const uint8_t *fname_lens,
-                               uint8_t *dst_base, size_t dst_cap, uint64_t *dst_offsets, int *statuses,
-                               int strategy = ZB_STRATEGY_DEFAULT, int window_bits = 15) {
+                               int data_format, const uint8_t *dict_base, const uint64_t *dict_offsets, size_t k,
+                               const int32_t *dict_of, const uint8_t *fname_lens, uint8_t *dst_base, size_t dst_cap,
+                               uint64_t *dst_offsets, int *statuses, int strategy = ZB_STRATEGY_DEFAULT,
+                               int window_bits = 15) {
   return guarded(ctx, [&]() -> int {
-  if (!ctx || !src_offsets || !dst_offsets || (n && (!src_base || !dst_base)) || (dict_len && !dict)) return ZB200_ERR_ARG;
+  if (!ctx || !src_offsets || !dst_offsets || (n && (!src_base || !dst_base))) return ZB200_ERR_ARG;
   if (zb_window_bits(window_bits, data_format)) return ZB200_ERR_ARG;
-  if (dict_len) {  // zlib's deflateSetDictionary refuses gzip too: the format has no field for it
+  const bool shared = k && !dict_of;   // zb200_compress_batch_dict: its checks apply even to an empty batch
+  std::vector<int32_t> all0;
+  if (shared) {
+    all0.assign(n, 0);
+    dict_of = all0.data();
+  }
+  bool any = false;
+  if (int rc = check_dicts(dict_base, dict_offsets, k, dict_of, n, any)) return rc;
+  if (any || (shared && dict_offsets[1] > dict_offsets[0])) {
+    // zlib's deflateSetDictionary refuses gzip too: the format has no field for it
     if (level < -2 || level > 9) return ZB200_ERR_INVALID_LEVEL;
     if (data_format != ZB200_DF_ZLIB && data_format != ZB200_DF_DEFLATE) return ZB200_ERR_INVALID_FORMAT;
   }
@@ -2746,7 +2939,9 @@ static int compress_batch_host(zb200_ctx *ctx, const uint8_t *src_base, const ui
   DeviceGuard g(ctx->device);
   memset(&ctx->timing, 0, sizeof(ctx->timing));
   DictScope ds(ctx);
-  if (int rc = ds.set(dict, dict_len, level == -1 || level >= 2)) return rc;
+  if (any) {
+    if (int rc = ds.set(dict_base, dict_offsets, k, dict_of, n)) return rc;
+  }
   if (n == 0) {
     dst_offsets[0] = 0;
     return ZB200_OK;
@@ -2775,8 +2970,8 @@ static int compress_batch_host(zb200_ctx *ctx, const uint8_t *src_base, const ui
 int zb200_compress_batch(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n, int level,
                          int data_format, const uint8_t *fname_lens, uint8_t *dst_base, size_t dst_cap,
                          uint64_t *dst_offsets, int *statuses) {
-  return compress_batch_host(ctx, src_base, src_offsets, n, level, data_format, nullptr, 0, fname_lens, dst_base, dst_cap,
-                             dst_offsets, statuses);
+  return compress_batch_host(ctx, src_base, src_offsets, n, level, data_format, nullptr, nullptr, 0, nullptr, fname_lens,
+                             dst_base, dst_cap, dst_offsets, statuses);
 }
 
 int zb200_compress_batch_strategy(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n,
@@ -2789,15 +2984,30 @@ int zb200_compress_batch_strategy(zb200_ctx *ctx, const uint8_t *src_base, const
 int zb200_compress_batch_window(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n,
                                 int level, int strategy, int window_bits, int data_format, const uint8_t *fname_lens,
                                 uint8_t *dst_base, size_t dst_cap, uint64_t *dst_offsets, int *statuses) {
-  return compress_batch_host(ctx, src_base, src_offsets, n, level, data_format, nullptr, 0, fname_lens, dst_base, dst_cap,
-                             dst_offsets, statuses, strategy, window_bits);
+  return compress_batch_host(ctx, src_base, src_offsets, n, level, data_format, nullptr, nullptr, 0, nullptr, fname_lens,
+                             dst_base, dst_cap, dst_offsets, statuses, strategy, window_bits);
 }
 
 int zb200_compress_batch_dict(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n, int level,
                               int data_format, const uint8_t *dict, size_t dict_len, uint8_t *dst_base, size_t dst_cap,
                               uint64_t *dst_offsets, int *statuses) {
-  return compress_batch_host(ctx, src_base, src_offsets, n, level, data_format, dict, dict_len, nullptr, dst_base, dst_cap,
-                             dst_offsets, statuses);
+  if (dict_len && !dict) return ZB200_ERR_ARG;
+  const uint64_t offs[2] = {0, dict_len};
+  return compress_batch_host(ctx, src_base, src_offsets, n, level, data_format, dict, offs, 1, nullptr, nullptr,
+                             dst_base, dst_cap, dst_offsets, statuses);
+}
+
+int zb200_compress_batch_dicts(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n,
+                               int level, int data_format, int window_bits, const uint8_t *dict_base,
+                               const uint64_t *dict_offsets, size_t k, const int32_t *dict_of, uint8_t *dst_base,
+                               size_t dst_cap, uint64_t *dst_offsets, int *statuses) {
+  static const int32_t kNoMembers = -1;   // an empty batch may pass no dict_of (null means "shared" below)
+  if (!dict_of) {
+    if (n) return ZB200_ERR_ARG;
+    dict_of = &kNoMembers;
+  }
+  return compress_batch_host(ctx, src_base, src_offsets, n, level, data_format, dict_base, dict_offsets, k, dict_of,
+                             nullptr, dst_base, dst_cap, dst_offsets, statuses, ZB_STRATEGY_DEFAULT, window_bits);
 }
 
 // host inputs (pipelined H2D over launch groups) -> members left in device memory: the sharded
@@ -3187,17 +3397,56 @@ int zb200_uncompress_sizes_device(zb200_ctx *ctx, const uint8_t *d_src, const ui
   });
 }
 
-// zb200_uncompress_sizes, and with a non-empty dictionary zb200_uncompress_sizes_dict
+// The decode calls' dictionary table (check_dicts, then DictScope::set): of == null means every member names entry 0
+// (the *_dict calls).  Nothing happens without a member that names a non-empty entry.
+static int set_decode_dicts(zb200_ctx *ctx, DictScope &ds, const uint8_t *base, const uint64_t *offs, size_t k,
+                            const int32_t *of, size_t n) {
+  std::vector<int32_t> all0;
+  if (!of && k) {
+    all0.assign(n, 0);
+    of = all0.data();
+  }
+  bool any = false;
+  if (int rc = check_dicts(base, offs, k, of, n, any)) return rc;
+  return any ? ds.set(base, offs, k, of, n) : ZB200_OK;
+}
+
+// Group cuts for the decode calls' windows: gb (0, ..., n) with further cuts wherever a group's distinct windows
+// (DictWindows with class 0) would pass kDictGroupWindowBytes.
+static std::vector<size_t> dict_cut(const zb200_ctx *ctx, const std::vector<size_t> &gb) {
+  std::vector<size_t> out(1, 0), stamp(ctx->dict_k, SIZE_MAX);
+  uint64_t b = 0;
+  for (size_t g = 0; g + 1 < gb.size(); g++) {
+    for (size_t i = gb[g]; i < gb[g + 1]; i++) {
+      const int32_t j = ctx->dict_entry[i];
+      if (j < 0 || stamp[j] == out.size()) continue;
+      const uint64_t st = zb_win_stride(ctx->dict_member[i].win_len);
+      if (b + st > kDictGroupWindowBytes && i > out.back()) {
+        out.push_back(i);
+        b = 0;
+      }
+      stamp[j] = out.size();
+      b += st;
+    }
+    if (gb[g + 1] > out.back()) out.push_back(gb[g + 1]);
+    b = 0;
+  }
+  return out;
+}
+
+// zb200_uncompress_sizes, and with a dictionary table zb200_uncompress_sizes_dicts (dict_of null: every member names
+// entry 0, zb200_uncompress_sizes_dict)
 static int uncompress_sizes_host(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n,
-                                 int data_format, const uint8_t *dict, size_t dict_len, uint64_t *sizes, int *statuses) {
+                                 int data_format, const uint8_t *dict_base, const uint64_t *dict_offsets, size_t k,
+                                 const int32_t *dict_of, uint64_t *sizes, int *statuses) {
   return guarded(ctx, [&]() -> int {
-  if (!ctx || !src_offsets || !sizes || (n && !src_base) || (dict_len && !dict)) return ZB200_ERR_ARG;
+  if (!ctx || !src_offsets || !sizes || (n && !src_base)) return ZB200_ERR_ARG;
   if (data_format < ZB200_DF_DETECT || data_format > ZB200_DF_DEFLATE) return ZB200_ERR_INVALID_FORMAT;
   std::lock_guard<std::mutex> lk(ctx->mu);
   DeviceGuard g(ctx->device);
   memset(&ctx->timing, 0, sizeof(ctx->timing));
   DictScope ds(ctx);
-  if (int rc = ds.set(dict, dict_len)) return rc;
+  if (int rc = set_decode_dicts(ctx, ds, dict_base, dict_offsets, k, dict_of, n)) return rc;
   for (size_t i = 0; i < n; i++)
     if (src_offsets[i + 1] < src_offsets[i]) return ZB200_ERR_ARG;
   // gzip members answer from their trailer (gzip.nim:66) after the same wrapper checks the device decoder
@@ -3207,8 +3456,9 @@ static int uncompress_sizes_host(zb200_ctx *ctx, const uint8_t *src_base, const 
   for (size_t i = 0; i < n && !need_device; i++) {
     uint64_t payload = 0;
     uint32_t kind = 0, expect = 0, isize = 0;
+    const ZbMemberDict *md = ctx->dict_on && ctx->dict_member[i].win_len ? &ctx->dict_member[i] : nullptr;
     const int st = zb_parse_wrapper(src_base + src_offsets[i], src_offsets[i + 1] - src_offsets[i], data_format, 0, payload,
-                                    kind, expect, isize, ctx->dict_on ? &ctx->dict_id : nullptr);
+                                    kind, expect, isize, md ? &md->dict_id : nullptr);
     if (st == ZB200_OK && kind != ZB200_DF_GZIP) need_device = true;
     sizes[i] = st == ZB200_OK ? isize : 0;
     if (statuses) statuses[i] = st;
@@ -3217,36 +3467,63 @@ static int uncompress_sizes_host(zb200_ctx *ctx, const uint8_t *src_base, const 
   std::vector<uint64_t> reb;
   int rc = stage_in(ctx, src_base, src_offsets, n, reb);
   if (rc) return rc;
-  return uncompress_device_locked(ctx, (const uint8_t *)ctx->in_stage.p, reb.data(), n, data_format, 0, nullptr,
-                                  nullptr, sizes, statuses, true);
+  if (!ctx->dict_on)
+    return uncompress_device_locked(ctx, (const uint8_t *)ctx->in_stage.p, reb.data(), n, data_format, 0, nullptr,
+                                    nullptr, sizes, statuses, true);
+  // with dictionaries: one counting launch per group of members whose windows fit one slot
+  DictWindows dw;
+  if (int rc2 = dw.plan(ctx, dict_cut(ctx, {0, n}), nullptr, 1)) return rc2;
+  ENSURE(ctx->dict_md, n * sizeof(ZbMemberDict));
+  CK(cudaMemcpyAsync(ctx->dict_md.p, ctx->dict_member.data(), n * sizeof(ZbMemberDict), cudaMemcpyHostToDevice,
+                     ctx->stream));
+  for (size_t g = 0; g + 1 < dw.gb.size(); g++) {
+    const size_t m0 = dw.gb[g], m1 = dw.gb[g + 1];
+    if (int rc2 = dw.upload(ctx, g, ctx->stream)) return rc2;
+    rc = uncompress_device_locked(ctx, (const uint8_t *)ctx->in_stage.p, reb.data() + m0, m1 - m0, data_format, 0,
+                                  nullptr, nullptr, sizes + m0, statuses ? statuses + m0 : nullptr, true,
+                                  nullptr, nullptr, m0);
+    if (rc) return rc;   // (it ends with the stream synchronised: the slot is free again)
+  }
+  return ZB200_OK;
   });
 }
 
 int zb200_uncompress_sizes(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n,
                            int data_format, uint64_t *sizes, int *statuses) {
-  return uncompress_sizes_host(ctx, src_base, src_offsets, n, data_format, nullptr, 0, sizes, statuses);
+  return uncompress_sizes_host(ctx, src_base, src_offsets, n, data_format, nullptr, nullptr, 0, nullptr, sizes, statuses);
 }
 
 int zb200_uncompress_sizes_dict(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n,
                                 int data_format, const uint8_t *dict, size_t dict_len, uint64_t *sizes, int *statuses) {
-  return uncompress_sizes_host(ctx, src_base, src_offsets, n, data_format, dict, dict_len, sizes, statuses);
+  if (dict_len && !dict) return ZB200_ERR_ARG;
+  const uint64_t offs[2] = {0, dict_len};
+  return uncompress_sizes_host(ctx, src_base, src_offsets, n, data_format, dict, offs, 1, nullptr, sizes, statuses);
 }
 
-// zb200_uncompress_batch, with crcs (host, may be null) zb200_inflate_batch_crc32, with a non-empty dictionary
-// zb200_uncompress_batch_dict
+int zb200_uncompress_sizes_dicts(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n,
+                                 int data_format, const uint8_t *dict_base, const uint64_t *dict_offsets, size_t k,
+                                 const int32_t *dict_of, uint64_t *sizes, int *statuses) {
+  if (n && !dict_of) return ZB200_ERR_ARG;
+  return uncompress_sizes_host(ctx, src_base, src_offsets, n, data_format, dict_base, dict_offsets, k, dict_of, sizes,
+                               statuses);
+}
+
+// zb200_uncompress_batch, with crcs (host, may be null) zb200_inflate_batch_crc32, with a dictionary table
+// zb200_uncompress_batch_dicts (dict_of null: every member names entry 0, zb200_uncompress_batch_dict)
 static int uncompress_batch_host(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n,
                                  int data_format, uint8_t *dst_base, const uint64_t *dst_offsets, uint64_t *dst_lens,
-                                 int *statuses, uint32_t *crcs, const uint8_t *dict = nullptr, size_t dict_len = 0) {
+                                 int *statuses, uint32_t *crcs, const uint8_t *dict_base = nullptr,
+                                 const uint64_t *dict_offsets = nullptr, size_t k = 0, const int32_t *dict_of = nullptr) {
   return guarded(ctx, [&]() -> int {
-  if (!ctx || !src_offsets || !dst_offsets || !dst_lens || (n && !src_base) || (dict_len && !dict)) return ZB200_ERR_ARG;
+  if (!ctx || !src_offsets || !dst_offsets || !dst_lens || (n && !src_base)) return ZB200_ERR_ARG;
   std::lock_guard<std::mutex> lk(ctx->mu);
   DeviceGuard g(ctx->device);
   memset(&ctx->timing, 0, sizeof(ctx->timing));
-  DictScope ds(ctx);
-  if (int rc = ds.set(dict, dict_len)) return rc;
-  if (n == 0) return ZB200_OK;
   for (size_t i = 0; i < n; i++)
     if (src_offsets[i + 1] < src_offsets[i] || dst_offsets[i + 1] < dst_offsets[i]) return ZB200_ERR_ARG;
+  DictScope ds(ctx);
+  if (int rc = set_decode_dicts(ctx, ds, dict_base, dict_offsets, k, dict_of, n)) return rc;
+  if (n == 0) return ZB200_OK;
   const uint64_t slo = src_offsets[0], shi = src_offsets[n], lo = dst_offsets[0], hi = dst_offsets[n];
   std::vector<uint64_t> reb(n + 1), dreb(n + 1);
   for (size_t i = 0; i <= n; i++) {
@@ -3282,6 +3559,7 @@ static int uncompress_batch_host(zb200_ctx *ctx, const uint8_t *src_base, const 
         gb.push_back(i);
         a = i;
       }
+    if (ctx->dict_on) gb = dict_cut(ctx, gb);
   }
   const size_t ng = gb.size() - 1;
   {
@@ -3369,8 +3647,19 @@ int zb200_uncompress_batch(zb200_ctx *ctx, const uint8_t *src_base, const uint64
 int zb200_uncompress_batch_dict(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n,
                                 int data_format, const uint8_t *dict, size_t dict_len, uint8_t *dst_base,
                                 const uint64_t *dst_offsets, uint64_t *dst_lens, int *statuses) {
+  if (dict_len && !dict) return ZB200_ERR_ARG;
+  const uint64_t offs[2] = {0, dict_len};
   return uncompress_batch_host(ctx, src_base, src_offsets, n, data_format, dst_base, dst_offsets, dst_lens, statuses,
-                               nullptr, dict, dict_len);
+                               nullptr, dict, offs, 1, nullptr);
+}
+
+int zb200_uncompress_batch_dicts(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n,
+                                 int data_format, const uint8_t *dict_base, const uint64_t *dict_offsets, size_t k,
+                                 const int32_t *dict_of, uint8_t *dst_base, const uint64_t *dst_offsets,
+                                 uint64_t *dst_lens, int *statuses) {
+  if (n && !dict_of) return ZB200_ERR_ARG;
+  return uncompress_batch_host(ctx, src_base, src_offsets, n, data_format, dst_base, dst_offsets, dst_lens, statuses,
+                               nullptr, dict_base, dict_offsets, k, dict_of);
 }
 
 int zb200_inflate_batch_crc32(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n,

@@ -652,10 +652,10 @@ __device__ __forceinline__ void lz2_extend(const Lz2Pos &P, const uint8_t *data,
 // Stage a ZB_CHUNK_DICT chunk: its hb bytes of history are the end of the dictionary window W, the chunk itself
 // comes from src.  The region keeps the layout of zb_stage_chunk(rsrc, hb + len): region position q at
 // data[mis + q] with mis = (chunk start - hb) & 15, so the chunk's 16-byte granules start at the aligned offset
-// a0 = hb + mis - cmis.  win16's copy number cmis ends W at an address that is cmis modulo 16, so W's tail lines up
-// with the same granules: one bulk copy fills data[0, a0) from W, one fills data[a0, ..) from src (with the cmis
-// bytes of src in front of the chunk), and after the wait the <= 15 history bytes at q >= hb - cmis are stored
-// from W by plain stores.  Called by thread 0 (the copies) and then by every thread (fix_dict_head).
+// a0 = hb + mis - cmis.  The member's copy of W (ZbMemberDict::wend) ends at an address that is cmis modulo 16, so
+// W's tail lines up with the same granules: one bulk copy fills data[0, a0) from W, one fills data[a0, ..) from src
+// (with the cmis bytes of src in front of the chunk), and after the wait the <= 15 history bytes at q >= hb - cmis
+// are stored from W by plain stores.  Called by thread 0 (the copies) and then by every thread (fix_dict_head).
 __device__ __forceinline__ void stage_dict_chunk(uint8_t *data, const uint8_t *chunk, uint32_t len, uint32_t hb,
                                                  const uint8_t *wend, uint64_t *bar) {
   const uint32_t cmis = (uint32_t)((uintptr_t)chunk & 15u);
@@ -690,7 +690,7 @@ __global__ void __launch_bounds__(LZ_THREADS, 2)
     k_lz2(const uint8_t *__restrict__ src, const ZbChunkDesc *__restrict__ desc, uint2 *__restrict__ masks,
           uint32_t *__restrict__ recs, uint16_t *__restrict__ hist, ZbChunkCheck *__restrict__ chk,
           const ZbCrcTables *__restrict__ tabs, uint2 *__restrict__ tables, uint32_t n_chunks, ZbLz2Params prm,
-          const uint8_t *__restrict__ win16, uint32_t win_len, uint32_t win_stride) {
+          const ZbMemberDict *__restrict__ mdict) {
   extern __shared__ __align__(128) uint8_t smem[];
   uint8_t *data = smem;
   uint32_t *hist_all = reinterpret_cast<uint32_t *>(smem + LZ2_SM_HIST);
@@ -729,11 +729,8 @@ __global__ void __launch_bounds__(LZ_THREADS, 2)
     const uint32_t mis = (uint32_t)((uintptr_t)rsrc & 15u);
     const uint32_t off0 = mis + hb;           // chunk position x lives at data[off0 + x]
     const uint32_t rlen = hb + len;           // staged bytes; region position q = hb + chunk position
-    const uint8_t *wend = nullptr;            // DICT: the end of W in the copy that matches the chunk's alignment
-    if (DICT && (d.flags & ZB_CHUNK_DICT)) {
-      const uint32_t c = (uint32_t)((uintptr_t)(src + d.src_off) & 15u);
-      wend = win16 + (size_t)c * win_stride + ZB_WIN16_SLACK + ((c - win_len) & 15u) + win_len;
-    }
+    // DICT: the end of the member's W, in the copy that matches the chunk's alignment
+    const uint8_t *wend = DICT && (d.flags & ZB_CHUNK_DICT) ? mdict[d.member].wend : nullptr;
     if (DICT && wend) {
       if (tid == 0) stage_dict_chunk(data, src + d.src_off, len, hb, wend, bar);
     } else if (tid == 0 && rlen) {
@@ -925,9 +922,10 @@ extern "C" int zb200_huff_stage_clocks(unsigned long long *out) {
 #endif
 
 // ------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t frame_head_bytes(int fmt, const uint8_t *fname_len, uint32_t m, int has_dict) {
+__device__ __forceinline__ uint32_t frame_head_bytes(int fmt, const uint8_t *fname_len, uint32_t m,
+                                                     const ZbMemberDict *mdict) {
   if (fmt == ZB_DF_GZIP) return 10u + (fname_len ? (uint32_t)fname_len[m] : 0u) + 1u;
-  if (fmt == ZB_DF_ZLIB) return has_dict ? 6u : 2u;  // FDICT: DICTID follows CMF / FLG
+  if (fmt == ZB_DF_ZLIB) return mdict && mdict[m].win_len ? 6u : 2u;  // FDICT: DICTID follows CMF / FLG
   return 0u;
 }
 __device__ __forceinline__ uint32_t frame_tail_bytes(int fmt) {
@@ -952,7 +950,7 @@ __global__ void __launch_bounds__(SCAN_THREADS)
       member = d.member;
       sz = w.cb[c].total_bytes;
       if (flags & ZB_CHUNK_HEAD) {
-        head = frame_head_bytes(w.data_format, w.fname_len, member, w.has_dict);
+        head = frame_head_bytes(w.data_format, w.fname_len, member, w.mdict);
         sz += head;
       }
       if (flags & ZB_CHUNK_LAST) sz += frame_tail_bytes(w.data_format);
@@ -1298,9 +1296,9 @@ __global__ void __launch_bounds__(LZ_THREADS, 6)  // 6 CTAs (48 warps) per SM: <
       // CMF: CM 8, CINFO = window_bits - 8 (0x78 for 32 KiB); FLG: FLEVEL 0 and FCHECK, so that CMF FLG is 31 x k
       const uint32_t cmf = (uint32_t)(__ffs((int)w.max_dist) - 9) << 4 | 8u;
       h[0] = (uint8_t)cmf; h[1] = (uint8_t)((31u - (cmf << 8) % 31u) % 31u);
-      if (w.has_dict) {  // 0x7820 = 31 x 992: FDICT, FLEVEL 0, then the DICTID big-endian
-        const uint32_t id = w.dict_id;
-        h[1] = 0x20;
+      if (w.mdict && w.mdict[d.member].win_len) {  // FDICT, FLEVEL 0, FCHECK again, then the DICTID big-endian
+        const uint32_t id = w.mdict[d.member].dict_id;
+        h[1] = (uint8_t)(0x20u | (31u - ((cmf << 8) | 0x20u) % 31u) % 31u);
         h[2] = (uint8_t)(id >> 24); h[3] = (uint8_t)(id >> 16); h[4] = (uint8_t)(id >> 8); h[5] = (uint8_t)id;
       }
     }
@@ -1567,13 +1565,13 @@ cudaError_t zb_launch_lz(const ZbCompressWork &w, cudaStream_t s, bool index_crc
     if ((uint32_t)grid > w.n_chunks) grid = (int)w.n_chunks;
     if (w.strategy == ZB_STRATEGY_FILTERED)
       k_lz2<false, 6><<<grid, LZ_THREADS, LZ2_SM_TOTAL, s>>>(w.src, w.desc, w.masks, w.recs, w.hist, w.chk, w.tabs, w.lz2_tables,
-                                                             w.n_chunks, zb_lz2_params(w.level, w.max_dist), nullptr, 0u, 0u);
-    else if (w.win16)
+                                                             w.n_chunks, zb_lz2_params(w.level, w.max_dist), nullptr);
+    else if (w.dict_hist)
       k_lz2<true><<<grid, LZ_THREADS, LZ2_SM_TOTAL, s>>>(w.src, w.desc, w.masks, w.recs, w.hist, w.chk, w.tabs, w.lz2_tables,
-                                                         w.n_chunks, zb_lz2_params(w.level, w.max_dist), w.win16, w.win_len, w.win_stride);
+                                                         w.n_chunks, zb_lz2_params(w.level, w.max_dist), w.mdict);
     else
       k_lz2<false><<<grid, LZ_THREADS, LZ2_SM_TOTAL, s>>>(w.src, w.desc, w.masks, w.recs, w.hist, w.chk, w.tabs, w.lz2_tables,
-                                                          w.n_chunks, zb_lz2_params(w.level, w.max_dist), nullptr, 0u, 0u);
+                                                          w.n_chunks, zb_lz2_params(w.level, w.max_dist), nullptr);
   } else {
     const int mode = (w.level == -2 || w.level == 0) ? 0 : w.strategy == ZB_STRATEGY_RLE ? 2 : 1;
     const ZbLzKernel k = zb_lz_kernel(mode, w.data_format, index_crc);

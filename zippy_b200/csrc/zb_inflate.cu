@@ -725,8 +725,8 @@ __device__ __forceinline__ int symbol_loop(Grp<OutT> &g, const GroupSmem *gs, ui
 #ifndef INF_MIN_CTAS
 #define INF_MIN_CTAS 5   // register budget for 5 CTAs (20 warps) per SM, the shared-memory limit
 #endif
-// DICT: whole members decoded against w.dict (ZbInflateWork); <true, false, true> counts, <false, false, true>
-// writes bytes.  The instantiations without it compile as they did before the dictionary existed.
+// DICT: whole members decoded against their dictionaries (ZbInflateWork::mdict); <true, false, true> counts,
+// <false, false, true> writes bytes.  The instantiations without it compile as they did before the dictionary existed.
 template <bool COUNT_ONLY, bool MARK, bool DICT = false>
 __global__ void __launch_bounds__(INF_THREADS, INF_MIN_CTAS)
     k_inflate(ZbInflateWork w) {
@@ -760,6 +760,7 @@ __global__ void __launch_bounds__(INF_THREADS, INF_MIN_CTAS)
   g.op = g.cap = 0;
   g.out = nullptr;
   uint32_t rec_k = 0;   // the recorder's next multiple of 32768 (counting instantiation only)
+  const uint8_t *wend = nullptr;  // DICT: just past the current member's W
   for (;;) {
     int done = 1;  // status to report when `fin` is set
     bool fin = false;
@@ -832,9 +833,13 @@ __global__ void __launch_bounds__(INF_THREADS, INF_MIN_CTAS)
         g.expect = 0;
         int st;
         if (DICT) {
-          st = zb_parse_wrapper(g.src, g.len, w.data_format, w.pos, pos, g.kind, g.expect, isize, &w.dict_id);
+          // a member without a dictionary parses as in the plain instantiation: FDICT is ZB_ERR_FDICT
+          const ZbMemberDict md = w.mdict[i];
+          st = zb_parse_wrapper(g.src, g.len, w.data_format, w.pos, pos, g.kind, g.expect, isize,
+                                md.win_len ? &md.dict_id : nullptr);
           // raw members, and zlib members whose FDICT was accepted (payload at 6), see the window
-          g.win = (g.kind == ZB_DF_DEFLATE || (g.kind == ZB_DF_ZLIB && pos == 6)) ? w.dict_len : 0u;
+          g.win = (g.kind == ZB_DF_DEFLATE || (g.kind == ZB_DF_ZLIB && pos == 6)) ? md.win_len : 0u;
+          wend = md.wend;
         } else {
           st = zb_parse_wrapper(g.src, g.len, w.data_format, w.pos, pos, g.kind, g.expect, isize);
         }
@@ -910,7 +915,7 @@ __global__ void __launch_bounds__(INF_THREADS, INF_MIN_CTAS)
     // run the lockstep symbol loop only when no group of the warp is waiting for a header or a
     // new member: those are short, and would otherwise stall behind a whole block of symbols
     if (__any_sync(FULL_MASK, g.st == ST_FETCH || g.st == ST_BLOCK)) continue;
-    const int ev = symbol_loop<COUNT_ONLY, OutT, DICT>(g, gs, tab_addr, DICT ? w.dict + w.dict_len : nullptr);
+    const int ev = symbol_loop<COUNT_ONLY, OutT, DICT>(g, gs, tab_addr, wend);
     if (g.st == ST_SYMS && ev) {
       int st = ZB_OK;
       if (ev == 1) {
@@ -1815,7 +1820,7 @@ cudaError_t zb_launch_inflate(const ZbInflateWork &w, cudaStream_t s) {
   if (blocks > need) blocks = need;
   cudaError_t e = cudaMemsetAsync(w.counter, 0, sizeof(uint32_t), s);
   if (e != cudaSuccess) return e;
-  if (w.dict && !w.seg_bits) {
+  if (w.mdict && !w.seg_bits) {
     if (w.count_only) k_inflate<true, false, true><<<blocks, INF_THREADS, smem, s>>>(w);
     else k_inflate<false, false, true><<<blocks, INF_THREADS, smem, s>>>(w);
   } else if (w.count_only) k_inflate<true, false><<<blocks, INF_THREADS, smem, s>>>(w);

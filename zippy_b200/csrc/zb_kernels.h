@@ -34,6 +34,17 @@ struct ZbChunkCheck {
   uint32_t adler;     // Adler-32 of the chunk bytes as a standalone message
 };
 
+// One member's preset dictionary D.  wend: just past the window W (the last win_len = min(32768, |D|) bytes of D) on
+// the device.  For k_lz2 it is a copy of W whose end is congruent to the member's first chunk address modulo 16, so
+// that W's tail and the chunk share 16-byte granules (stage_dict_chunk); null when the launch stages no history.
+// win_len 0: the member has no dictionary.  dict_id: the Adler-32 of all of D (zlib's DICTID).
+struct ZbMemberDict {
+  const uint8_t *wend;
+  uint32_t win_len, dict_id;
+};
+#define ZB_WIN_SLACK 16u   // bytes in front of each aligned copy of W (the bulk copies read whole 16-byte granules)
+static inline uint32_t zb_win_stride(uint32_t win_len) { return ((win_len + 15u) & ~15u) + 3u * ZB_WIN_SLACK; }
+
 // All device scratch for one compress batch (arrays sized by n_chunks / n_members).
 struct ZbCompressWork {
   const uint8_t *src;          // device
@@ -65,16 +76,13 @@ struct ZbCompressWork {
   int strategy;
   // 2^window_bits (512..32768): no match reaches further back (k_lz<1>, k_lz2), and a zlib header's CINFO states it
   uint32_t max_dist;
-  // A preset dictionary (zb200_compress_batch_dict): has_dict puts FDICT and dict_id in the zlib header.  win16 holds
-  // 16 copies of the window W (win_len bytes; win16 256-byte aligned), copy c at
-  // win16 + c * win_stride + ZB_WIN16_SLACK + ((c - win_len) & 15), so that W ends at an address that is c modulo 16;
-  // chunks flagged ZB_CHUNK_DICT stage their history from copy (chunk start & 15).
-  const uint8_t *win16;
-  uint32_t win_len, win_stride, dict_id;
-  int has_dict;
+  // Preset dictionaries (zb200_compress_batch_dicts and its k = 1 case, zb200_compress_batch_dict; a compress
+  // stream's FDICT header): null, or [n_members] (group-relative, like desc[].member).  A member whose win_len is not
+  // 0 gets FDICT and its dict_id in a zlib header; its first chunk, flagged ZB_CHUNK_DICT, stages its `pad` bytes of
+  // history from wend (k_lz2).
+  const ZbMemberDict *mdict;
+  int dict_hist;               // some chunk is flagged ZB_CHUNK_DICT: the LZ levels run k_lz2<true>
 };
-#define ZB_WIN16_SLACK 16u   // bytes in front of each copy in win16 (the bulk copies read whole 16-byte granules)
-static inline uint32_t zb_win16_stride(uint32_t win_len) { return ((win_len + 15u) & ~15u) + 3u * ZB_WIN16_SLACK; }
 
 // per-device kernel attributes (dynamic shared memory limits); call with the device current
 cudaError_t zb_setup_deflate_attrs();
@@ -166,11 +174,10 @@ struct ZbInflateWork {
   uint64_t *rec;
   const uint64_t *rec_base;
   uint32_t nrec;
-  // A preset dictionary (whole members only, not seg_bits): null, or the device copy of its window W (the last
-  // dict_len <= 32768 bytes of the dictionary).  Raw members, and zlib members whose FDICT carries dict_id, decode
-  // as if W were output in front of their first byte; gzip and zlib members without FDICT ignore it.
-  const uint8_t *dict;
-  uint32_t dict_len, dict_id;
+  // Preset dictionaries (whole members only, not seg_bits): null, or [n] (indexed like src_off).  A raw member, or a
+  // zlib member whose FDICT carries its dict_id, decodes as if its W were output in front of its first byte; gzip
+  // members and zlib members without FDICT ignore it.  A member with win_len 0 decodes as without a dictionary.
+  const ZbMemberDict *mdict;
 };
 cudaError_t zb_launch_inflate(const ZbInflateWork &w, cudaStream_t s);
 // positions just past every byte sequence 00 00 ff ff (the empty stored block that byte-aligns a
