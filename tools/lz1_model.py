@@ -10,7 +10,9 @@ that is staged again: the piece at 32768 gets 1 KiB), one probe per position, th
 chain "match -> first candidate at or after its end".  Same-hash stores of one window resolve as "highest lane
 wins".  Prints, per entered window: lanes that pass the 4-byte check, extension steps (max over the warp and
 summed over lanes), matches the chain selects and windows whose last match hits the lane cap.  Those numbers
-size the stages tools/lz1_stages.py times.  tests/test_gpu_lz1_model.py checks them against the token-exact
+size the stages tools/lz1_stages.py times.  It also counts the windows in which any lane's match reaches the lane
+cap: the windows after which k_lz<1> drains its one-window pipeline (the next window's probe waits for the
+selection), on top of every piece's last window.  tests/test_gpu_lz1_model.py checks them against the token-exact
 model tests/native/lz1_model.c.
 """
 import argparse
@@ -28,10 +30,13 @@ def lz_hash(v):
     return ((v * 0x9E3779B1) & 0xffffffff) >> 21
 
 
-def window_stats(blocks):
-    """Per-window work of the parse of `blocks` (each 64 KiB of text without NUL bytes), summed."""
+def window_stats(blocks, any_cap=False):
+    """Per-window work of the parse of `blocks` (each 64 KiB of text without NUL bytes), summed.  any_cap: also
+    count the entered windows with any lane at the lane cap (key "any_cap")."""
     B = 65536
     tot = dict(windows=0, entered=0, verified=0, ext_steps_warp=0, ext_steps_lanes=0, chain=0, cap=0)
+    if any_cap:
+        tot["any_cap"] = 0
     for blk in blocks:
         assert len(blk) == B
         d = blk + b"\0" * 400
@@ -71,6 +76,8 @@ def window_stats(blocks):
                         ms[l] = m if m >= CAP else min(m, lim)
                         tot["verified"] += 1
                 tot["ext_steps_warp"] += steps_max
+                if any_cap and max(ms) >= CAP:
+                    tot["any_cap"] += 1
                 l, endw = entry - wb, 0
                 while l < 32:
                     if ms[l]:
@@ -95,10 +102,10 @@ def main():
     args = ap.parse_args()
     from tests import util
     T = util.text_corpus(util.load_corpus())
-    tot = window_stats([util.c2_block(T, i) for i in range(args.blocks)])
+    tot = window_stats([util.c2_block(T, i) for i in range(args.blocks)], any_cap=True)
     n = tot["entered"]
     print("%d C2 blocks: %d windows, %d entered" % (args.blocks, tot["windows"], n))
-    for k in ("verified", "ext_steps_warp", "ext_steps_lanes", "chain", "cap"):
+    for k in ("verified", "ext_steps_warp", "ext_steps_lanes", "chain", "cap", "any_cap"):
         print("  %-16s %8.3f per entered window" % (k, tot[k] / float(n)))
 
 

@@ -25,9 +25,11 @@ import types
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-# the order of the LZS_* enum in zb_deflate.cu
-LZ1_STAGE_NAMES = ["wait + table load", "checksum", "clear + pre-seed", "probe", "verify + extend", "select",
-                   "batch pass", "phase barrier + epilogue"]
+# the order of the LZS_* enum in zb_deflate.cu.  The window loop is a one-window pipeline: "probe" counts only the
+# probes that start it (a piece's first window, one after skipped windows or a drain); the other windows' probes,
+# 4-byte checks and first extension steps run inside the previous window's selection and count there
+LZ1_STAGE_NAMES = ["wait + table load", "checksum", "clear + pre-seed", "probe (pipeline start)", "verify + extend",
+                   "select + next window's probe", "batch pass", "phase barrier + epilogue"]
 # the order of the HWS_* enum in zb_huff_warp.cuh
 HUFF_STAGE_NAMES = ["sum", "sort", "Moffat-Katajainen", "limit", "assign + sums", "RLE", "code-length code",
                     "choice + header", "canonical codes", "bit ranges", "store"]

@@ -89,6 +89,10 @@ __device__ __forceinline__ uint32_t lz_final_rec(uint32_t mlen, uint32_t dist, i
 // end" (3 doubling rounds cover the at most 8 matches a window can start); a last match that
 // hit the lane cap necessarily leaves the window and is extended by the whole warp, 8 bytes
 // per lane.  Position x of the sub-chunk lives at data[off0 + x].
+// CAPPED = false: the caller knows that no lane's m reached the lane cap and that no lane below cur has a match;
+// then the selection is straight-line code (no exit extension, no test for a window without matches), which lets
+// the compiler interleave its chain of warp-wide operations with independent work around it.
+template <bool CAPPED = true>
 __device__ __forceinline__ void lz_select(const uint8_t *data, uint32_t off0, uint32_t wb, uint32_t b1, uint32_t cur,
                                           uint32_t nvalid, uint32_t &m, uint32_t dist, uint32_t *ring_slot,
                                           uint32_t &sel, uint32_t &ism, uint32_t &endw) {
@@ -96,12 +100,12 @@ __device__ __forceinline__ void lz_select(const uint8_t *data, uint32_t off0, ui
   const uint32_t mm = __ballot_sync(ZB_FULL, m != 0);
   endw = 0;
   ism = 0;
-  if (mm) {
+  if (!CAPPED || mm) {
     const uint32_t lbit = 1u << lane;
     const uint32_t endp = (uint32_t)lane + m;
     const uint32_t rest = shl_clamp(1u, endp) ? (mm >> endp) : 0u;
     uint32_t nc = rest ? endp + (uint32_t)(__ffs((int)rest) - 1) : 32u;
-    uint32_t vis = 1u << (cur + (uint32_t)(__ffs((int)(mm >> cur)) - 1));
+    uint32_t vis = CAPPED ? 1u << (cur + (uint32_t)(__ffs((int)(mm >> cur)) - 1)) : mm & (0u - mm);
 #pragma unroll
     for (int r = 0; r < 3; r++) {
       vis |= __reduce_or_sync(ZB_FULL, (vis & lbit) ? shl_clamp(1u, nc) : 0u);
@@ -116,7 +120,7 @@ __device__ __forceinline__ void lz_select(const uint8_t *data, uint32_t off0, ui
     const uint32_t cov = (ism & lbit) ? (low_mask(endp) & ~low_mask((uint32_t)lane)) : 0u;
     const uint32_t covered = __reduce_or_sync(ZB_FULL, cov);
     uint32_t mlast = __shfl_sync(ZB_FULL, m, lastm);
-    if (mlast >= LZ_LANE_CAP) {
+    if (CAPPED && mlast >= LZ_LANE_CAP) {
       const uint32_t md = __shfl_sync(ZB_FULL, dist, lastm);
       const uint32_t pos = wb + (uint32_t)lastm;
       const uint32_t off = off0 + pos + LZ_LANE_CAP + 8u * (uint32_t)lane;
@@ -134,14 +138,115 @@ __device__ __forceinline__ void lz_select(const uint8_t *data, uint32_t off0, ui
       if (lane == lastm) m = mlast;
     }
     sel = ism | (~covered & ~low_mask(cur) & low_mask(nvalid));
-    endw = (uint32_t)lastm + mlast;
-    if (ism & lbit) {
-      uint32_t rank = (uint32_t)__popc(ism & (lbit - 1u));
-      ring_slot[rank] = (m - 3u) | ((dist - 1u) << 9);
-    }
+    endw = (CAPPED || ism) ? (uint32_t)lastm + mlast : 0u;  // !CAPPED: ism = 0 when the window has no match
+    // rank and record for every lane, so that the store alone is conditional (a predicated store, no branch)
+    const uint32_t rank = (uint32_t)__popc(ism & (lbit - 1u));
+    const uint32_t rec = (m - 3u) | ((dist - 1u) << 9);
+    if (ism & lbit) ring_slot[rank] = rec;
   } else {
     sel = low_mask(nvalid) & ~low_mask(cur);
   }
+}
+
+// k_lz<1>'s work on one lane's position p of a window between its probe and its selection, in three steps:
+// lz1_probe (the table load and store), lz1_check (the 4-byte check and the first 8-byte extension step, for every
+// lane: it needs no entry), lz1_extend (drops a match below entry and extends the others up to the lane cap).
+// Position x of the piece lives at data[doff + x].
+struct Lz1Lane {
+  uint32_t c, lit, m;  // the candidate the probe read, the byte at p, the match length found so far
+  uint32_t limit;      // min(258, b1 - p); 0 past the piece end
+  uint32_t ip, ic;     // word indices of p and of the compared candidate in data
+  uint32_t sp, sc;     // their bit offsets within a word
+  uint32_t hp, hc;     // the upper words of the last step, carried into the next one
+  bool more;           // the first 12 bytes match: the extension goes on
+};
+
+__device__ __forceinline__ void lz1_probe(const uint8_t *data, uint16_t *table, uint32_t doff, uint32_t p,
+                                          uint32_t len, Lz1Lane &L, uint32_t &v, bool &can) {
+  const uint32_t *w = reinterpret_cast<const uint32_t *>(data);
+  L.ip = (doff + p) >> 2;
+  L.sp = ((doff + p) & 3u) * 8u;
+  L.hp = w[L.ip + 1];  // stays for the check
+  v = __funnelshift_r(w[L.ip], L.hp, L.sp);
+  L.lit = v & 255u;
+  can = p + 4 <= len;
+  const uint32_t h = lz_hash(v);
+  L.c = table[h];
+  __syncwarp();
+  // Lanes of this window that share a hash store to the same entry in one instruction:
+  // exactly one of them lands, and WHICH is up to the hardware (resolving the winner with
+  // __match_any_sync is a large share of the kernel) ...
+  if (can) table[h] = (uint16_t)p;
+#if ZB_LZ1_RESOLVE_WINNER
+  __syncwarp();
+  // make the outcome independent of the arbitration: the highest position wins (every round strictly
+  // raises the entry, so it ends).  Slows the kernel; off by default because the
+  // arbitration IS fixed on this hardware: the lowest lane lands, which tests/test_gpu_lz1_model.py
+  // asserts token by token (and this variant's tokens under the highest-position rule)
+  for (;;) {
+    const bool lost = can && table[h] < (uint16_t)p;
+    if (!__any_sync(ZB_FULL, lost)) break;
+    if (lost) table[h] = (uint16_t)p;
+    __syncwarp();
+  }
+#endif
+}
+
+// Unaligned compare, 8 bytes per step, carrying the upper word of each side: the first step's words are loaded with
+// the 4-byte check, so a lane waits for one round of shared-memory loads per 8 bytes.  Branch-free: a lane without a
+// candidate in reach compares p with itself, which keeps its loads inside the data region, and has no match.
+__device__ __forceinline__ void lz1_check(const uint8_t *data, uint32_t doff, uint32_t p, uint32_t b1,
+                                          uint32_t max_dist, uint32_t v, bool can, Lz1Lane &L) {
+  const uint32_t *w = reinterpret_cast<const uint32_t *>(data);
+  // a match may not cross the piece end (another warp starts its own parse there)
+  L.limit = p < b1 ? min((uint32_t)ZB_MAX_MATCH, b1 - p) : 0u;
+  const bool ok = can && L.c < p && p - L.c <= max_dist && L.limit >= ZB_MIN_MATCH;
+  const uint32_t q = ok ? L.c : p;
+  L.ic = (doff + q) >> 2;
+  L.sc = ((doff + q) & 3u) * 8u;
+  const uint32_t c0 = w[L.ic], hc = w[L.ic + 1];
+  const uint32_t np = w[L.ip + 2], nq = w[L.ic + 2], np2 = w[L.ip + 3], nq2 = w[L.ic + 3];
+  const uint32_t x = __funnelshift_r(L.hp, np, L.sp) ^ __funnelshift_r(hc, nq, L.sc);
+  const uint32_t x2 = __funnelshift_r(np, np2, L.sp) ^ __funnelshift_r(nq, nq2, L.sc);
+  const bool hit = ok && __funnelshift_r(c0, hc, L.sc) == v;
+  // equal bytes after the first four, up to 8: from the trailing zero bits of x, or of x2 when x is 0 (32 for none)
+  const uint32_t tx = __clz((int)__brev(x)), tx2 = __clz((int)__brev(x2));
+  const uint32_t eq = (tx + (x ? 0u : tx2)) >> 3;
+  L.m = hit ? 4u + eq : 0u;
+  L.more = hit && eq == 8u;
+  L.hp = np2;
+  L.hc = nq2;
+}
+
+__device__ __forceinline__ void lz1_extend(const uint8_t *data, bool before_entry, Lz1Lane &L) {
+  const uint32_t *w = reinterpret_cast<const uint32_t *>(data);
+  if (before_entry) {
+    L.m = 0;
+  } else if (L.more) {
+    uint32_t hp = L.hp, hc = L.hc;
+#pragma unroll 1
+    for (uint32_t k = 4;; k += 2) {
+      const uint32_t np = w[L.ip + k], nq = w[L.ic + k], np2 = w[L.ip + k + 1], nq2 = w[L.ic + k + 1];
+      const uint32_t x = __funnelshift_r(hp, np, L.sp) ^ __funnelshift_r(hc, nq, L.sc);
+      const uint32_t x2 = __funnelshift_r(np, np2, L.sp) ^ __funnelshift_r(nq, nq2, L.sc);
+      if (x) {
+        L.m += (uint32_t)(__ffs((int)x) - 1) >> 3;
+        break;
+      }
+      if (k == LZ_LANE_CAP / 4) {
+        L.m += 4;
+        break;
+      }
+      if (x2) {
+        L.m += 4u + ((uint32_t)(__ffs((int)x2) - 1) >> 3);
+        break;
+      }
+      L.m += 8;
+      hp = np2;
+      hc = nq2;
+    }
+  }
+  if (L.m < LZ_LANE_CAP) L.m = min(L.m, L.limit);
 }
 
 // LPW lanes per window (lane l: window l % (32 / LPW), part l / (32 / LPW)): publish the window's masks, turn
@@ -352,120 +457,107 @@ __global__ void __launch_bounds__(LZ_THREADS, 3)
     uint32_t *grecs = recs + (size_t)chunk * ZB_RECS_PER_CHUNK + (b0 >> 2);  // this piece's record stream
     uint32_t rec_base = 0;
     const uint32_t bl = (uint32_t)lane & (LZ_BATCH_WINDOWS - 1u);
-    for (uint32_t wb = b0; wb < b1; wb += 32) {
+    // the window's masks into this lane's batch slot, and every 16 windows (or at the end) two lanes per window
+    // walk its tokens
+    auto window_done = [&](uint32_t wb, uint32_t sel, uint32_t ism) {
       const uint32_t win = wb >> 5, slot = win & (LZ_BATCH_WINDOWS - 1u);
-      uint32_t sel = 0, ism = 0;
-      if (entry < wb + 32) {
-        const uint32_t p = wb + (uint32_t)lane;
-        const uint32_t nvalid = min(32u, b1 - wb);
-        const uint32_t cur = entry - wb;
-        uint32_t m = 0, c = 0, lit = 0;
-        if (MODE == 2) {
-          // run lengths from one ballot per 32 positions: bit i of eq says byte wb + i equals the byte before it (never
-          // at the chunk's first byte); the run at p is the count of consecutive set bits from p, seen 32 bytes ahead
-          const uint32_t x = doff + p;
-          lit = data[x];
-          const uint32_t eq0 = __ballot_sync(ZB_FULL, p != 0u && lit == data[x - 1u]);
-          const uint32_t eq1 = __ballot_sync(ZB_FULL, data[x + 32u] == data[x + 31u]);
-          const uint32_t ahead = __funnelshift_r(eq0, eq1, (uint32_t)lane);  // bits p .. p + 31
-          const uint32_t run = ahead == ~0u ? (uint32_t)LZ_LANE_CAP : (uint32_t)(__ffs((int)~ahead) - 1);
-          // a run that fills the lane cap is at least that long: lz_select extends it (distance 1) and cuts it there
-          const uint32_t limit = p < b1 ? b1 - p : 0u;
-          const uint32_t r = run < (uint32_t)LZ_LANE_CAP ? min(run, limit) : run;
-          if (p >= entry && r >= 3u && limit >= 3u) m = r;
-          c = p - 1u;
-        }
-        if (MODE == 1) {
-          // this lane's 4 bytes; the word pair stays in registers for the compare below
-          const uint32_t *wp = reinterpret_cast<const uint32_t *>(data) + ((doff + p) >> 2);
-          const uint32_t sp = ((doff + p) & 3u) * 8u;
-          const uint32_t p0 = wp[0], p1 = wp[1];
-          const uint32_t v = __funnelshift_r(p0, p1, sp);
-          lit = v & 255u;
-          const bool can = (p + 4 <= len);
-          const uint32_t h = lz_hash(v);
-          c = table[h];
-          __syncwarp();
-          // Lanes of this window that share a hash store to the same entry in one instruction:
-          // exactly one of them lands, and WHICH is up to the hardware (resolving the winner with
-          // __match_any_sync is a large share of the kernel) ...
-          if (can) table[h] = (uint16_t)p;
-#if ZB_LZ1_RESOLVE_WINNER
-          __syncwarp();
-          // make the outcome independent of the arbitration: the highest position wins (every round strictly
-          // raises the entry, so it ends).  Slows the kernel; off by default because the
-          // arbitration IS fixed on this hardware: the lowest lane lands, which tests/test_gpu_lz1_model.py
-          // asserts token by token (and this variant's tokens under the highest-position rule)
-          for (;;) {
-            const bool lost = can && table[h] < (uint16_t)p;
-            if (!__any_sync(ZB_FULL, lost)) break;
-            if (lost) table[h] = (uint16_t)p;
-            __syncwarp();
-          }
-#endif
-          LZ_CLK(LZS_PROBE)
-          // a match may not cross the piece end (another warp starts its own parse there)
-          const uint32_t limit = p < b1 ? min((uint32_t)ZB_MAX_MATCH, b1 - p) : 0u;
-          if (can && c < p && p - c <= max_dist && p >= entry && limit >= ZB_MIN_MATCH) {
-            // unaligned compare, 8 bytes per step, carrying the upper word of each side; the first step's four words
-            // are loaded with the 4-byte check and every step loads the next one's, so a lane waits for one round of
-            // shared-memory loads per 8 bytes (4 before)
-            const uint32_t *wc = reinterpret_cast<const uint32_t *>(data) + ((doff + c) >> 2);
-            const uint32_t sc = ((doff + c) & 3u) * 8u;
-            uint32_t hp = p1, hc = wc[1];
-            uint32_t np = wp[2], nq = wc[2], np2 = wp[3], nq2 = wc[3];
-            if (__funnelshift_r(wc[0], hc, sc) == v) {
-              m = 4;
-#pragma unroll 1
-              for (int k = 2;; k += 2) {
-                const uint32_t x = __funnelshift_r(hp, np, sp) ^ __funnelshift_r(hc, nq, sc);
-                const uint32_t x2 = __funnelshift_r(np, np2, sp) ^ __funnelshift_r(nq, nq2, sc);
-                if (x) {
-                  m += (uint32_t)(__ffs((int)x) - 1) >> 3;
-                  break;
-                }
-                if (k == LZ_LANE_CAP / 4) {
-                  m += 4;
-                  break;
-                }
-                if (x2) {
-                  m += 4u + ((uint32_t)(__ffs((int)x2) - 1) >> 3);
-                  break;
-                }
-                m += 8;
-                hp = np2;
-                hc = nq2;
-                np = wp[k + 2];
-                nq = wc[k + 2];
-                np2 = wp[k + 3];
-                nq2 = wc[k + 3];
-              }
-              if (m < LZ_LANE_CAP) m = min(m, limit);
-            }
-          }
-          LZ_CLK(LZS_EXTEND)
-        }
-        uint32_t endw;
-        lz_select(data, doff, wb, b1, cur, nvalid, m, p - c, ring + slot * ZB_MATCH_SLOTS, sel, ism, endw);
-        entry = wb + max(endw, nvalid);
-        // level 1 counts the window's literals here, one atomic per lane, from the byte the probe already holds
-        if (MODE != 0 && ((sel & ~ism) >> lane & 1u)) atomicAdd(&whist[lit >> 1], 1u << ((lit & 1u) * 16u));
-        LZ_CLK(LZS_SELECT)
-      }
       if (bl == slot) {
         ksel = sel;
         kism = ism;
       }
-      // ---- every 16 windows (or at the end): two lanes per window walk its tokens ----
       if (slot == LZ_BATCH_WINDOWS - 1u || wb + 32 >= b1) {
         __syncwarp();
         const uint32_t bwin = win - slot + bl;  // this lane's window
-        lz_batch_pass<LZ_BATCH_LPW, MODE == 0>(data + (uint32_t)(doff + (bwin << 5)), bl <= slot, ksel, kism, ring + bl * ZB_MATCH_SLOTS,
-                                    whist, gmask + bwin, grecs, rec_base);
+        lz_batch_pass<LZ_BATCH_LPW, MODE == 0>(data + (uint32_t)(doff + (bwin << 5)), bl <= slot, ksel, kism,
+                                               ring + bl * ZB_MATCH_SLOTS, whist, gmask + bwin, grecs, rec_base);
         ksel = kism = 0;
         __syncwarp();
       }
       LZ_CLK(LZS_BATCH)
+    };
+    if (MODE == 1) {
+      // A one-window software pipeline.  A window whose lanes all stop below the lane cap ends its last match by
+      // wb + 62, so the next window is entered whatever the selection picks: its probe (with its table stores),
+      // 4-byte check and first extension step are then exactly the serial parse's, and are issued together with this
+      // window's selection, in one basic block; only its lanes below the new entry wait for the selection.  A
+      // capped lane (rare), or the piece's last window, drains the pipeline: the next window starts after the
+      // selection, as the first one of the piece does and one after skipped windows.
+      Lz1Lane L;           // window wb's lane, probed and extended by the previous step when `ahead`
+      bool ahead = false;  // warp-uniform
+      for (uint32_t wb = b0; wb < b1; wb += 32) {
+        uint32_t *ring_win = ring + ((wb >> 5) & (LZ_BATCH_WINDOWS - 1u)) * ZB_MATCH_SLOTS;
+        uint32_t sel = 0, ism = 0;
+        if (entry < wb + 32) {
+          const uint32_t p = wb + (uint32_t)lane;
+          const uint32_t nvalid = min(32u, b1 - wb);
+          const uint32_t cur = entry - wb;
+          uint32_t v, endw;
+          bool can;
+          if (!ahead) {
+            lz1_probe(data, table, doff, p, len, L, v, can);
+            LZ_CLK(LZS_PROBE)
+            lz1_check(data, doff, p, b1, max_dist, v, can, L);
+            lz1_extend(data, p < entry, L);
+            LZ_CLK(LZS_EXTEND)
+          }
+          ahead = wb + 32 < b1 && !__any_sync(ZB_FULL, L.m >= LZ_LANE_CAP);
+          if (ahead) {
+            Lz1Lane N;
+            lz1_probe(data, table, doff, p + 32, len, N, v, can);
+            lz1_check(data, doff, p + 32, b1, max_dist, v, can, N);
+            lz_select<false>(data, doff, wb, b1, cur, nvalid, L.m, p - L.c, ring_win, sel, ism, endw);
+            entry = wb + max(endw, nvalid);
+            // the window's literals, one atomic per lane, from the byte the probe already holds
+            uint32_t *hw = &whist[L.lit >> 1];
+            const uint32_t one = 1u << ((L.lit & 1u) * 16u);
+            if ((sel & ~ism) >> lane & 1u) atomicAdd(hw, one);
+            LZ_CLK(LZS_SELECT)
+            lz1_extend(data, p + 32 < entry, N);
+            L = N;
+            LZ_CLK(LZS_EXTEND)
+          } else {
+            lz_select(data, doff, wb, b1, cur, nvalid, L.m, p - L.c, ring_win, sel, ism, endw);
+            entry = wb + max(endw, nvalid);
+            if ((sel & ~ism) >> lane & 1u) atomicAdd(&whist[L.lit >> 1], 1u << ((L.lit & 1u) * 16u));
+            LZ_CLK(LZS_SELECT)
+          }
+        }
+        window_done(wb, sel, ism);
+      }
+    } else {
+      for (uint32_t wb = b0; wb < b1; wb += 32) {
+        uint32_t sel = 0, ism = 0;
+        if (entry < wb + 32) {
+          const uint32_t p = wb + (uint32_t)lane;
+          const uint32_t nvalid = min(32u, b1 - wb);
+          const uint32_t cur = entry - wb;
+          uint32_t m = 0, c = 0, lit = 0;
+          if (MODE == 2) {
+            // run lengths from one ballot per 32 positions: bit i of eq says byte wb + i equals the byte before it
+            // (never at the chunk's first byte); the run at p is the count of consecutive set bits from p, seen 32
+            // bytes ahead
+            const uint32_t x = doff + p;
+            lit = data[x];
+            const uint32_t eq0 = __ballot_sync(ZB_FULL, p != 0u && lit == data[x - 1u]);
+            const uint32_t eq1 = __ballot_sync(ZB_FULL, data[x + 32u] == data[x + 31u]);
+            const uint32_t ahead = __funnelshift_r(eq0, eq1, (uint32_t)lane);  // bits p .. p + 31
+            const uint32_t run = ahead == ~0u ? (uint32_t)LZ_LANE_CAP : (uint32_t)(__ffs((int)~ahead) - 1);
+            // a run that fills the lane cap is at least that long: lz_select extends it (distance 1) and cuts it there
+            const uint32_t limit = p < b1 ? b1 - p : 0u;
+            const uint32_t r = run < (uint32_t)LZ_LANE_CAP ? min(run, limit) : run;
+            if (p >= entry && r >= 3u && limit >= 3u) m = r;
+            c = p - 1u;
+          }
+          uint32_t endw;
+          lz_select(data, doff, wb, b1, cur, nvalid, m, p - c, ring + ((wb >> 5) & (LZ_BATCH_WINDOWS - 1u)) * ZB_MATCH_SLOTS,
+                    sel, ism, endw);
+          entry = wb + max(endw, nvalid);
+          // the run-length parse counts the window's literals here, one atomic per lane
+          if (MODE == 2 && ((sel & ~ism) >> lane & 1u)) atomicAdd(&whist[lit >> 1], 1u << ((lit & 1u) * 16u));
+          LZ_CLK(LZS_SELECT)
+        }
+        window_done(wb, sel, ism);
+      }
     }
   }
   if (lane == 0) {
