@@ -457,6 +457,30 @@ int zb200_compress_batch_device_window(zb200_ctx *ctx, const uint8_t *d_src, con
 int zb200_compress_stream_begin_window(zb200_ctx *ctx, int level, int strategy, int window_bits, int data_format,
                                        int fname_len, zb200_compress_stream **out);
 
+/* ---- optimal parse: the smallest members this library writes (DESIGN.md sections 4 and 5, "k_opt") ----
+ * Each 64 KiB chunk is parsed by a shortest path over its candidate matches under integer bit costs, in two cost
+ * rounds (fixed-code costs, then the code lengths of the first round's histogram), instead of level 9's lazy
+ * matching.  The members are valid gzip / zlib / raw DEFLATE members in the layout of the other calls: one block per
+ * 64 KiB chunk, the smallest of stored, fixed and dynamic, chunks joined by empty stored blocks, the zlib header of
+ * the _window calls (FLEVEL 0).  zb200_compress_bound and zb200_compress_stream_bound bound them.
+ *  - history as at the LZ levels: a chunk sees up to min(32 KiB, 2^window_bits) of the member's earlier bytes; a
+ *    stream's sync flush keeps the history, a full flush drops it.  Matches are 4..258 bytes, at most 2^window_bits
+ *    back, and none crosses the end of its 8 KiB sub-chunk;
+ *  - a member's bytes depend on its input, window_bits, the format and the FNAME length alone (and for a stream on
+ *    its flush offsets and modes, not on how the input was split into writes; a stream writes the one-shot member);
+ *  - an invalid window_bits fails with ZB200_ERR_ARG and leaves statuses alone.  There is no dictionary,
+ *    compress-time index, zb200_compress_batch_h2d or multi-GPU form.
+ * The calls take the arguments of the _window calls without `level` and `strategy`; the stream form is driven by the
+ * zb200_compress_stream_write / _flush / _finish / _free calls. */
+int zb200_compress_batch_optimal(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n,
+                                 int window_bits, int data_format, const uint8_t *fname_lens, uint8_t *dst_base,
+                                 size_t dst_cap, uint64_t *dst_offsets, int *statuses);
+int zb200_compress_batch_device_optimal(zb200_ctx *ctx, const uint8_t *d_src, const uint64_t *src_offsets, size_t n,
+                                        int window_bits, int data_format, const uint8_t *fname_lens, uint8_t *d_dst,
+                                        size_t dst_cap, uint64_t *dst_offsets, int *statuses);
+int zb200_compress_stream_begin_optimal(zb200_ctx *ctx, int window_bits, int data_format, int fname_len,
+                                        zb200_compress_stream **out);
+
 /* ---- device-resident variants (pointers prefixed d_ are device memory on ctx's device;
  * offsets / statuses / sizes stay host arrays).  Used when the data already lives in HBM
  * (bench.py's `value`) and by the multi-GPU sharded path.  The call returns after the

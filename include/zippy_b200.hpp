@@ -204,6 +204,25 @@ inline std::string compress(const std::string &src, int level, CompressedDataFor
   return compress(src.data(), src.size(), level, dataFormat, strategy, windowBits);
 }
 
+// The optimal parse (zb200_compress_batch_optimal): smaller members than level 9, with zlib's window size
+// (windowBits 9..15; 8 for dfZlib means 9).  No strategy, dictionary or index.
+inline std::string compressOptimal(const void *srcp, size_t len, CompressedDataFormat dataFormat, int windowBits = 15) {
+  const uint64_t offs[2] = {0, len};
+  uint64_t out_offs[2] = {0, 0};
+  int st = 0;
+  const uint8_t fl = dataFormat == dfGzip ? (uint8_t)(std::random_device()() % 26) : 0;
+  std::string result(zb200_compress_bound(len, dataFormat) + 64, '\0');
+  uint8_t dummy = 0;
+  detail::check(zb200_compress_batch_optimal(detail::ctx(), len ? static_cast<const uint8_t *>(srcp) : &dummy, offs, 1,
+                                             windowBits, dataFormat, &fl, reinterpret_cast<uint8_t *>(&result[0]),
+                                             result.size(), out_offs, &st));
+  result.resize(out_offs[1]);
+  return result;
+}
+inline std::string compressOptimal(const std::string &src, CompressedDataFormat dataFormat, int windowBits = 15) {
+  return compressOptimal(src.data(), src.size(), dataFormat, windowBits);
+}
+
 // gzip.nim:3-88
 inline void uncompressGzip(std::string &dst, const uint8_t *src, size_t len) {
   auto fail = [] { throw ZippyError(ZB200_ERR_UNCOMPRESS, "Invalid buffer, unable to uncompress"); };
@@ -437,6 +456,12 @@ class CompressStream {
     if (fnameLen < 0) fnameLen = dataFormat == dfGzip ? (int)(std::random_device()() % 26) : 0;
     detail::check(zb200_compress_stream_begin_window(ctx ? ctx : detail::ctx(), level, strategy, windowBits, dataFormat,
                                                      fnameLen, &st_));
+  }
+  // the optimal parse (zb200_compress_stream_begin_optimal), selected by the tag CompressStream::Optimal{}
+  struct Optimal {};
+  CompressStream(Optimal, CompressedDataFormat dataFormat, int windowBits = 15, int fnameLen = -1, zb200_ctx *ctx = nullptr) {
+    if (fnameLen < 0) fnameLen = dataFormat == dfGzip ? (int)(std::random_device()() % 26) : 0;
+    detail::check(zb200_compress_stream_begin_optimal(ctx ? ctx : detail::ctx(), windowBits, dataFormat, fnameLen, &st_));
   }
   // that also writes the member's index (zb200_compress_stream_begin_index): index() after finish()
   CompressStream(int level, CompressedDataFormat dataFormat, int fnameLen, uint64_t indexSpan, zb200_ctx *ctx = nullptr)

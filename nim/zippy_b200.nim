@@ -695,3 +695,31 @@ proc newCompressStream*(level: int, dataFormat: CompressedDataFormat, strategy: 
   let k = if fnameLen < 0: randomFnameLen(dataFormat) else: fnameLen
   check zb200_compress_stream_begin_window(getCtx(), level.cint, strategy.cint, windowBits.cint, dataFormat.cint,
                                            k.cint, result.st.addr)
+
+# ---- optimal parse (include/zippy_b200.h "optimal parse"): smaller members than level 9; windowBits as above; not
+# combined with strategies, dictionaries or compress-time indexes ----
+proc zb200_compress_batch_optimal(ctx: Zb200Ctx, srcBase: pointer, srcOffsets: ptr uint64, n: csize_t,
+                                  windowBits, dataFormat: cint, fnameLens: pointer, dstBase: pointer,
+                                  dstCap: csize_t, dstOffsets: ptr uint64,
+                                  statuses: ptr cint): cint {.importc, cdecl, dynlib: lib.}
+proc zb200_compress_stream_begin_optimal(ctx: Zb200Ctx, windowBits, dataFormat, fnameLen: cint,
+                                         st: ptr Zb200CompressStream): cint {.importc, cdecl, dynlib: lib.}
+
+proc compressOptimal*(src: string, dataFormat: CompressedDataFormat, windowBits = 15): string {.raises: [ZippyError].} =
+  ## one member of zb200_compress_batch_optimal; gzip draws its FNAME length at random, as compress does
+  var
+    offs = [0'u64, src.len.uint64]
+    outOffs = [0'u64, 0'u64]
+    fl = randomFnameLen(dataFormat).uint8
+    dummy: uint8
+  result = newString(zb200_compress_bound(src.len.csize_t, dataFormat.cint).int + 64)
+  check zb200_compress_batch_optimal(getCtx(), (if src.len > 0: src[0].unsafeAddr else: dummy.addr),
+                                     offs[0].addr, 1, windowBits.cint, dataFormat.cint,
+                                     fl.addr, result[0].addr, result.len.csize_t, outOffs[0].addr, nil)
+  result.setLen(outOffs[1].int)
+
+proc newOptimalCompressStream*(dataFormat: CompressedDataFormat, windowBits = 15,
+                               fnameLen = -1): CompressStream {.raises: [ZippyError].} =
+  ## a stream under the optimal parse: zb200_compress_stream_begin_optimal
+  let k = if fnameLen < 0: randomFnameLen(dataFormat) else: fnameLen
+  check zb200_compress_stream_begin_optimal(getCtx(), windowBits.cint, dataFormat.cint, k.cint, result.st.addr)

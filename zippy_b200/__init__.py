@@ -113,6 +113,21 @@ def _params_alone(strategy, window_bits=15, dictionary=None, index_span=None):
     return True
 
 
+def _check_optimal(level, strategy=StrategyDefault, dictionary=None, index_span=None, dictionaries=None):
+    """optimal=True (the optimal parse, zb200_compress_batch_optimal): its members do not depend on the level, which
+    must be an LZ level (-1, 1..9); a strategy, a dictionary or a compress-time index is not combined with it."""
+    if level < -2 or level > 9:
+        raise ZippyError(1, "Invalid compression level %d" % level)
+    if level in (NoCompression, HuffmanOnly):
+        raise ZippyError(22, "the optimal parse is not combined with level %d" % level)
+    if strategy != StrategyDefault:
+        raise ZippyError(22, "the optimal parse is not combined with a compression strategy")
+    if dictionary is not None or dictionaries is not None:
+        raise ZippyError(22, "the optimal parse is not combined with a dictionary")
+    if index_span is not None:
+        raise ZippyError(22, "the optimal parse is not combined with a compress-time index")
+
+
 def _pack(items):
     """list of bytes-like -> (base uint8 array, offsets uint64[n+1])"""
     lens = np.fromiter((len(x) for x in items), dtype=np.uint64, count=len(items))
@@ -155,8 +170,11 @@ class Context:
 
     # ---- batches over host buffers -------------------------------------------------
     def compress_batch(self, base, offsets, level=DefaultCompression, dataFormat=dfGzip, fname_lens=None,
-                       dictionary=None, index_span=None, strategy=StrategyDefault, window_bits=15, dictionaries=None):
+                       dictionary=None, index_span=None, strategy=StrategyDefault, window_bits=15, dictionaries=None,
+                       optimal=False):
         """-> (out uint8 array, out_offsets uint64[n+1]).  fname_lens: per-input gzip FNAME letters (0..25).
+        optimal: the optimal parse, smaller than level 9 (zb200_compress_batch_optimal): any LZ level (-1, 1..9)
+        gives the same bytes; no strategy, dictionary or index.
         strategy: zlib's compression strategy (Strategy*; zb200_compress_batch_window; no dictionary or index).
         window_bits: zlib's window size, 9..15 (8 for zlib: 9); no match reaches more than 2^window_bits back
         (zb200_compress_batch_window; no dictionary or index).
@@ -176,6 +194,15 @@ class Context:
         out = np.empty(int(bound) + (4 * n if with_dicts else 0) + 64, dtype=np.uint8)
         out_offs = np.zeros(n + 1, dtype=np.uint64)
         st = np.zeros(max(n, 1), dtype=np.int32)
+        if optimal:
+            _check_optimal(level, strategy, dictionary, index_span, dictionaries)
+            fl = np.ascontiguousarray(fname_lens, dtype=np.uint8) if fname_lens is not None else None
+            _check(self._h, L.zb200_compress_batch_optimal(self._h, base.ctypes.data, offsets.ctypes.data, n,
+                                                            window_bits, dataFormat,
+                                                            fl.ctypes.data if fl is not None else None,
+                                                            out.ctypes.data, out.size, out_offs.ctypes.data,
+                                                            st.ctypes.data))
+            return out[:int(out_offs[n])], out_offs
         if dictionaries is not None:
             if strategy != StrategyDefault:
                 raise ZippyError(22, "a compression strategy is not combined with a dictionary")
@@ -364,15 +391,22 @@ class Context:
 
     # ---- device-resident batches (raw device pointers; e.g. torch tensor .data_ptr()) ----
     def compress_batch_device(self, d_src, offsets, level, dataFormat, d_dst, dst_cap, fname_lens=None,
-                              index_span=None, strategy=StrategyDefault, window_bits=15):
+                              index_span=None, strategy=StrategyDefault, window_bits=15, optimal=False):
         """-> out_offsets; with index_span also each member's Index (zb200_compress_batch_device_index):
         -> (out_offsets, list of Index).  strategy, window_bits: zlib's compression strategy and window size
-        (zb200_compress_batch_device_window; no index)."""
+        (zb200_compress_batch_device_window; no index).  optimal: the optimal parse
+        (zb200_compress_batch_device_optimal; no strategy or index)."""
         L = _native.lib()
         offsets = np.ascontiguousarray(offsets, dtype=np.uint64)
         n = len(offsets) - 1
         out_offs = np.zeros(n + 1, dtype=np.uint64)
         fl = np.ascontiguousarray(fname_lens, dtype=np.uint8) if fname_lens is not None else None
+        if optimal:
+            _check_optimal(level, strategy, None, index_span)
+            _check(self._h, L.zb200_compress_batch_device_optimal(self._h, d_src, offsets.ctypes.data, n, window_bits,
+                                                                   dataFormat, fl.ctypes.data if fl is not None else None,
+                                                                   d_dst, dst_cap, out_offs.ctypes.data, None))
+            return out_offs
         if _params_alone(strategy, window_bits, None, index_span):
             _check(self._h, L.zb200_compress_batch_device_window(self._h, d_src, offsets.ctypes.data, n, level,
                                                                   strategy, window_bits, dataFormat,
@@ -444,12 +478,12 @@ class Context:
         return {f: getattr(t, f) for f, _ in t._fields_}
 
     # ---- the single-input seam (deflate.nim:207, inflate.nim:268, crc.nim:53, adler32.nim:6) ----
-    def deflate(self, src, level=DefaultCompression, strategy=StrategyDefault, window_bits=15):
+    def deflate(self, src, level=DefaultCompression, strategy=StrategyDefault, window_bits=15, optimal=False):
         L = _native.lib()
         src = _as_u8(src)
-        if strategy != StrategyDefault or window_bits != 15:   # one raw DEFLATE member of the batch call
+        if strategy != StrategyDefault or window_bits != 15 or optimal:   # one raw DEFLATE member of the batch call
             out, _ = self.compress_batch(src, [0, src.size], level, dfDeflate, strategy=strategy,
-                                         window_bits=window_bits)
+                                         window_bits=window_bits, optimal=optimal)
             return out.tobytes()
         cap = L.zb200_deflate_bound(src.size)
         out = np.empty(cap + 8, dtype=np.uint8)
@@ -501,13 +535,21 @@ class CompressStream:
     length is drawn at random, as compress() does (zippy.nim:28-42)."""
 
     def __init__(self, level=DefaultCompression, dataFormat=dfGzip, fname_len=None, ctx=None, dictionary=None,
-                 index_span=None, strategy=StrategyDefault, window_bits=15):
+                 index_span=None, strategy=StrategyDefault, window_bits=15, optimal=False):
         """index_span: also write the member's Index with this span (zb200_compress_stream_begin_index; no
         dictionary), returned by index() after finish().  strategy, window_bits: zlib's compression strategy and
-        window size, kept for the stream's whole life (zb200_compress_stream_begin_window; no dictionary or index)."""
+        window size, kept for the stream's whole life (zb200_compress_stream_begin_window; no dictionary or index).
+        optimal: the optimal parse (zb200_compress_stream_begin_optimal; no strategy, dictionary or index)."""
         self._ctx = ctx if ctx is not None else default_context()
         self._h = ctypes.c_void_p()
         d = _dict(dictionary)
+        if optimal:
+            _check_optimal(level, strategy, d, index_span)
+            if fname_len is None:
+                fname_len = os.urandom(1)[0] % 26 if dataFormat == dfGzip else 0
+            _check(self._ctx._h, _native.lib().zb200_compress_stream_begin_optimal(
+                self._ctx._h, window_bits, dataFormat, fname_len, ctypes.byref(self._h)))
+            return
         if _params_alone(strategy, window_bits, d, index_span):
             if fname_len is None:
                 fname_len = os.urandom(1)[0] % 26 if dataFormat == dfGzip else 0
@@ -834,10 +876,11 @@ def default_context():
 
 # ---- the reference's public procs ------------------------------------------------------
 def compress(src, level=DefaultCompression, dataFormat=dfGzip, dictionary=None, strategy=StrategyDefault,
-             window_bits=15):
+             window_bits=15, optimal=False):
     """zippy.compress (zippy.nim:11-98).  dictionary: a preset dictionary (zlib / raw only; zlib's zdict).
     strategy: zlib's compression strategy (Strategy*), not with a dictionary.  window_bits: zlib's window size
-    (9..15; 8 for zlib means 9): no match reaches more than 2^window_bits back; other than 15 not with a dictionary."""
+    (9..15; 8 for zlib means 9): no match reaches more than 2^window_bits back; other than 15 not with a dictionary.
+    optimal: the optimal parse, smaller than level 9 (any LZ level gives the same bytes; no strategy or dictionary)."""
     if level < -2 or level > 9:
         raise ZippyError(1, "Invalid compression level %d" % level)          # deflate.nim:208-209
     if dataFormat not in (dfGzip, dfZlib, dfDeflate):
@@ -847,7 +890,7 @@ def compress(src, level=DefaultCompression, dataFormat=dfGzip, dictionary=None, 
         fl = [os.urandom(1)[0] % 26]                                         # zippy.nim:28-42
     base, offs = _pack([src])
     out, _ = default_context().compress_batch(base, offs, level, dataFormat, fl, dictionary=dictionary,
-                                              strategy=strategy, window_bits=window_bits)
+                                              strategy=strategy, window_bits=window_bits, optimal=optimal)
     return out.tobytes()
 
 
@@ -881,8 +924,8 @@ def adler32(src):
     return default_context().adler32(src)
 
 
-def deflate(src, level=DefaultCompression, strategy=StrategyDefault, window_bits=15):
-    return default_context().deflate(src, level, strategy, window_bits)
+def deflate(src, level=DefaultCompression, strategy=StrategyDefault, window_bits=15, optimal=False):
+    return default_context().deflate(src, level, strategy, window_bits, optimal)
 
 
 def inflate(src, pos=0):
@@ -890,12 +933,14 @@ def inflate(src, pos=0):
 
 
 def compress_batch(items, level=DefaultCompression, dataFormat=dfGzip, fname_lens=None, dictionary=None,
-                   strategy=StrategyDefault, window_bits=15, dictionaries=None):
+                   strategy=StrategyDefault, window_bits=15, dictionaries=None, optimal=False):
     """list of bytes -> list of bytes (one zippy.compress per item, one GPU launch sequence).  dictionaries: one
-    preset dictionary (bytes-like or None) per item, with any window_bits (zb200_compress_batch_dicts)."""
+    preset dictionary (bytes-like or None) per item, with any window_bits (zb200_compress_batch_dicts).  optimal:
+    the optimal parse (zb200_compress_batch_optimal)."""
     base, offs = _pack(items)
     out, oo = default_context().compress_batch(base, offs, level, dataFormat, fname_lens, dictionary=dictionary,
-                                               strategy=strategy, window_bits=window_bits, dictionaries=dictionaries)
+                                               strategy=strategy, window_bits=window_bits, dictionaries=dictionaries,
+                                               optimal=optimal)
     return [out[int(oo[i]):int(oo[i + 1])].tobytes() for i in range(len(items))]
 
 

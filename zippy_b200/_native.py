@@ -48,6 +48,10 @@ SYMBOLS = {
                                             c_u8p, c_size_t, c_u64p, c_intp]),
     "zb200_compress_batch_device_window": (c_int, [ctypes.c_void_p, c_u8p, c_u64p, c_size_t, c_int, c_int, c_int, c_int,
                                                    c_u8p, c_u8p, c_size_t, c_u64p, c_intp]),
+    "zb200_compress_batch_optimal": (c_int, [ctypes.c_void_p, c_u8p, c_u64p, c_size_t, c_int, c_int, c_u8p, c_u8p,
+                                             c_size_t, c_u64p, c_intp]),
+    "zb200_compress_batch_device_optimal": (c_int, [ctypes.c_void_p, c_u8p, c_u64p, c_size_t, c_int, c_int, c_u8p,
+                                                    c_u8p, c_size_t, c_u64p, c_intp]),
     "zb200_compress_batch_h2d": (c_int, [ctypes.c_void_p, c_u8p, c_u64p, c_size_t, c_int, c_int, c_u8p, c_u8p, c_size_t,
                                          c_u64p, c_intp]),
     "zb200_download": (c_int, [ctypes.c_void_p, c_u8p, c_u8p, c_size_t]),
@@ -83,6 +87,8 @@ SYMBOLS = {
                                                      ctypes.POINTER(ctypes.c_void_p)]),
     "zb200_compress_stream_begin_window": (c_int, [ctypes.c_void_p, c_int, c_int, c_int, c_int, c_int,
                                                    ctypes.POINTER(ctypes.c_void_p)]),
+    "zb200_compress_stream_begin_optimal": (c_int, [ctypes.c_void_p, c_int, c_int, c_int,
+                                                    ctypes.POINTER(ctypes.c_void_p)]),
     "zb200_compress_stream_begin_dict": (c_int, [ctypes.c_void_p, c_int, c_int, c_u8p, c_size_t,
                                                  ctypes.POINTER(ctypes.c_void_p)]),
     "zb200_compress_stream_bound": (c_size_t, [ctypes.c_void_p, c_size_t]),

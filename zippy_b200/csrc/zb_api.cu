@@ -181,6 +181,7 @@ struct zb200_ctx {
   DevBuf src_off, dst_off, out_len, status, expect, kind, ck_out, ck_pieces, ck_first, ck_piece_out, ck_partials;
   DevBuf counter;           // ZbCounters (allocated with the ctx), then uncompress_host_pipelined's per-group counters
   DevBuf in_stage, out_stage, lz2_tables;
+  DevBuf opt_scratch;       // k_opt's per-CTA scratch (the _optimal calls)
   DevBuf carry;             // a compress stream's member carry: [0] in, [1] out
   size_t stream_batch_bytes = ZB_STREAM_BATCH_BYTES;  // pending input at which a stream write launches
   size_t dstream_batch_bytes = ZB_DSTREAM_BATCH_BYTES;  // pending compressed input at which a decompress stream launches
@@ -253,6 +254,7 @@ struct zb200_compress_stream {
   zb200_ctx *ctx = nullptr;
   int level = 0, data_format = 0;
   int strategy = ZB_STRATEGY_DEFAULT;  // folded with the level by zb_strategy_level
+  bool optimal = false;        // begun by zb200_compress_stream_begin_optimal (level 9's history rules, k_opt's parse)
   int window_bits = 15;        // after zb_window_bits: every launch, flush and carried history keeps to it
   uint8_t fname_len = 0;
   size_t batch_bytes = 0;      // launch once this much input is pending
@@ -717,13 +719,15 @@ static int zb_window_bits(int &window_bits, int data_format) {
 // the only host waits are for the small per-group offset arrays that size the D2H copies.
 // sp (host buffers, n == 1 only): the member is one part of a stream; null for every batch call.
 // ix: null, or the records of a compress-time index (k_index_rec after k_scan; ix->rec_first counts the batch's members).
+// optimal: the optimal parse (k_opt); the caller passes level 9, whose history rules it keeps.
 int compress_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint8_t *h_src, const uint64_t *src_offsets,
                     size_t n, int level, int data_format, const uint8_t *fname_lens, uint8_t *d_dst,
                     size_t dst_cap, uint8_t *h_dst, size_t h_dst_cap, uint64_t *dst_offsets, int *statuses,
                     size_t max_group_chunks, StreamPart *sp = nullptr, const ZbIndexWork *ix = nullptr,
-                    int strategy = ZB_STRATEGY_DEFAULT, int window_bits = 15) {
+                    int strategy = ZB_STRATEGY_DEFAULT, int window_bits = 15, bool optimal = false) {
   const auto t_entry = std::chrono::steady_clock::now();
   if (int rc = zb_strategy_level(level, strategy)) return rc;
+  if (optimal) strategy = ZB_STRATEGY_OPTIMAL;
   if (int rc = zb_window_bits(window_bits, data_format)) return rc;
   if (data_format != ZB200_DF_GZIP && data_format != ZB200_DF_ZLIB && data_format != ZB200_DF_DEFLATE)
     return ZB200_ERR_INVALID_FORMAT;
@@ -843,7 +847,8 @@ int compress_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint8_t *h_src, 
   ENSURE(ctx->chunk_off, max_nc * sizeof(uint64_t));
   ENSURE(ctx->member_check, max_nm * sizeof(uint32_t));
   ENSURE(ctx->member_isize, max_nm * sizeof(uint32_t));
-  if (lz) ENSURE(ctx->lz2_tables, zb_lz2_table_bytes(nullptr));
+  if (optimal) ENSURE(ctx->opt_scratch, zb_opt_scratch_bytes(nullptr));
+  else if (lz) ENSURE(ctx->lz2_tables, zb_lz2_table_bytes(nullptr));
   if (sp) ENSURE(ctx->carry, 2 * sizeof(ZbMemberCarry));
   {
     int rc = ensure_group_events(ctx, 3 * ng + 1);
@@ -906,6 +911,7 @@ int compress_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint8_t *h_src, 
     w.out_base_ptr = (const uint64_t *)ctx->group_end.p + gi;
     w.mdict = mdict.empty() ? nullptr : (const ZbMemberDict *)ctx->dict_md.p + g.m0;
     w.dict_hist = dict_hist ? 1 : 0;
+    w.opt_scratch = (uint8_t *)ctx->opt_scratch.p;
     return w;
   };
 
@@ -1167,7 +1173,7 @@ int stream_run(zb200_compress_stream *st, size_t nbytes, bool last, uint8_t *dst
   int rc = compress_locked(ctx, (const uint8_t *)ctx->in_stage.p, st->buf.data(), offs, 1, st->level, st->data_format,
                            &st->fname_len, (uint8_t *)ctx->out_stage.p, ctx->out_stage.cap & ~(size_t)3, dst, dst_cap,
                            dst_offs, nullptr, ctx->host_group_chunks, &sp, st->ix ? &x : nullptr, st->strategy,
-                           st->window_bits);
+                           st->window_bits, st->optimal);
   if (rc) return rc;
   *dst_len = (size_t)dst_offs[1];
   if (st->ix) {
@@ -2810,7 +2816,7 @@ void zb200_shutdown(zb200_ctx *ctx) {
   DevBuf *bufs[] = {&ctx->desc, &ctx->member_first, &ctx->fname, &ctx->masks, &ctx->recs, &ctx->hist, &ctx->chk,
                     &ctx->cb, &ctx->chunk_off, &ctx->member_off, &ctx->member_check, &ctx->member_isize,
                     &ctx->src_off, &ctx->dst_off, &ctx->out_len, &ctx->status, &ctx->expect, &ctx->kind,
-                    &ctx->counter, &ctx->cix_rec, &ctx->cix_crc, &ctx->cix_first, &ctx->cix_out, &ctx->ck_out, &ctx->ck_pieces, &ctx->ck_first, &ctx->ck_piece_out, &ctx->ck_partials, &ctx->in_stage, &ctx->out_stage, &ctx->lz2_tables, &ctx->carry,
+                    &ctx->counter, &ctx->cix_rec, &ctx->cix_crc, &ctx->cix_first, &ctx->cix_out, &ctx->ck_out, &ctx->ck_pieces, &ctx->ck_first, &ctx->ck_piece_out, &ctx->ck_partials, &ctx->in_stage, &ctx->out_stage, &ctx->lz2_tables, &ctx->opt_scratch, &ctx->carry,
                     &ctx->seg_src, &ctx->seg_dst, &ctx->seg_len, &ctx->seg_status, &ctx->seg_kind, &ctx->seg_expect, &ctx->seg_cand, &ctx->skip_mask, &ctx->order, &ctx->mark_scratch, &ctx->mark_segs, &ctx->seg_bits, &ctx->mark_win, &ctx->gate,
                     &ctx->idx_desc, &ctx->idx_out, &ctx->dict_win, &ctx->dict_md};
   for (DevBuf *b : bufs)
@@ -2898,6 +2904,20 @@ int zb200_compress_batch_device_window(zb200_ctx *ctx, const uint8_t *d_src, con
   });
 }
 
+int zb200_compress_batch_device_optimal(zb200_ctx *ctx, const uint8_t *d_src, const uint64_t *src_offsets, size_t n,
+                                        int window_bits, int data_format, const uint8_t *fname_lens, uint8_t *d_dst,
+                                        size_t dst_cap, uint64_t *dst_offsets, int *statuses) {
+  return guarded(ctx, [&]() -> int {
+  if (!ctx || !src_offsets || !dst_offsets || (n && (!d_src || !d_dst))) return ZB200_ERR_ARG;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  DeviceGuard g(ctx->device);
+  ctx->timing.kernel_launches = 0;
+  return compress_locked(ctx, d_src, nullptr, src_offsets, n, 9, data_format, fname_lens, d_dst, dst_cap, nullptr, 0,
+                         dst_offsets, statuses, ctx->dev_group_chunks, nullptr, nullptr, ZB_STRATEGY_DEFAULT, window_bits,
+                         true);
+  });
+}
+
 int zb200_compress_batch_device_strategy(zb200_ctx *ctx, const uint8_t *d_src, const uint64_t *src_offsets, size_t n,
                                          int level, int strategy, int data_format, const uint8_t *fname_lens,
                                          uint8_t *d_dst, size_t dst_cap, uint64_t *dst_offsets, int *statuses) {
@@ -2918,7 +2938,7 @@ static int compress_batch_host(zb200_ctx *ctx, const uint8_t *src_base, const ui
                                int data_format, const uint8_t *dict_base, const uint64_t *dict_offsets, size_t k,
                                const int32_t *dict_of, const uint8_t *fname_lens, uint8_t *dst_base, size_t dst_cap,
                                uint64_t *dst_offsets, int *statuses, int strategy = ZB_STRATEGY_DEFAULT,
-                               int window_bits = 15) {
+                               int window_bits = 15, bool optimal = false) {
   return guarded(ctx, [&]() -> int {
   if (!ctx || !src_offsets || !dst_offsets || (n && (!src_base || !dst_base))) return ZB200_ERR_ARG;
   if (zb_window_bits(window_bits, data_format)) return ZB200_ERR_ARG;
@@ -2957,7 +2977,7 @@ static int compress_batch_host(zb200_ctx *ctx, const uint8_t *src_base, const ui
   int rc = compress_locked(ctx, (const uint8_t *)ctx->in_stage.p, src_base, src_offsets, n, level, data_format,
                            fname_lens, (uint8_t *)ctx->out_stage.p, ctx->out_stage.cap & ~(size_t)3, dst_base,
                            dst_cap, dst_offsets, statuses, ctx->host_group_chunks, nullptr, nullptr, strategy,
-                           window_bits);
+                           window_bits, optimal);
   if (rc) return rc;
   ctx->timing.h2d_ms = ev_ms(ctx->ev[6], ctx->ev[7]);
   ctx->timing.d2h_ms = ev_ms(ctx->ev[8], ctx->ev[9]);
@@ -2986,6 +3006,13 @@ int zb200_compress_batch_window(zb200_ctx *ctx, const uint8_t *src_base, const u
                                 uint8_t *dst_base, size_t dst_cap, uint64_t *dst_offsets, int *statuses) {
   return compress_batch_host(ctx, src_base, src_offsets, n, level, data_format, nullptr, nullptr, 0, nullptr, fname_lens,
                              dst_base, dst_cap, dst_offsets, statuses, strategy, window_bits);
+}
+
+int zb200_compress_batch_optimal(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n,
+                                 int window_bits, int data_format, const uint8_t *fname_lens, uint8_t *dst_base,
+                                 size_t dst_cap, uint64_t *dst_offsets, int *statuses) {
+  return compress_batch_host(ctx, src_base, src_offsets, n, 9, data_format, nullptr, nullptr, 0, nullptr, fname_lens,
+                             dst_base, dst_cap, dst_offsets, statuses, ZB_STRATEGY_DEFAULT, window_bits, true);
 }
 
 int zb200_compress_batch_dict(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n, int level,
@@ -3043,7 +3070,7 @@ int zb200_compress_batch_h2d(zb200_ctx *ctx, const uint8_t *src_base, const uint
 // history in front of the first chunk (LZ levels), exactly as after a sync flush of it, and zlib's header carries it
 static int compress_stream_begin(zb200_ctx *ctx, int level, int data_format, int fname_len, const uint8_t *dict,
                                  size_t dict_len, zb200_compress_stream **out, int strategy = ZB_STRATEGY_DEFAULT,
-                                 int window_bits = 15) {
+                                 int window_bits = 15, bool optimal = false) {
   return guarded(ctx, [&]() -> int {
     if (!ctx || !out || (dict_len && !dict)) return ZB200_ERR_ARG;
     *out = nullptr;
@@ -3058,6 +3085,7 @@ static int compress_stream_begin(zb200_ctx *ctx, int level, int data_format, int
     st->ctx = ctx;
     st->level = level;
     st->strategy = strategy;
+    st->optimal = optimal;
     st->window_bits = window_bits;
     st->data_format = data_format;
     st->fname_len = (uint8_t)fname_len;
@@ -3091,6 +3119,11 @@ int zb200_compress_stream_begin_strategy(zb200_ctx *ctx, int level, int strategy
 int zb200_compress_stream_begin_window(zb200_ctx *ctx, int level, int strategy, int window_bits, int data_format,
                                        int fname_len, zb200_compress_stream **out) {
   return compress_stream_begin(ctx, level, data_format, fname_len, nullptr, 0, out, strategy, window_bits);
+}
+
+int zb200_compress_stream_begin_optimal(zb200_ctx *ctx, int window_bits, int data_format, int fname_len,
+                                        zb200_compress_stream **out) {
+  return compress_stream_begin(ctx, 9, data_format, fname_len, nullptr, 0, out, ZB_STRATEGY_DEFAULT, window_bits, true);
 }
 
 int zb200_compress_stream_begin_dict(zb200_ctx *ctx, int level, int data_format, const uint8_t *dict, size_t dict_len,

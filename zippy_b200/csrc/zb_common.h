@@ -65,6 +65,8 @@ enum {
 enum { ZB_DF_DETECT = 0, ZB_DF_ZLIB = 1, ZB_DF_GZIP = 2, ZB_DF_DEFLATE = 3 };
 // compression strategies: zlib's values (ZB200_STRATEGY_* in zippy_b200.h)
 enum { ZB_STRATEGY_DEFAULT = 0, ZB_STRATEGY_FILTERED = 1, ZB_STRATEGY_HUFFMAN_ONLY = 2, ZB_STRATEGY_RLE = 3, ZB_STRATEGY_FIXED = 4 };
+// the optimal parse (k_opt, the _optimal calls): a work's strategy only, never one a caller can pass
+enum { ZB_STRATEGY_OPTIMAL = 5 };
 
 // RFC 1951 section 3.2.5 tables.
 #define ZB_BASE_LENGTHS                                                                          \

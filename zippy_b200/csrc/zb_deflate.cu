@@ -1640,6 +1640,7 @@ cudaError_t zb_setup_deflate_attrs() {
   if (e == cudaSuccess) e = cudaFuncSetAttribute(k_lz2<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, LZ2_SM_TOTAL);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(k_lz2<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, LZ2_SM_TOTAL);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(k_lz2<false, 6>, cudaFuncAttributeMaxDynamicSharedMemorySize, LZ2_SM_TOTAL);
+  if (e == cudaSuccess) e = zb_setup_opt_attrs();
   // load the remaining kernels now rather than at their first launch (see zb_setup_inflate_attrs)
   cudaFuncAttributes fa;
   if (e == cudaSuccess) e = cudaFuncGetAttributes(&fa, k_huff);
@@ -1651,6 +1652,7 @@ cudaError_t zb_setup_deflate_attrs() {
 }
 cudaError_t zb_launch_lz(const ZbCompressWork &w, cudaStream_t s, bool index_crc) {
   if (w.n_chunks == 0) return cudaSuccess;
+  if (w.strategy == ZB_STRATEGY_OPTIMAL) return zb_launch_opt(w, s);
   if (zb_is_lz_level(w.level)) {
     int grid = 0;
     (void)zb_lz2_table_bytes(&grid);

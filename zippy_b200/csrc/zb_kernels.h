@@ -72,7 +72,8 @@ struct ZbCompressWork {
   uint32_t n_chunks, n_members;
   int level, data_format;
   // ZB_STRATEGY_*, after zb_strategy_level: RLE only at level 1 (k_lz<2>), FILTERED only at the LZ levels (k_lz2<false, 6>),
-  // FIXED at any level but 0 (k_huff: stored or fixed blocks); HUFFMAN_ONLY never (it is level -2)
+  // FIXED at any level but 0 (k_huff: stored or fixed blocks); HUFFMAN_ONLY never (it is level -2); OPTIMAL with
+  // level 9 (k_opt instead of k_lz2)
   int strategy;
   // 2^window_bits (512..32768): no match reaches further back (k_lz<1>, k_lz2), and a zlib header's CINFO states it
   uint32_t max_dist;
@@ -82,6 +83,7 @@ struct ZbCompressWork {
   // history from wend (k_lz2).
   const ZbMemberDict *mdict;
   int dict_hist;               // some chunk is flagged ZB_CHUNK_DICT: the LZ levels run k_lz2<true>
+  uint8_t *opt_scratch;        // strategy ZB_STRATEGY_OPTIMAL: k_opt's per-CTA chain links and path choices (zb_opt_scratch_bytes)
 };
 
 // per-device kernel attributes (dynamic shared memory limits); call with the device current
@@ -102,6 +104,11 @@ size_t zb_lz2_table_bytes(int *grid_out);
 // index_crc: the chunk checksums also hold the raw CRC-32 whatever the format (a compress-time index needs it)
 cudaError_t zb_launch_lz(const ZbCompressWork &w, cudaStream_t s, bool index_crc = false);
 cudaError_t zb_launch_huff(const ZbCompressWork &w, cudaStream_t s);
+// the optimal parse (zb_optimal.cu): k_opt writes what k_lz2 writes; its scratch is opt_scratch, grid x (96 KiB of u16
+// links + 64 KiB of u32 choices)
+size_t zb_opt_scratch_bytes(int *grid_out);
+cudaError_t zb_setup_opt_attrs();
+cudaError_t zb_launch_opt(const ZbCompressWork &w, cudaStream_t s);
 cudaError_t zb_launch_scan(const ZbCompressWork &w, cudaStream_t s);
 cudaError_t zb_launch_pack(const ZbCompressWork &w, cudaStream_t s);
 // A compress-time index (k_index_rec, after k_scan): the access-point records of zb200_index_build's recorder
