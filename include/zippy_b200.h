@@ -481,6 +481,45 @@ int zb200_compress_batch_device_optimal(zb200_ctx *ctx, const uint8_t *d_src, co
 int zb200_compress_stream_begin_optimal(zb200_ctx *ctx, int window_bits, int data_format, int fname_len,
                                         zb200_compress_stream **out);
 
+/* ---- rsyncable compression: content-defined chunk starts (DESIGN.md sections 4 and 5, "Rsyncable") ----
+ * The _rsyncable calls write one ordinary gzip / zlib / raw DEFLATE member per input, in the layout of the other
+ * calls (one block per chunk, chunks joined by empty stored blocks), but a member's chunks start where its content
+ * says, not every 64 KiB.  An edit then changes only the compressed bytes near it: the chunks before it keep their
+ * bytes, and so do the chunks from the first cut at which the two inputs agree again, as with gzip --rsyncable.
+ * The rule, for member bytes m[0..L), is a format promise (it does not change):
+ *  - G[b], b = 0..255, is the (b + 1)-th output of splitmix64 started from state 0: each step adds
+ *    0x9E3779B97F4A7C15 to the state, then z ^= z >> 30; z *= 0xBF58476D1CE4E5B9; z ^= z >> 27;
+ *    z *= 0x94D049BB133111EB; z ^= z >> 31;
+ *  - h(0) = 0 and h(p) = 2 h(p - 1) + G[m[p - 1]] mod 2^64 (so h(p) depends on the 64 bytes before p alone);
+ *  - p is a candidate if 0 < p < L and h(p) >> 48 == 0;
+ *  - a candidate p is an accepted cut if p >= 16384 (MIN) and no other candidate lies in (p - MIN, p);
+ *  - each consecutive pair a < b of {0} + cuts + {L} gives the chunk starts a, a + 65536, a + 2 * 65536, ... below
+ *    b.  An empty member is one empty chunk at 0.  Without cuts this is the 64 KiB grid of the other calls.
+ * So a member of L bytes has at most zb200_rsyncable_chunks_bound(L) = ceil(L / 65536) + floor(L / 16384) chunks
+ * (1 for L = 0).  At levels -1 and 2..9 a chunk sees up to 32 KiB of the member in front of its start as history.
+ * A member's bytes depend on its input, level, format and FNAME length alone.  zb200_compress_bound can be too small
+ * for these members; zb200_compress_bound_rsyncable bounds them.  gzip headers are byte-stable only with fixed
+ * fname_lens (compress() in the language bindings draws the FNAME length at random), or in the zlib and raw formats.
+ * The host-buffer call copies the whole batch in before it compresses (the map needs every byte first), so it does
+ * not overlap copy-in with compression.  There is no stream, dictionary, strategy, window size, compress-time index,
+ * optimal-parse, zb200_compress_batch_h2d or multi-GPU form.  The compress calls take the arguments of
+ * zb200_compress_batch / zb200_compress_batch_device. */
+int zb200_compress_batch_rsyncable(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n,
+                                   int level, int data_format, const uint8_t *fname_lens, uint8_t *dst_base,
+                                   size_t dst_cap, uint64_t *dst_offsets, int *statuses);
+int zb200_compress_batch_device_rsyncable(zb200_ctx *ctx, const uint8_t *d_src, const uint64_t *src_offsets, size_t n,
+                                          int level, int data_format, const uint8_t *fname_lens, uint8_t *d_dst,
+                                          size_t dst_cap, uint64_t *dst_offsets, int *statuses);
+size_t zb200_compress_bound_rsyncable(size_t len, int data_format);
+size_t zb200_rsyncable_chunks_bound(size_t len);
+/* The chunk map the _rsyncable calls compress by (the same code path), for callers that index or deduplicate by
+ * chunk: counts[i] receives member i's chunk count, and starts its chunk starts (positions in the member, ascending,
+ * the first 0), member after member with nothing between.  starts_cap is the room in starts (entries); the sum of
+ * zb200_rsyncable_chunks_bound over the members always suffices.  ZB200_ERR_DST_TOO_SMALL, with counts filled, when
+ * the starts do not fit. */
+int zb200_rsyncable_chunks(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n,
+                           uint64_t *counts, uint64_t *starts, size_t starts_cap);
+
 /* ---- device-resident variants (pointers prefixed d_ are device memory on ctx's device;
  * offsets / statuses / sizes stay host arrays).  Used when the data already lives in HBM
  * (bench.py's `value`) and by the multi-GPU sharded path.  The call returns after the

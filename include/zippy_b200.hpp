@@ -223,6 +223,52 @@ inline std::string compressOptimal(const std::string &src, CompressedDataFormat 
   return compressOptimal(src.data(), src.size(), dataFormat, windowBits);
 }
 
+// Rsyncable compression (zb200_compress_batch_rsyncable): chunk starts taken from the content, so an edit changes
+// only the compressed bytes near it.  Any level and format; a gzip member's FNAME length is drawn at random, as
+// compress() does (fnameLen >= 0 fixes it, for byte-stable gzip output).
+inline std::string compressRsyncable(const void *srcp, size_t len, int level = DefaultCompression,
+                                     CompressedDataFormat dataFormat = dfGzip, int fnameLen = -1) {
+  const uint64_t offs[2] = {0, len};
+  uint64_t out_offs[2] = {0, 0};
+  int st = 0;
+  const uint8_t fl = fnameLen >= 0 ? (uint8_t)fnameLen
+                                   : dataFormat == dfGzip ? (uint8_t)(std::random_device()() % 26) : 0;
+  std::string result(zb200_compress_bound_rsyncable(len, dataFormat) + 64, '\0');
+  uint8_t dummy = 0;
+  detail::check(zb200_compress_batch_rsyncable(detail::ctx(), len ? static_cast<const uint8_t *>(srcp) : &dummy, offs,
+                                               1, level, dataFormat, &fl, reinterpret_cast<uint8_t *>(&result[0]),
+                                               result.size(), out_offs, &st));
+  result.resize(out_offs[1]);
+  return result;
+}
+inline std::string compressRsyncable(const std::string &src, int level = DefaultCompression,
+                                     CompressedDataFormat dataFormat = dfGzip, int fnameLen = -1) {
+  return compressRsyncable(src.data(), src.size(), level, dataFormat, fnameLen);
+}
+// one member per input, one launch sequence; fnameLens: one gzip FNAME length (0..25) per input, or empty for none
+inline std::vector<std::string> compressRsyncableBatch(const std::vector<std::string> &srcs, int level = DefaultCompression,
+                                                      CompressedDataFormat dataFormat = dfGzip,
+                                                      const std::vector<uint8_t> &fnameLens = {}) {
+  std::vector<uint64_t> offs(srcs.size() + 1, 0), out_offs(srcs.size() + 1, 0);
+  std::string all;
+  size_t cap = 64;
+  for (size_t i = 0; i < srcs.size(); i++) {
+    all += srcs[i];
+    offs[i + 1] = all.size();
+    cap += zb200_compress_bound_rsyncable(srcs[i].size(), dataFormat) + 64;
+  }
+  std::vector<int> st(srcs.size() + 1, 0);
+  std::string out(cap, '\0');
+  uint8_t dummy = 0;
+  detail::check(zb200_compress_batch_rsyncable(
+      detail::ctx(), all.empty() ? &dummy : reinterpret_cast<const uint8_t *>(all.data()), offs.data(), srcs.size(),
+      level, dataFormat, fnameLens.empty() ? nullptr : fnameLens.data(), reinterpret_cast<uint8_t *>(&out[0]),
+      out.size(), out_offs.data(), st.data()));
+  std::vector<std::string> result;
+  for (size_t i = 0; i < srcs.size(); i++) result.push_back(out.substr(out_offs[i], out_offs[i + 1] - out_offs[i]));
+  return result;
+}
+
 // gzip.nim:3-88
 inline void uncompressGzip(std::string &dst, const uint8_t *src, size_t len) {
   auto fail = [] { throw ZippyError(ZB200_ERR_UNCOMPRESS, "Invalid buffer, unable to uncompress"); };

@@ -723,3 +723,25 @@ proc newOptimalCompressStream*(dataFormat: CompressedDataFormat, windowBits = 15
   ## a stream under the optimal parse: zb200_compress_stream_begin_optimal
   let k = if fnameLen < 0: randomFnameLen(dataFormat) else: fnameLen
   check zb200_compress_stream_begin_optimal(getCtx(), windowBits.cint, dataFormat.cint, k.cint, result.st.addr)
+
+# ---- rsyncable compression (include/zippy_b200.h "rsyncable compression"): chunk starts taken from the content, so
+# an edit changes only the compressed bytes near it; any level and format ----
+proc zb200_compress_batch_rsyncable(ctx: Zb200Ctx, srcBase: pointer, srcOffsets: ptr uint64, n: csize_t,
+                                    level, dataFormat: cint, fnameLens: pointer, dstBase: pointer,
+                                    dstCap: csize_t, dstOffsets: ptr uint64,
+                                    statuses: ptr cint): cint {.importc, cdecl, dynlib: lib.}
+proc zb200_compress_bound_rsyncable(len: csize_t, dataFormat: cint): csize_t {.importc, cdecl, dynlib: lib.}
+
+proc compressRsyncable*(src: string, level = DefaultCompression, dataFormat = dfGzip,
+                        fnameLen = -1): string {.raises: [ZippyError].} =
+  ## one member of zb200_compress_batch_rsyncable; gzip draws its FNAME length at random unless fnameLen >= 0
+  var
+    offs = [0'u64, src.len.uint64]
+    outOffs = [0'u64, 0'u64]
+    fl = (if fnameLen >= 0: fnameLen else: randomFnameLen(dataFormat)).uint8
+    dummy: uint8
+  result = newString(zb200_compress_bound_rsyncable(src.len.csize_t, dataFormat.cint).int + 64)
+  check zb200_compress_batch_rsyncable(getCtx(), (if src.len > 0: src[0].unsafeAddr else: dummy.addr),
+                                       offs[0].addr, 1, level.cint, dataFormat.cint,
+                                       fl.addr, result[0].addr, result.len.csize_t, outOffs[0].addr, nil)
+  result.setLen(outOffs[1].int)

@@ -32,7 +32,7 @@ StrategyDefault, StrategyFiltered, StrategyHuffmanOnly, StrategyRle, StrategyFix
 
 __all__ = ["compress", "uncompress", "crc32", "adler32", "deflate", "inflate", "compress_batch", "uncompress_batch",
            "uncompressed_sizes", "checksum_batch", "ZippyError", "Context", "CompressStream", "DecompressStream",
-           "compress_with_index", "compress_batch_with_index",
+           "compress_with_index", "compress_batch_with_index", "rsyncable_chunks",
            "MultiGpu", "Index", "dfDetect",
            "dfZlib", "dfGzip",
            "dfDeflate", "NoCompression", "BestSpeed", "BestCompression", "DefaultCompression", "HuffmanOnly",
@@ -128,6 +128,19 @@ def _check_optimal(level, strategy=StrategyDefault, dictionary=None, index_span=
         raise ZippyError(22, "the optimal parse is not combined with a compress-time index")
 
 
+def _check_rsyncable(strategy=StrategyDefault, window_bits=15, dictionary=None, index_span=None, dictionaries=None,
+                     optimal=False):
+    """rsyncable=True (content-defined chunk starts, zb200_compress_batch_rsyncable) is combined with every level and
+    format, and with none of these."""
+    for bad, what in ((dictionary is not None or dictionaries is not None, "a dictionary"),
+                      (index_span is not None, "a compress-time index"),
+                      (strategy != StrategyDefault, "a compression strategy"),
+                      (window_bits != 15, "a window size other than 15"),
+                      (optimal, "the optimal parse")):
+        if bad:
+            raise ZippyError(22, "rsyncable compression is not combined with " + what)
+
+
 def _pack(items):
     """list of bytes-like -> (base uint8 array, offsets uint64[n+1])"""
     lens = np.fromiter((len(x) for x in items), dtype=np.uint64, count=len(items))
@@ -171,8 +184,11 @@ class Context:
     # ---- batches over host buffers -------------------------------------------------
     def compress_batch(self, base, offsets, level=DefaultCompression, dataFormat=dfGzip, fname_lens=None,
                        dictionary=None, index_span=None, strategy=StrategyDefault, window_bits=15, dictionaries=None,
-                       optimal=False):
+                       optimal=False, rsyncable=False):
         """-> (out uint8 array, out_offsets uint64[n+1]).  fname_lens: per-input gzip FNAME letters (0..25).
+        rsyncable: content-defined chunk starts, so an edit changes only the compressed bytes near it
+        (zb200_compress_batch_rsyncable; any level and format; no strategy, window size, dictionary, index or
+        optimal parse).
         optimal: the optimal parse, smaller than level 9 (zb200_compress_batch_optimal): any LZ level (-1, 1..9)
         gives the same bytes; no strategy, dictionary or index.
         strategy: zlib's compression strategy (Strategy*; zb200_compress_batch_window; no dictionary or index).
@@ -187,13 +203,23 @@ class Context:
         base = _as_u8(base)
         offsets = np.ascontiguousarray(offsets, dtype=np.uint64)
         n = len(offsets) - 1
-        bound = sum(L.zb200_compress_bound(int(offsets[i + 1] - offsets[i]), dataFormat) for i in range(n)) \
-            if n <= 4096 else int(L.zb200_compress_bound(int(offsets[-1] - offsets[0]), dataFormat)) + 64 * n
+        if rsyncable:
+            _check_rsyncable(strategy, window_bits, dictionary, index_span, dictionaries, optimal)
+        fbound = L.zb200_compress_bound_rsyncable if rsyncable else L.zb200_compress_bound
+        bound = sum(fbound(int(offsets[i + 1] - offsets[i]), dataFormat) for i in range(n)) \
+            if n <= 4096 else int(fbound(int(offsets[-1] - offsets[0]), dataFormat)) + 64 * n
         _one_table(dictionary, dictionaries)
         with_dicts = _dict(dictionary) is not None or dictionaries is not None
         out = np.empty(int(bound) + (4 * n if with_dicts else 0) + 64, dtype=np.uint8)
         out_offs = np.zeros(n + 1, dtype=np.uint64)
         st = np.zeros(max(n, 1), dtype=np.int32)
+        if rsyncable:
+            fl = np.ascontiguousarray(fname_lens, dtype=np.uint8) if fname_lens is not None else None
+            _check(self._h, L.zb200_compress_batch_rsyncable(self._h, base.ctypes.data, offsets.ctypes.data, n, level,
+                                                              dataFormat, fl.ctypes.data if fl is not None else None,
+                                                              out.ctypes.data, out.size, out_offs.ctypes.data,
+                                                              st.ctypes.data))
+            return out[:int(out_offs[n])], out_offs
         if optimal:
             _check_optimal(level, strategy, dictionary, index_span, dictionaries)
             fl = np.ascontiguousarray(fname_lens, dtype=np.uint8) if fname_lens is not None else None
@@ -391,16 +417,26 @@ class Context:
 
     # ---- device-resident batches (raw device pointers; e.g. torch tensor .data_ptr()) ----
     def compress_batch_device(self, d_src, offsets, level, dataFormat, d_dst, dst_cap, fname_lens=None,
-                              index_span=None, strategy=StrategyDefault, window_bits=15, optimal=False):
+                              index_span=None, strategy=StrategyDefault, window_bits=15, optimal=False,
+                              rsyncable=False):
         """-> out_offsets; with index_span also each member's Index (zb200_compress_batch_device_index):
         -> (out_offsets, list of Index).  strategy, window_bits: zlib's compression strategy and window size
         (zb200_compress_batch_device_window; no index).  optimal: the optimal parse
-        (zb200_compress_batch_device_optimal; no strategy or index)."""
+        (zb200_compress_batch_device_optimal; no strategy or index).  rsyncable: content-defined chunk starts
+        (zb200_compress_batch_device_rsyncable; size d_dst by zb200_compress_bound_rsyncable; no strategy, window
+        size, index or optimal parse)."""
         L = _native.lib()
         offsets = np.ascontiguousarray(offsets, dtype=np.uint64)
         n = len(offsets) - 1
         out_offs = np.zeros(n + 1, dtype=np.uint64)
         fl = np.ascontiguousarray(fname_lens, dtype=np.uint8) if fname_lens is not None else None
+        if rsyncable:
+            _check_rsyncable(strategy, window_bits, None, index_span, None, optimal)
+            _check(self._h, L.zb200_compress_batch_device_rsyncable(self._h, d_src, offsets.ctypes.data, n, level,
+                                                                     dataFormat,
+                                                                     fl.ctypes.data if fl is not None else None,
+                                                                     d_dst, dst_cap, out_offs.ctypes.data, None))
+            return out_offs
         if optimal:
             _check_optimal(level, strategy, None, index_span)
             _check(self._h, L.zb200_compress_batch_device_optimal(self._h, d_src, offsets.ctypes.data, n, window_bits,
@@ -477,13 +513,30 @@ class Context:
         _check(self._h, _native.lib().zb200_last_timing(self._h, ctypes.byref(t)))
         return {f: getattr(t, f) for f, _ in t._fields_}
 
+    def rsyncable_chunks(self, base, offsets):
+        """The chunk starts the rsyncable compress calls cut each member base[offsets[i], offsets[i + 1]) at
+        (zb200_rsyncable_chunks): -> list of uint64 arrays, positions in the member, ascending, the first 0."""
+        L = _native.lib()
+        base = _as_u8(base)
+        offsets = np.ascontiguousarray(offsets, dtype=np.uint64)
+        n = len(offsets) - 1
+        cap = sum(L.zb200_rsyncable_chunks_bound(int(offsets[i + 1] - offsets[i])) for i in range(n))
+        counts = np.zeros(max(n, 1), dtype=np.uint64)
+        starts = np.zeros(max(cap, 1), dtype=np.uint64)
+        _check(self._h, L.zb200_rsyncable_chunks(self._h, base.ctypes.data, offsets.ctypes.data, n, counts.ctypes.data,
+                                                  starts.ctypes.data, cap))
+        at = np.zeros(n + 1, dtype=np.uint64)
+        np.cumsum(counts[:n], out=at[1:])
+        return [starts[int(at[i]):int(at[i + 1])].copy() for i in range(n)]
+
     # ---- the single-input seam (deflate.nim:207, inflate.nim:268, crc.nim:53, adler32.nim:6) ----
-    def deflate(self, src, level=DefaultCompression, strategy=StrategyDefault, window_bits=15, optimal=False):
+    def deflate(self, src, level=DefaultCompression, strategy=StrategyDefault, window_bits=15, optimal=False,
+                rsyncable=False):
         L = _native.lib()
         src = _as_u8(src)
-        if strategy != StrategyDefault or window_bits != 15 or optimal:   # one raw DEFLATE member of the batch call
+        if strategy != StrategyDefault or window_bits != 15 or optimal or rsyncable:   # one raw DEFLATE member of the batch call
             out, _ = self.compress_batch(src, [0, src.size], level, dfDeflate, strategy=strategy,
-                                         window_bits=window_bits, optimal=optimal)
+                                         window_bits=window_bits, optimal=optimal, rsyncable=rsyncable)
             return out.tobytes()
         cap = L.zb200_deflate_bound(src.size)
         out = np.empty(cap + 8, dtype=np.uint8)
@@ -876,11 +929,14 @@ def default_context():
 
 # ---- the reference's public procs ------------------------------------------------------
 def compress(src, level=DefaultCompression, dataFormat=dfGzip, dictionary=None, strategy=StrategyDefault,
-             window_bits=15, optimal=False):
+             window_bits=15, optimal=False, rsyncable=False):
     """zippy.compress (zippy.nim:11-98).  dictionary: a preset dictionary (zlib / raw only; zlib's zdict).
     strategy: zlib's compression strategy (Strategy*), not with a dictionary.  window_bits: zlib's window size
     (9..15; 8 for zlib means 9): no match reaches more than 2^window_bits back; other than 15 not with a dictionary.
-    optimal: the optimal parse, smaller than level 9 (any LZ level gives the same bytes; no strategy or dictionary)."""
+    optimal: the optimal parse, smaller than level 9 (any LZ level gives the same bytes; no strategy or dictionary).
+    rsyncable: content-defined chunk starts (as gzip --rsyncable), so an edit to src changes only the compressed bytes
+    near it; any level and format, no dictionary, strategy, window size or optimal parse.  A gzip member's FNAME length
+    is still drawn at random: byte-stable gzip output needs compress_batch(..., fname_lens=...), or dfZlib / dfDeflate."""
     if level < -2 or level > 9:
         raise ZippyError(1, "Invalid compression level %d" % level)          # deflate.nim:208-209
     if dataFormat not in (dfGzip, dfZlib, dfDeflate):
@@ -890,7 +946,8 @@ def compress(src, level=DefaultCompression, dataFormat=dfGzip, dictionary=None, 
         fl = [os.urandom(1)[0] % 26]                                         # zippy.nim:28-42
     base, offs = _pack([src])
     out, _ = default_context().compress_batch(base, offs, level, dataFormat, fl, dictionary=dictionary,
-                                              strategy=strategy, window_bits=window_bits, optimal=optimal)
+                                              strategy=strategy, window_bits=window_bits, optimal=optimal,
+                                              rsyncable=rsyncable)
     return out.tobytes()
 
 
@@ -924,8 +981,8 @@ def adler32(src):
     return default_context().adler32(src)
 
 
-def deflate(src, level=DefaultCompression, strategy=StrategyDefault, window_bits=15, optimal=False):
-    return default_context().deflate(src, level, strategy, window_bits, optimal)
+def deflate(src, level=DefaultCompression, strategy=StrategyDefault, window_bits=15, optimal=False, rsyncable=False):
+    return default_context().deflate(src, level, strategy, window_bits, optimal, rsyncable)
 
 
 def inflate(src, pos=0):
@@ -933,15 +990,22 @@ def inflate(src, pos=0):
 
 
 def compress_batch(items, level=DefaultCompression, dataFormat=dfGzip, fname_lens=None, dictionary=None,
-                   strategy=StrategyDefault, window_bits=15, dictionaries=None, optimal=False):
+                   strategy=StrategyDefault, window_bits=15, dictionaries=None, optimal=False, rsyncable=False):
     """list of bytes -> list of bytes (one zippy.compress per item, one GPU launch sequence).  dictionaries: one
     preset dictionary (bytes-like or None) per item, with any window_bits (zb200_compress_batch_dicts).  optimal:
-    the optimal parse (zb200_compress_batch_optimal)."""
+    the optimal parse (zb200_compress_batch_optimal).  rsyncable: content-defined chunk starts
+    (zb200_compress_batch_rsyncable)."""
     base, offs = _pack(items)
     out, oo = default_context().compress_batch(base, offs, level, dataFormat, fname_lens, dictionary=dictionary,
                                                strategy=strategy, window_bits=window_bits, dictionaries=dictionaries,
-                                               optimal=optimal)
+                                               optimal=optimal, rsyncable=rsyncable)
     return [out[int(oo[i]):int(oo[i + 1])].tobytes() for i in range(len(items))]
+
+
+def rsyncable_chunks(items):
+    """list of bytes -> one uint64 array per item: the chunk starts compress(..., rsyncable=True) cuts it at."""
+    base, offs = _pack(items)
+    return default_context().rsyncable_chunks(base, offs)
 
 
 def uncompress_batch(items, dataFormat=dfDetect, dictionary=None, dictionaries=None):

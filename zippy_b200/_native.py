@@ -52,6 +52,13 @@ SYMBOLS = {
                                              c_size_t, c_u64p, c_intp]),
     "zb200_compress_batch_device_optimal": (c_int, [ctypes.c_void_p, c_u8p, c_u64p, c_size_t, c_int, c_int, c_u8p,
                                                     c_u8p, c_size_t, c_u64p, c_intp]),
+    "zb200_compress_batch_rsyncable": (c_int, [ctypes.c_void_p, c_u8p, c_u64p, c_size_t, c_int, c_int, c_u8p, c_u8p,
+                                               c_size_t, c_u64p, c_intp]),
+    "zb200_compress_batch_device_rsyncable": (c_int, [ctypes.c_void_p, c_u8p, c_u64p, c_size_t, c_int, c_int, c_u8p,
+                                                      c_u8p, c_size_t, c_u64p, c_intp]),
+    "zb200_compress_bound_rsyncable": (c_size_t, [c_size_t, c_int]),
+    "zb200_rsyncable_chunks_bound": (c_size_t, [c_size_t]),
+    "zb200_rsyncable_chunks": (c_int, [ctypes.c_void_p, c_u8p, c_u64p, c_size_t, c_u64p, c_u64p, c_size_t]),
     "zb200_compress_batch_h2d": (c_int, [ctypes.c_void_p, c_u8p, c_u64p, c_size_t, c_int, c_int, c_u8p, c_u8p, c_size_t,
                                          c_u64p, c_intp]),
     "zb200_download": (c_int, [ctypes.c_void_p, c_u8p, c_u8p, c_size_t]),

@@ -182,6 +182,7 @@ struct zb200_ctx {
   DevBuf counter;           // ZbCounters (allocated with the ctx), then uncompress_host_pipelined's per-group counters
   DevBuf in_stage, out_stage, lz2_tables;
   DevBuf opt_scratch;       // k_opt's per-CTA scratch (the _optimal calls)
+  DevBuf rs_meta, rs_tiles, rs_counts, rs_starts;  // the rsyncable chunk map (rsync_chunks_locked)
   DevBuf carry;             // a compress stream's member carry: [0] in, [1] out
   size_t stream_batch_bytes = ZB_STREAM_BATCH_BYTES;  // pending input at which a stream write launches
   size_t dstream_batch_bytes = ZB_DSTREAM_BATCH_BYTES;  // pending compressed input at which a decompress stream launches
@@ -486,6 +487,12 @@ struct Group {
   uint64_t in_lo, in_hi;  // source byte range
 };
 
+// The chunk starts of an rsyncable batch (rsync_chunks_locked): member i's count[i] starts, member positions in
+// ascending order from 0, are starts[off[i]] .. starts[off[i] + count[i] - 1]; off[i + 1] - off[i] = zb_rsync_cap.
+struct RsyncMap {
+  std::vector<uint64_t> count, off, starts;
+};
+
 // One launch of a compress stream (zb200_compress_stream_*): a run of chunks of ONE member that continues
 // what earlier launches compressed; only the run's last chunk may be short (the end of a flush segment, or of
 // the member).  The source holds `hist` bytes (0..32768) of the member's preceding input in front of the run
@@ -720,11 +727,14 @@ static int zb_window_bits(int &window_bits, int data_format) {
 // sp (host buffers, n == 1 only): the member is one part of a stream; null for every batch call.
 // ix: null, or the records of a compress-time index (k_index_rec after k_scan; ix->rec_first counts the batch's members).
 // optimal: the optimal parse (k_opt); the caller passes level 9, whose history rules it keeps.
+// rs (batch calls only): the members' chunk starts (an rsyncable batch) instead of the 64 KiB grid; at the LZ levels a
+// chunk sees up to 32 KiB of the member in front of its start as history.
 int compress_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint8_t *h_src, const uint64_t *src_offsets,
                     size_t n, int level, int data_format, const uint8_t *fname_lens, uint8_t *d_dst,
                     size_t dst_cap, uint8_t *h_dst, size_t h_dst_cap, uint64_t *dst_offsets, int *statuses,
                     size_t max_group_chunks, StreamPart *sp = nullptr, const ZbIndexWork *ix = nullptr,
-                    int strategy = ZB_STRATEGY_DEFAULT, int window_bits = 15, bool optimal = false) {
+                    int strategy = ZB_STRATEGY_DEFAULT, int window_bits = 15, bool optimal = false,
+                    const RsyncMap *rs = nullptr) {
   const auto t_entry = std::chrono::steady_clock::now();
   if (int rc = zb_strategy_level(level, strategy)) return rc;
   if (optimal) strategy = ZB_STRATEGY_OPTIMAL;
@@ -759,9 +769,12 @@ int compress_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint8_t *h_src, 
   // One pass over the members validates their offsets and writes the descriptors and member_first entries straight
   // into pinned memory, so that their upload is a true asynchronous copy; the member offsets come back at its
   // start.  With offsets that do not decrease a member of len bytes has at most len / 64 KiB + 1 chunks, so the
-  // batch at most nc_cap; member_first holds n entries plus one per group, and a group holds at least one member.
+  // batch at most nc_cap (rsyncable: len / MIN more, zb_rsync_cap); member_first holds n entries plus one per group,
+  // and a group holds at least one member.
   auto chunks_of = [](uint64_t len) { return len == 0 ? (size_t)1 : (size_t)((len + ZB_CHUNK_BYTES - 1) / ZB_CHUNK_BYTES); };
-  const size_t nc_cap = n + (size_t)((src_offsets[n] - src_offsets[0]) / ZB_CHUNK_BYTES), nfirst_cap = 2 * n;
+  const uint64_t total_in = src_offsets[n] - src_offsets[0];
+  const size_t nc_cap = n + (size_t)(total_in / ZB_CHUNK_BYTES) + (rs ? (size_t)(total_in / ZB_RSYNC_MIN) : 0),
+               nfirst_cap = 2 * n;
   {
     int rc = ensure_pinned(ctx, nfirst_cap * (sizeof(uint64_t) + sizeof(uint32_t)) + sizeof(ZbMemberCarry) +
                                     nc_cap * sizeof(ZbChunkDesc) + 64);
@@ -778,7 +791,7 @@ int compress_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint8_t *h_src, 
   // used: the plan stops at the first such member)
   size_t chunks_left = 0;
   if (h_src)
-    for (size_t i = 0; i < n; i++) chunks_left += chunks_of(src_offsets[i + 1] - src_offsets[i]);
+    for (size_t i = 0; i < n; i++) chunks_left += rs ? (size_t)rs->count[i] : chunks_of(src_offsets[i + 1] - src_offsets[i]);
   const size_t group_cap = max_group_chunks;
   for (size_t m0 = 0; m0 < n;) {
     // host pipeline: the work after the last H2D (kernels + D2H of the last group) is not overlapped
@@ -792,18 +805,21 @@ int compress_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint8_t *h_src, 
     while (m1 < n) {
       if (src_offsets[m1 + 1] < src_offsets[m1]) return ZB200_ERR_ARG;
       uint64_t len = src_offsets[m1 + 1] - src_offsets[m1];
-      size_t nc = chunks_of(len);
+      size_t nc = rs ? (size_t)rs->count[m1] : chunks_of(len);
       if (nd + nc > nc_cap) return ZB200_ERR_ARG;  // only offsets that decrease further on get here
       if (nd > g.c0 && nd - g.c0 + nc > max_group_chunks) break;
       if (statuses) statuses[m1] = ZB200_OK;
       first[nfirst++] = (uint32_t)(nd - g.c0);
+      const uint64_t *rs_starts = rs ? rs->starts.data() + rs->off[m1] : nullptr;
       for (size_t k = 0; k < nc; k++) {
         ZbChunkDesc &d = desc[nd++];
-        d.src_off = src_offsets[m1] - (h_src ? src_lo : 0) + (uint64_t)k * ZB_CHUNK_BYTES;
-        d.len = (uint32_t)std::min<uint64_t>(ZB_CHUNK_BYTES, len - (uint64_t)k * ZB_CHUNK_BYTES);
+        const uint64_t at = rs ? rs_starts[k] : (uint64_t)k * ZB_CHUNK_BYTES;
+        d.src_off = src_offsets[m1] - (h_src ? src_lo : 0) + at;
+        d.len = (uint32_t)(rs ? (k + 1 < nc ? rs_starts[k + 1] : len) - at
+                              : std::min<uint64_t>(ZB_CHUNK_BYTES, len - at));
         d.member = (uint32_t)(m1 - m0);
         d.flags = (k == 0 ? ZB_CHUNK_FIRST | (head ? ZB_CHUNK_HEAD : 0u) : 0u) | (k == nc - 1 && last ? ZB_CHUNK_LAST : 0u);
-        d.pad = lz ? (uint32_t)std::min<uint64_t>(32768, hist + (uint64_t)k * ZB_CHUNK_BYTES) : 0u;
+        d.pad = lz ? (uint32_t)std::min<uint64_t>(32768, hist + at) : 0u;
         if (dict_hist && k == 0 && ctx->dict_member[m1].win_len) {
           d.pad = ctx->dict_member[m1].win_len;
           d.flags |= ZB_CHUNK_DICT;
@@ -2816,7 +2832,7 @@ void zb200_shutdown(zb200_ctx *ctx) {
   DevBuf *bufs[] = {&ctx->desc, &ctx->member_first, &ctx->fname, &ctx->masks, &ctx->recs, &ctx->hist, &ctx->chk,
                     &ctx->cb, &ctx->chunk_off, &ctx->member_off, &ctx->member_check, &ctx->member_isize,
                     &ctx->src_off, &ctx->dst_off, &ctx->out_len, &ctx->status, &ctx->expect, &ctx->kind,
-                    &ctx->counter, &ctx->cix_rec, &ctx->cix_crc, &ctx->cix_first, &ctx->cix_out, &ctx->ck_out, &ctx->ck_pieces, &ctx->ck_first, &ctx->ck_piece_out, &ctx->ck_partials, &ctx->in_stage, &ctx->out_stage, &ctx->lz2_tables, &ctx->opt_scratch, &ctx->carry,
+                    &ctx->counter, &ctx->cix_rec, &ctx->cix_crc, &ctx->cix_first, &ctx->cix_out, &ctx->ck_out, &ctx->ck_pieces, &ctx->ck_first, &ctx->ck_piece_out, &ctx->ck_partials, &ctx->in_stage, &ctx->out_stage, &ctx->lz2_tables, &ctx->opt_scratch, &ctx->rs_meta, &ctx->rs_tiles, &ctx->rs_counts, &ctx->rs_starts, &ctx->carry,
                     &ctx->seg_src, &ctx->seg_dst, &ctx->seg_len, &ctx->seg_status, &ctx->seg_kind, &ctx->seg_expect, &ctx->seg_cand, &ctx->skip_mask, &ctx->order, &ctx->mark_scratch, &ctx->mark_segs, &ctx->seg_bits, &ctx->mark_win, &ctx->gate,
                     &ctx->idx_desc, &ctx->idx_out, &ctx->dict_win, &ctx->dict_md};
   for (DevBuf *b : bufs)
@@ -3013,6 +3029,166 @@ int zb200_compress_batch_optimal(zb200_ctx *ctx, const uint8_t *src_base, const 
                                  size_t dst_cap, uint64_t *dst_offsets, int *statuses) {
   return compress_batch_host(ctx, src_base, src_offsets, n, 9, data_format, nullptr, nullptr, 0, nullptr, fname_lens,
                              dst_base, dst_cap, dst_offsets, statuses, ZB_STRATEGY_DEFAULT, window_bits, true);
+}
+
+// ---- rsyncable compression (zb_rsync.cu; DESIGN.md section 5 "Rsyncable") ----
+// The chunk map of the members d_src[src_offsets[i], src_offsets[i + 1]) (offsets checked by the caller: they do
+// not decrease), on ctx->stream: the one path behind zb200_rsyncable_chunks and the _rsyncable compress calls.  Two
+// launches, then one copy of the counts and starts back to the host.
+static int rsync_chunks_locked(zb200_ctx *ctx, const uint8_t *d_src, const uint64_t *src_offsets, size_t n,
+                               RsyncMap &map) {
+  if (n > UINT32_MAX) return ZB200_ERR_ARG;
+  std::vector<uint64_t> meta(3 * (n + 1), 0);   // src_off, tile_off, start_off: [n + 1] each
+  uint64_t *src_off = meta.data(), *tile_off = src_off + (n + 1), *start_off = tile_off + (n + 1);
+  for (size_t i = 0; i < n; i++) {
+    const uint64_t len = src_offsets[i + 1] - src_offsets[i];
+    src_off[i] = src_offsets[i];
+    tile_off[i + 1] = tile_off[i] + (len + ZB_RSYNC_MIN - 1) / ZB_RSYNC_MIN;
+    start_off[i + 1] = start_off[i] + zb_rsync_cap(len);
+  }
+  src_off[n] = src_offsets[n];
+  ENSURE(ctx->rs_meta, meta.size() * sizeof(uint64_t));
+  ENSURE(ctx->rs_tiles, (size_t)tile_off[n] * sizeof(uint32_t) + 4);
+  ENSURE(ctx->rs_counts, n * sizeof(uint64_t));
+  ENSURE(ctx->rs_starts, (size_t)start_off[n] * sizeof(uint64_t));
+  cudaStream_t s = ctx->stream;
+  CK(cudaMemcpyAsync(ctx->rs_meta.p, meta.data(), meta.size() * sizeof(uint64_t), cudaMemcpyHostToDevice, s));
+  ZbRsyncWork w;
+  w.src = d_src;
+  w.src_off = (const uint64_t *)ctx->rs_meta.p;
+  w.tile_off = w.src_off + (n + 1);
+  w.start_off = w.tile_off + (n + 1);
+  w.tile_cand = (uint32_t *)ctx->rs_tiles.p;
+  w.counts = (uint64_t *)ctx->rs_counts.p;
+  w.starts = (uint64_t *)ctx->rs_starts.p;
+  w.n = (uint32_t)n;
+  w.n_tiles = tile_off[n];
+  CK(zb_launch_rsync(w, s));
+  ctx->timing.kernel_launches += w.n_tiles ? 2 : 1;
+  map.count.resize(n);
+  map.off.assign(start_off, start_off + n + 1);
+  map.starts.resize(start_off[n]);
+  CK(cudaMemcpyAsync(map.count.data(), w.counts, n * sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(map.starts.data(), w.starts, map.starts.size() * sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  // the plan trusts the map with source ranges: check its shape before any descriptor is built from it
+  for (size_t i = 0; i < n; i++) {
+    const uint64_t len = src_offsets[i + 1] - src_offsets[i], c = map.count[i], *st = map.starts.data() + map.off[i];
+    bool ok = c >= 1 && c <= map.off[i + 1] - map.off[i] && st[0] == 0;
+    for (uint64_t k = 1; ok && k < c; k++) ok = st[k] > st[k - 1] && st[k] - st[k - 1] <= ZB_CHUNK_BYTES;
+    ok = ok && (len == 0 ? c == 1 : st[c - 1] < len && len - st[c - 1] <= ZB_CHUNK_BYTES);
+    if (!ok) {
+      ctx->last_err = "rsyncable chunk map: malformed starts";
+      return ZB200_ERR_CUDA;
+    }
+  }
+  return ZB200_OK;
+}
+
+static int rsync_check_offsets(const uint64_t *src_offsets, size_t n) {
+  for (size_t i = 0; i < n; i++)
+    if (src_offsets[i + 1] < src_offsets[i]) return ZB200_ERR_ARG;
+  return ZB200_OK;
+}
+
+// the batch src_base[src_offsets[0], src_offsets[n]) into in_stage, whole (no copy-in / compress overlap: the chunk
+// map needs every byte first); offs receives the offsets rebased to in_stage
+static int rsync_stage(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n,
+                       std::vector<uint64_t> &offs) {
+  const uint64_t in_bytes = src_offsets[n] - src_offsets[0];
+  ENSURE(ctx->in_stage, (size_t)in_bytes + 64);
+  offs.resize(n + 1);
+  for (size_t i = 0; i <= n; i++) offs[i] = src_offsets[i] - src_offsets[0];
+  const uint8_t *h = src_base + src_offsets[0];
+  return h2d_copy(ctx, (uint8_t *)ctx->in_stage.p, h, (size_t)in_bytes, ctx->stream, is_pageable(h));
+}
+
+size_t zb200_rsyncable_chunks_bound(size_t len) { return (size_t)zb_rsync_cap(len); }
+
+size_t zb200_compress_bound_rsyncable(size_t len, int data_format) {
+  size_t frame = data_format == ZB200_DF_GZIP ? 36 + 8 : data_format == ZB200_DF_ZLIB ? 6 : 0;
+  return len + (size_t)zb_rsync_cap(len) * 10 + 8 + frame;
+}
+
+int zb200_rsyncable_chunks(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n,
+                           uint64_t *counts, uint64_t *starts, size_t starts_cap) {
+  return guarded(ctx, [&]() -> int {
+  if (!ctx || !src_offsets || (n && (!src_base || !counts))) return ZB200_ERR_ARG;
+  if (int rc = rsync_check_offsets(src_offsets, n)) return rc;
+  if (n == 0) return ZB200_OK;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  DeviceGuard g(ctx->device);
+  ctx->timing.kernel_launches = 0;
+  std::vector<uint64_t> offs;
+  RsyncMap map;
+  if (int rc = rsync_stage(ctx, src_base, src_offsets, n, offs)) return rc;
+  if (int rc = rsync_chunks_locked(ctx, (const uint8_t *)ctx->in_stage.p, offs.data(), n, map)) return rc;
+  uint64_t total = 0;
+  for (size_t i = 0; i < n; i++) total += counts[i] = map.count[i];
+  if (total > starts_cap || (total && !starts)) return ZB200_ERR_DST_TOO_SMALL;
+  for (size_t i = 0; i < n; i++) {
+    memcpy(starts, map.starts.data() + map.off[i], (size_t)map.count[i] * sizeof(uint64_t));
+    starts += map.count[i];
+  }
+  return ZB200_OK;
+  });
+}
+
+int zb200_compress_batch_rsyncable(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n,
+                                   int level, int data_format, const uint8_t *fname_lens, uint8_t *dst_base,
+                                   size_t dst_cap, uint64_t *dst_offsets, int *statuses) {
+  return guarded(ctx, [&]() -> int {
+  if (!ctx || !src_offsets || !dst_offsets || (n && (!src_base || !dst_base))) return ZB200_ERR_ARG;
+  if (level < -2 || level > 9) return ZB200_ERR_INVALID_LEVEL;
+  if (data_format != ZB200_DF_GZIP && data_format != ZB200_DF_ZLIB && data_format != ZB200_DF_DEFLATE)
+    return ZB200_ERR_INVALID_FORMAT;
+  if (int rc = rsync_check_offsets(src_offsets, n)) return rc;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  DeviceGuard g(ctx->device);
+  memset(&ctx->timing, 0, sizeof(ctx->timing));
+  dst_offsets[0] = 0;
+  if (n == 0) return ZB200_OK;
+  uint64_t bound = 0;
+  for (size_t i = 0; i < n; i++)
+    bound += zb200_compress_bound_rsyncable((size_t)(src_offsets[i + 1] - src_offsets[i]), data_format) + 64;
+  ENSURE(ctx->out_stage, (size_t)bound + 64);
+  std::vector<uint64_t> offs;
+  RsyncMap map;
+  if (int rc = rsync_stage(ctx, src_base, src_offsets, n, offs)) return rc;
+  if (int rc = rsync_chunks_locked(ctx, (const uint8_t *)ctx->in_stage.p, offs.data(), n, map)) return rc;
+  // the input is on the device already: the plan runs as for device input, with the output copied back per group
+  int rc = compress_locked(ctx, (const uint8_t *)ctx->in_stage.p, nullptr, offs.data(), n, level, data_format,
+                           fname_lens, (uint8_t *)ctx->out_stage.p, ctx->out_stage.cap & ~(size_t)3, dst_base,
+                           dst_cap, dst_offsets, statuses, ctx->host_group_chunks, nullptr, nullptr,
+                           ZB_STRATEGY_DEFAULT, 15, false, &map);
+  if (rc) return rc;
+  ctx->timing.d2h_ms = ev_ms(ctx->ev[8], ctx->ev[9]);
+  ctx->timing.h2d_bytes = src_offsets[n] - src_offsets[0];
+  ctx->timing.d2h_bytes = dst_offsets[n];
+  return ZB200_OK;
+  });
+}
+
+int zb200_compress_batch_device_rsyncable(zb200_ctx *ctx, const uint8_t *d_src, const uint64_t *src_offsets, size_t n,
+                                          int level, int data_format, const uint8_t *fname_lens, uint8_t *d_dst,
+                                          size_t dst_cap, uint64_t *dst_offsets, int *statuses) {
+  return guarded(ctx, [&]() -> int {
+  if (!ctx || !src_offsets || !dst_offsets || (n && (!d_src || !d_dst))) return ZB200_ERR_ARG;
+  if (level < -2 || level > 9) return ZB200_ERR_INVALID_LEVEL;
+  if (data_format != ZB200_DF_GZIP && data_format != ZB200_DF_ZLIB && data_format != ZB200_DF_DEFLATE)
+    return ZB200_ERR_INVALID_FORMAT;
+  if (int rc = rsync_check_offsets(src_offsets, n)) return rc;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  DeviceGuard g(ctx->device);
+  ctx->timing.kernel_launches = 0;
+  dst_offsets[0] = 0;
+  if (n == 0) return ZB200_OK;
+  RsyncMap map;
+  if (int rc = rsync_chunks_locked(ctx, d_src, src_offsets, n, map)) return rc;
+  return compress_locked(ctx, d_src, nullptr, src_offsets, n, level, data_format, fname_lens, d_dst, dst_cap, nullptr,
+                         0, dst_offsets, statuses, ctx->dev_group_chunks, nullptr, nullptr, ZB_STRATEGY_DEFAULT, 15,
+                         false, &map);
+  });
 }
 
 int zb200_compress_batch_dict(zb200_ctx *ctx, const uint8_t *src_base, const uint64_t *src_offsets, size_t n, int level,

@@ -26,6 +26,15 @@
 #define ZB_REC_PIECE_WINDOWS (ZB_REC_PIECE_BYTES / ZB_WINDOW)
 #define ZB_RECS_PER_CHUNK (ZB_WARPS_PER_CHUNK * ZB_RECS_PER_SUB)
 
+// ---- rsyncable compression: the content-defined chunk rule (zb_rsync.cu, DESIGN.md section 5 "Rsyncable") ----
+// A format promise: members written under these values must keep their chunk starts, so they never change silently.
+#define ZB_RSYNC_MIN 16384        // an accepted cut has no other candidate in the MIN bytes before it
+#define ZB_RSYNC_BITS 16          // p is a candidate when the top BITS bits of its gear hash are zero
+// most chunks of a member of len bytes: ceil(len / 64 KiB) + floor(len / MIN), and the one empty chunk of len 0
+ZB_HD uint64_t zb_rsync_cap(uint64_t len) {
+  return len == 0 ? 1 : (len + ZB_CHUNK_BYTES - 1) / ZB_CHUNK_BYTES + len / ZB_RSYNC_MIN;
+}
+
 #define ZB_NUM_LITLEN 286
 #define ZB_NUM_DIST 30
 #define ZB_HIST_SYMS (ZB_NUM_LITLEN + ZB_NUM_DIST)  // 316

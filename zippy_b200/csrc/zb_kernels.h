@@ -109,6 +109,21 @@ cudaError_t zb_launch_huff(const ZbCompressWork &w, cudaStream_t s);
 size_t zb_opt_scratch_bytes(int *grid_out);
 cudaError_t zb_setup_opt_attrs();
 cudaError_t zb_launch_opt(const ZbCompressWork &w, cudaStream_t s);
+// rsyncable chunk map (zb_rsync.cu): member i is src[src_off[i], src_off[i + 1]); it is cut into tiles of
+// ZB_RSYNC_MIN bytes, tiles tile_off[i] .. tile_off[i + 1] - 1 of the batch.  k_rsync_cand writes each tile's first
+// and last gear-hash candidate into tile_cand; k_rsync_starts turns them into the member's chunk starts (member
+// positions, ascending, the first 0) at starts + start_off[i] (start_off: prefix sums of zb_rsync_cap) and their
+// number at counts[i].  Every array is device memory.
+struct ZbRsyncWork {
+  const uint8_t *src;
+  const uint64_t *src_off, *tile_off, *start_off;   // [n + 1]
+  uint32_t *tile_cand;                              // [n_tiles]
+  uint64_t *counts;                                 // [n]
+  uint64_t *starts;                                 // [start_off[n]]
+  uint32_t n;
+  uint64_t n_tiles;
+};
+cudaError_t zb_launch_rsync(const ZbRsyncWork &w, cudaStream_t s);
 cudaError_t zb_launch_scan(const ZbCompressWork &w, cudaStream_t s);
 cudaError_t zb_launch_pack(const ZbCompressWork &w, cudaStream_t s);
 // A compress-time index (k_index_rec, after k_scan): the access-point records of zb200_index_build's recorder
